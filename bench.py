@@ -41,7 +41,7 @@ sys.path.insert(0, str(ROOT))
 METRIC = "rendered views/sec fwd+bwd @256x256, 3 gauss/px"
 WORKLOAD = ("configs[1]: re10k-like 2-view -> 1 target, 256x256, 3 gauss/px, batch 1, rasterizer fwd+bwd "
             "(SH degree 4)")          # the SAME string in both arms (driver's same_config check)
-ISSUE_PEAK = 148 * 4 * 1.965e9        # warp instructions / s: SMs x schedulers x max SM clock
+ISSUE_PEAK = 132 * 4 * 1.98e9         # warp instructions / s: H100 SXM SMs x schedulers x max SM clock
 UNIT = "views/s"
 IMAGE = (256, 256)
 STAGES = ["preprocess", "count_scan_scatter", "tile_sort", "composite_fwd", "grad_zero_fill",
@@ -51,8 +51,8 @@ STAGES = ["preprocess", "count_scan_scatter", "tile_sort", "composite_fwd", "gra
 def peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
-        return json.loads(p.read_text()), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0}, "fallback"
+        return json.loads(p.read_text()), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet (no MEASURED_PEAKS.json)"
 
 
 def csrc_sha() -> str:
@@ -226,10 +226,32 @@ def build_roofline(stage_ms: dict, V: int, P: int, N: float, vis: float, HW: int
                     "algorithmic bytes (no re-reads) and what bounds it is instruction issue, so `frac` (HBM) is "
                     "small by construction and `issue_frac` (warp instructions / s over SMs x 4 x clock) is the "
                     "roofline that moves; see profiles/README.md",
-            "peak_source": f"{pk_kind} (MEASURED_PEAKS.json hbm_gbs, burst copy)",
+            "peak_source": pk_kind,
             "algorithmic_bytes_per_launch": V * ab[dom], "avg_launch_ms": stage_ms[dom],
             "pair_evals_per_s": (V * N * 256 / (stage_ms[dom] * 1e-3) if dom.startswith("composite") else None),
             "all_stages_gbs": {s: V * ab[s] / (stage_ms[s] * 1e-3) / 1e9 for s in STAGES if stage_ms[s] > 0}}
+
+
+DUMP_ROWS = 65536      # Gaussians sampled for the per-Gaussian gradients (harmonics alone are 118 MB at P = 393 216)
+
+
+def sample_outputs(img, grads) -> dict:
+    """What one timed step returns to its caller -- the rendered image and the gradients of means, covariances,
+    harmonics and opacities -- copied on the device.  Per-Gaussian gradients are restricted to a fixed, seeded
+    sample of Gaussians (its indices are kept too), which keeps the dump a few tens of MB."""
+    P = grads[0].shape[1]
+    idx = torch.randperm(P, generator=torch.Generator().manual_seed(0))[:min(DUMP_ROWS, P)].sort().values
+    out = {"image": img.detach().clone(), "gaussian_index": idx.to(torch.float64)}
+    for k, gr in zip(GAUSS_KEYS, grads):
+        out[f"grad_{k}"] = gr[:, idx.to(gr.device)]
+    return out
+
+
+def write_outputs(out_dir: Path, arrays: dict):
+    import numpy as np
+    out_dir.mkdir(parents=True, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(out_dir / f"{name}.npy", a.cpu().numpy().astype(np.float64 if a.dtype == torch.float64 else np.float32))
 
 
 def cpu_threads() -> int:
@@ -322,6 +344,8 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="issue every step from Python instead of replaying a CUDA graph")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the image and gradients of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     global IMAGE, CONTEXT_VIEWS
     IMAGE, CONTEXT_VIEWS = (args.image, args.image), args.context_views
@@ -333,6 +357,8 @@ def main():
             args.steps, args.warmup = 2, 1
         run_reference(args, rank, world)
         return
+    if args.steps < 1:
+        raise SystemExit("--steps must be at least 1")
     if args.warmup < 3:
         args.warmup = 3
     if not torch.cuda.is_available():
@@ -385,13 +411,15 @@ def main():
     barrier()
     launches0 = _lib.lib.ps_launch_count()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    last = {}
     def run_steps(n):
         if graphs is not None:
             for i in range(n):
                 graphs[i % args.pool][0].replay()
+            last["out"] = graphs[(n - 1) % args.pool][1]
         else:
             for i in range(n):
-                render_step(pool_dev[i % args.pool], d_img, V)
+                last["out"] = render_step(pool_dev[i % args.pool], d_img, V)
 
     with ClockSampler(local_rank) as clk:
         barrier()
@@ -402,6 +430,7 @@ def main():
         barrier()
         t_end = time.monotonic()
         launches_timed = _lib.lib.ps_launch_count() - launches0
+        dumped = sample_outputs(*last["out"]) if (args.dump_outputs and rank == 0) else None
         clock_window = "timed region"
         if clk.proc is not None and clk.count_between(t_begin, t_end) < 3:
             # the timed region is shorter than a few nvidia-smi sampling periods: keep the SAME load running,
@@ -599,6 +628,8 @@ def main():
             "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches),
             "roofline": roofline, "cpu_baseline": cpu, "stage_ms": stage_ms, "workload_stats": stats, "throughput_concurrent_streams": concurrent, "throughput_batched_views": batched,
         }
+        if dumped is not None:
+            write_outputs(Path(args.dump_outputs), dumped)
         emit(line)
     if world > 1:
         dist.destroy_process_group()

@@ -1,5 +1,5 @@
 /*
- * pixelsplat_b200.h -- C ABI of the B200-native render hot path of pixelSplat.
+ * pixelsplat_b200.h -- C ABI of the native (H100, sm_90a) render hot path of pixelSplat.
  *
  * Drop-in boundary (SURVEY.md section 8b).  The reference binds its rasterizer through the
  * Python extension `diff_gaussian_rasterization` (imported at
@@ -288,7 +288,7 @@ PS_API int ps_epipolar_attention_backward(const ps_epipolar_desc *desc, const ps
                                           const float *dmass, const float *d_row, float *dq_feat,
                                           float *dq_pe, float *dbias, float *dfeatures, void *stream);
 
-/* ---- dense per-image self-attention (tcgen05, TF32 operands, FP32 accumulate) ---------------------
+/* ---- dense per-image self-attention (wgmma, TF32 operands, FP32 accumulate) -----------------------
  * Replaces the z = None branch of /root/reference/src/model/transformer/attention.py:54-70 as used by
  * ImageSelfAttention (/root/reference/src/model/encoder/epipolar/image_self_attention.py:57-79):
  *   qkv  [n_images, tokens, 3 * heads * dim_head]   output of to_qkv ("b n (qkv h d)")
@@ -305,7 +305,7 @@ PS_API int ps_self_attention_forward(int32_t n_images, int32_t tokens, int32_t h
 PS_API int ps_self_attention_forward_stats(int32_t n_images, int32_t tokens, int32_t heads, int32_t dim_head,
                                            const float *qkv, float scale, float *out, float *stats, void *stream);
 
-/* Backward (tcgen05, TF32 operands, FP32 accumulate; csrc/self_attention_tc_bwd.cu): autograd of the forward
+/* Backward (wgmma, TF32 operands, FP32 accumulate; csrc/self_attention_tc_bwd.cu): autograd of the forward
  * above.  out / d_out [n_images, 256, heads * 128]; d_qkv has qkv's layout and is fully written. */
 PS_API int ps_self_attention_backward(int32_t n_images, int32_t tokens, int32_t heads, int32_t dim_head,
                                       const float *qkv, const float *out, const float *d_out, const float *stats,

@@ -107,7 +107,7 @@ class NativeLibraryMissing(ImportError):
 def _load() -> ctypes.CDLL:
     if not LIB_PATH.exists():
         raise NativeLibraryMissing(
-            f"{LIB_PATH} not found: the sm_100a CUDA library is not built. Run "
+            f"{LIB_PATH} not found: the sm_90a CUDA library is not built. Run "
             f"`make -C {_PKG / 'csrc'}` (or __graft_entry__.build()). There is no CPU fallback.")
     lib = ctypes.CDLL(str(LIB_PATH))
     lib.ps_version.restype = ctypes.c_int

@@ -1,4 +1,4 @@
-// Shared declarations of the rasterizer kernels (sm_100a only).
+// Shared declarations of the rasterizer kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -162,8 +162,7 @@ __device__ void bitonic_sort_smem(unsigned long long *s_keys, int n_pad) {
 //     through HBM.  Always correct, just slower.
 // 16 warps each own a contiguous ~n/16-key slice, so a pass is two short warp loops (count with
 // fire-and-forget shared atomics, stable rank with match.any) around one column scan: the sort is
-// bound by shared-memory latency chains, and short slices are what keeps those chains short
-// (8 warps x 11-bit digits: 32 us for 256 tiles of ~1.6k keys; see profiles/).
+// bound by shared-memory latency chains, and short slices are what keeps those chains short.
 constexpr int kSortThreads = 512;   // 64 regs x 512 threads: two CTAs per SM
 constexpr int kSortWarps = kSortThreads / 32;
 

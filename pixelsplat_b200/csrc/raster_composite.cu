@@ -4,7 +4,7 @@
 // One CTA per (view, 16x16 tile); each warp owns an 8x4 pixel sub-rectangle, each lane a pixel.
 // The tile's sorted instance list is staged 256 entries at a time in shared memory.
 //
-// B200-first differences from upstream's renderCUDA (SURVEY.md A.3 / A.5), none of which
+// Differences from upstream's renderCUDA (SURVEY.md A.3 / A.5), none of which
 // change a per-pixel decision:
 //   * warp-level culling: for every staged Gaussian one lane tests the axis-aligned bound of
 //     the region where alpha >= 1/255 can hold (|d| <= sqrt(2 ln(255 o) Sigma_ii)) against the
@@ -167,7 +167,7 @@ k_composite_fwd(Dims d, Geom geo, const float *__restrict__ bg_all,
                 uint32_t mask = __ballot_sync(0xffffffffu, hit);
                 // four entries per iteration: their power / exp evaluations are independent, only
                 // the transmittance update chains (the warp has few peers to hide latency behind:
-                // a 256x256 view is just 2048 warps on 148 SMs).  (Carrying partial groups across
+                // a 256x256 view is just 2048 warps on 132 SMs).  (Carrying partial groups across
                 // chunks as the backward does costs the forward more in bookkeeping than it saves.)
                 while (mask) {
                     uint32_t jx[4];
@@ -274,7 +274,7 @@ struct PixelState {
 
 // Straight-line (predicated, no divergent branches): on average only ~10 of a warp's 32 pixels
 // take a given entry, but the warp executes the whole body anyway, and the reconvergence
-// bookkeeping of a branchy version was 13 % of the issued instructions (profiles/r01_*).
+// bookkeeping of a branchy version costs issued instructions of its own.
 __device__ __forceinline__ bool pixel_bwd(bool in_range, const float2 exy, const float4 eco, const float4 ergb,
                                           float px, float py, float dpr, float dpg, float dpb, float T_final,
                                           float bg_dot, float ddelx_dx, float ddely_dy, PixelState &st,
@@ -313,13 +313,18 @@ __device__ __forceinline__ bool pixel_bwd(bool in_range, const float2 exy, const
     return active;
 }
 
-// Two list entries at once with Blackwell's packed FP32x2 arithmetic (FADD2 / FMUL2 / FFMA2,
-// sm_100 only: one issue slot, two results).  Everything that is element-wise per entry -- the
-// quadratic form, alpha, the gradient terms -- is evaluated on (entry a, entry b) register pairs;
-// the short per-pixel recurrences (T, colour behind) stay scalar and run a then b, exactly as the
-// list order demands.  The composite backward is issue-bound (63 % issue-active at 14 warps/SM,
-// profiles/r01_ncu_metrics_v10.csv), so instructions saved are time saved.
+// Two list entries at once.  Everything that is element-wise per entry -- the quadratic form,
+// alpha, the gradient terms -- is evaluated on (entry a, entry b) register pairs; the short
+// per-pixel recurrences (T, colour behind) stay scalar and run a then b, exactly as the list
+// order demands.  sm_90 has no packed FP32x2 arithmetic, so each pair operation is two scalar
+// round-to-nearest operations that the compiler may not contract (the same roundings as packed
+// FADD2 / FMUL2 / FFMA2), and the pairing gives the scheduler two independent chains.
 __device__ __forceinline__ float2 pk(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
 
 __device__ __forceinline__ void pixel_bwd_pair(bool in_a, bool in_b, const float2 xya, const float2 xyb,
                                                const float4 coa, const float4 cob, const float4 ca,
@@ -327,21 +332,21 @@ __device__ __forceinline__ void pixel_bwd_pair(bool in_a, bool in_b, const float
                                                float dpb, float T_final, float bg_dot, float kx, float ky,
                                                PixelState &st, float *ga, float *gb, float &opa, float &opb,
                                                bool &act_a, bool &act_b) {
-    const float2 DX = __fadd2_rn(pk(xya.x, xyb.x), pk(-px, -px));
-    const float2 DY = __fadd2_rn(pk(xya.y, xyb.y), pk(-py, -py));
+    const float2 DX = add2(pk(xya.x, xyb.x), pk(-px, -px));
+    const float2 DY = add2(pk(xya.y, xyb.y), pk(-py, -py));
     const float2 QA = pk(coa.x, cob.x), QB = pk(coa.y, cob.y), QC = pk(coa.z, cob.z), W = pk(coa.w, cob.w);
-    float2 P = __fmul2_rn(__fmul2_rn(QA, DX), DX);
-    P = __ffma2_rn(__fmul2_rn(QC, DY), DY, P);
-    P = __ffma2_rn(__fmul2_rn(QB, DX), DY, P);                       // power * log2(e), both entries
+    float2 P = mul2(mul2(QA, DX), DX);
+    P = fma2(mul2(QC, DY), DY, P);
+    P = fma2(mul2(QB, DX), DY, P);                       // power * log2(e), both entries
     const float2 G = pk(fast_exp2(P.x), fast_exp2(P.y));
-    const float2 AL = __fmul2_rn(W, G);
+    const float2 AL = mul2(W, G);
     const float al_a = fminf(0.99f, AL.x), al_b = fminf(0.99f, AL.y);
     act_a = in_a && !(P.x > 0.0f) && !(al_a < kAlphaMin);
     act_b = in_b && !(P.y > 0.0f) && !(al_b < kAlphaMin);
     // skipped entries behave like alpha = 0, G = 0 (see pixel_bwd)
     const float2 A = pk(act_a ? al_a : 0.0f, act_b ? al_b : 0.0f);
     const float2 GS = pk(act_a ? G.x : 0.0f, act_b ? G.y : 0.0f);
-    const float2 OM = __fadd2_rn(pk(1.0f, 1.0f), pk(-A.x, -A.y));
+    const float2 OM = add2(pk(1.0f, 1.0f), pk(-A.x, -A.y));
     const float rcp_a = __fdividef(1.0f, OM.x), rcp_b = __fdividef(1.0f, OM.y);
     // ---- entry a, then entry b: transmittance and colour-behind recurrences (scalar / channel-packed)
     const float Ta = st.T * rcp_a;
@@ -349,21 +354,21 @@ __device__ __forceinline__ void pixel_bwd_pair(bool in_a, bool in_b, const float
     float acc_b_ = st.acc_b;
     {
         const float la = st.last_alpha;
-        acc_rg = __ffma2_rn(pk(la, la), __fadd2_rn(pk(st.lc_r, st.lc_g), pk(-acc_rg.x, -acc_rg.y)), acc_rg);
+        acc_rg = fma2(pk(la, la), add2(pk(st.lc_r, st.lc_g), pk(-acc_rg.x, -acc_rg.y)), acc_rg);
         acc_b_ = acc_b_ + la * (st.lc_b - acc_b_);
     }
-    const float2 da_rg = __fadd2_rn(pk(ca.x, ca.y), pk(-acc_rg.x, -acc_rg.y));
-    const float2 ta_rg = __fmul2_rn(da_rg, pk(dpr, dpg));
+    const float2 da_rg = add2(pk(ca.x, ca.y), pk(-acc_rg.x, -acc_rg.y));
+    const float2 ta_rg = mul2(da_rg, pk(dpr, dpg));
     float dLa = ta_rg.x + ta_rg.y + (ca.z - acc_b_) * dpb;
     dLa = dLa * Ta - T_final * rcp_a * bg_dot;
     const float Tb = Ta * rcp_b;
     {
         const float la = A.x;
-        acc_rg = __ffma2_rn(pk(la, la), __fadd2_rn(pk(ca.x, ca.y), pk(-acc_rg.x, -acc_rg.y)), acc_rg);
+        acc_rg = fma2(pk(la, la), add2(pk(ca.x, ca.y), pk(-acc_rg.x, -acc_rg.y)), acc_rg);
         acc_b_ = acc_b_ + la * (ca.z - acc_b_);
     }
-    const float2 db_rg = __fadd2_rn(pk(cb.x, cb.y), pk(-acc_rg.x, -acc_rg.y));
-    const float2 tb_rg = __fmul2_rn(db_rg, pk(dpr, dpg));
+    const float2 db_rg = add2(pk(cb.x, cb.y), pk(-acc_rg.x, -acc_rg.y));
+    const float2 tb_rg = mul2(db_rg, pk(dpr, dpg));
     float dLb = tb_rg.x + tb_rg.y + (cb.z - acc_b_) * dpb;
     dLb = dLb * Tb - T_final * rcp_b * bg_dot;
     st.T = Tb;
@@ -372,17 +377,17 @@ __device__ __forceinline__ void pixel_bwd_pair(bool in_a, bool in_b, const float
     st.last_alpha = A.y;
     // ---- gradient terms, packed across the two entries
     const float2 DL = pk(dLa, dLb);
-    const float2 WC = __fmul2_rn(A, pk(Ta, Tb));                     // alpha * T
-    const float2 CR = __fmul2_rn(WC, pk(dpr, dpr)), CG = __fmul2_rn(WC, pk(dpg, dpg)), CB = __fmul2_rn(WC, pk(dpb, dpb));
-    const float2 WG = __fmul2_rn(__fmul2_rn(W, DL), GS);             // dL/dG * G
-    const float2 SX = __fmul2_rn(WG, DX), SY = __fmul2_rn(WG, DY);
+    const float2 WC = mul2(A, pk(Ta, Tb));                     // alpha * T
+    const float2 CR = mul2(WC, pk(dpr, dpr)), CG = mul2(WC, pk(dpg, dpg)), CB = mul2(WC, pk(dpb, dpb));
+    const float2 WG = mul2(mul2(W, DL), GS);             // dL/dG * G
+    const float2 SX = mul2(WG, DX), SY = mul2(WG, DY);
     const float2 two = pk(2.0f, 2.0f);
-    const float2 MX = __fmul2_rn(pk(kx, kx), __ffma2_rn(__fmul2_rn(two, QA), SX, __fmul2_rn(QB, SY)));
-    const float2 MY = __fmul2_rn(pk(ky, ky), __ffma2_rn(__fmul2_rn(two, QC), SY, __fmul2_rn(QB, SX)));
+    const float2 MX = mul2(pk(kx, kx), fma2(mul2(two, QA), SX, mul2(QB, SY)));
+    const float2 MY = mul2(pk(ky, ky), fma2(mul2(two, QC), SY, mul2(QB, SX)));
     const float2 mh = pk(-0.5f, -0.5f);
-    const float2 HX = __fmul2_rn(mh, SX), HY = __fmul2_rn(mh, SY);
-    const float2 CA = __fmul2_rn(HX, DX), CBc = __fmul2_rn(HX, DY), CC = __fmul2_rn(HY, DY);
-    const float2 OP = __fmul2_rn(GS, DL);
+    const float2 HX = mul2(mh, SX), HY = mul2(mh, SY);
+    const float2 CA = mul2(HX, DX), CBc = mul2(HX, DY), CC = mul2(HY, DY);
+    const float2 OP = mul2(GS, DL);
     ga[0] = MX.x; ga[1] = MY.x; ga[2] = CA.x; ga[3] = CBc.x; ga[4] = CC.x; ga[5] = CR.x; ga[6] = CG.x; ga[7] = CB.x;
     gb[0] = MX.y; gb[1] = MY.y; gb[2] = CA.y; gb[3] = CBc.y; gb[4] = CC.y; gb[5] = CR.y; gb[6] = CG.y; gb[7] = CB.y;
     opa = OP.x; opb = OP.y;

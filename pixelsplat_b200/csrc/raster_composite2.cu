@@ -682,7 +682,7 @@ int launch_composite_backward(const Dims &d, const Inputs &in, const Geom &g, co
     }
 }
 
-// Runs per task for a batch of `tasks` warp tasks: enough warps to fill the machine (148 SMs x ~24 resident
+// Runs per task for a batch of `tasks` warp tasks: enough warps to fill the machine (132 SMs x ~24 resident
 // warps), none when the batch already does.  PIXELSPLAT_B200_SEGMENTS = 1 | 2 | 4 overrides (A/B runs).
 int composite_segments(long long tasks) {
     if (g_segments < 0) {

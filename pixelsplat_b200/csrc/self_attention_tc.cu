@@ -1,26 +1,20 @@
-// Dense per-image multi-head self-attention on the 5th-generation tensor cores (tcgen05, TF32):
+// Dense per-image multi-head self-attention on the Hopper tensor cores (wgmma, TF32):
 //     out[img, :, head] = softmax(Q K^T * scale) V      Q, K, V: [256 tokens, 128] per (image, head)
-// for the ViT blocks of pixelSplat's ImageSelfAttention
-// (/root/reference/src/model/encoder/epipolar/image_self_attention.py:57-79 ->
-//  /root/reference/src/model/transformer/attention.py:54-70 with z = None): the only dense
+// for the ViT blocks of pixelSplat's ImageSelfAttention (reference: src/model/encoder/epipolar/
+// image_self_attention.py:57-79 -> src/model/transformer/attention.py:54-70 with z = None): the only dense
 // contractions of the hot path (SURVEY.md 8 row a14).
 //
-// One CTA (8 warps) per (image, head, 128-query half):
+// One CTA (two warpgroups) per (image, head, 128-query half); warpgroup w owns queries 64 w .. 64 w + 63:
 //   1. Q half [128 x 128] and K [256 x 128] are copied (fp32 rounded to the nearest TF32) into shared
-//      memory in the canonical K-major no-swizzle UMMA layout (8-row x 16-byte core matrices);
-//   2. one elected thread issues 16 tcgen05.mma (M=128, N=256, K=8) accumulating S = Q K^T in TMEM
-//      (256 columns), commits to an mbarrier;
-//   3. warps 0-3, soft-max in place: thread i owns query row i = TMEM lane i; tcgen05.ld 32 columns
-//      at a time, row max, exp2, round to TF32, row sum, tcgen05.st the un-normalised probabilities
-//      back over S;  warps 4-7, concurrently: K's shared buffer is overwritten with V^T (d-major x
-//      tokens, same K-major layout);
-//   4. 32 tcgen05.mma (M=128, N=128, K=8) with A = P read straight from TMEM and B = V^T from
-//      shared memory accumulate O in TMEM columns 256..383;
-//   5. epilogue, all 8 warps (lane quarter x 64 channels each): tcgen05.ld O, scale by 1 / row sum,
-//      16-byte stores to global.
-// No TMA: the tiles are tiny and L2-resident (112 CTAs x 320 KB); the copy is plain ld.global /
-// st.shared followed by a proxy fence.
-#include "umma_tf32.cuh"
+//      memory in the canonical K-major no-swizzle layout (8-row x 16-byte core matrices);
+//   2. each warpgroup issues 16 wgmma m64n256k8 accumulating its S = Q K^T rows in registers (128 per thread);
+//   3. K's shared buffer is overwritten with V^T (d-major x tokens, same K-major layout); each thread turns
+//      its two rows' S into un-normalised probabilities in place (row max and sum over the four threads that
+//      share a row), rounded to TF32;
+//   4. 32 wgmma m64n128k8 with A = P straight from those registers and B = V^T from shared memory accumulate O;
+//   5. epilogue: scale by 1 / row sum, store.
+// No TMA: the tiles are tiny and L2-resident; the copy is plain ld.global / st.shared followed by a proxy fence.
+#include "wgmma_tf32.cuh"
 
 namespace ps {
 
@@ -32,174 +26,104 @@ k_self_attention_tc(const float *__restrict__ qkv, float *__restrict__ out, floa
     extern __shared__ __align__(128) unsigned char s_sa[];
     unsigned char *sQ = s_sa;                                                      // 128 x 128 fp32 = 64 KB
     unsigned char *sK = s_sa + 64 * 1024;                                          // 256 x 128 fp32 = 128 KB (later V^T)
-    uint64_t *bar = reinterpret_cast<uint64_t *>(s_sa + 192 * 1024);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(s_sa + 192 * 1024 + 16);
-    float *s_inv = reinterpret_cast<float *>(s_sa + 192 * 1024 + 64);              // 1 / row sum, 128 rows
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+    const int t = lane & 3;
+    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);                       // first of this thread's rows (+8)
     const int half = blockIdx.x, head = blockIdx.y, img = blockIdx.z;
     const int inner = n_heads * kSaD;
     const size_t row_stride = 3 * (size_t)inner;                                   // floats per token in qkv
     const float *q_base = qkv + ((size_t)img * kSaL + (size_t)half * 128) * row_stride + (size_t)head * kSaD;
     const float *k_base = qkv + (size_t)img * kSaL * row_stride + inner + (size_t)head * kSaD;
     const float *v_base = qkv + (size_t)img * kSaL * row_stride + 2 * inner + (size_t)head * kSaD;
-
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     :: "r"(smem_u32(tmem_slot)), "n"(kSaTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(smem_u32(bar)) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    // ---- stage Q (128 rows) and K (256 rows): consecutive threads take consecutive rows of the same
-    // 16-byte chunk, so the shared stores are contiguous (chunk c of row r lives at c * LBO + r * 16);
-    // eight independent 16-byte loads are in flight per thread before the first is consumed.
     constexpr uint32_t kLboQ = 128 * 16, kLboK = 256 * 16, kLboV = 128 * 16;       // bytes between K chunks
-    constexpr int kBatch = 8;
-#pragma unroll 1
-    for (int i0 = tid; i0 < 128 * 32; i0 += kSaThreads * kBatch) {
-        float4 v[kBatch];
-#pragma unroll
-        for (int j = 0; j < kBatch; ++j) {
-            const int i = i0 + j * kSaThreads;
-            v[j] = __ldg(reinterpret_cast<const float4 *>(q_base + (size_t)(i & 127) * row_stride) + (i >> 7));
-        }
-#pragma unroll
-        for (int j = 0; j < kBatch; ++j) {
-            const int i = i0 + j * kSaThreads;
-            *reinterpret_cast<float4 *>(sQ + (size_t)(i >> 7) * kLboQ + (i & 127) * 16) = to_tf32(v[j]);
-        }
-    }
-#pragma unroll 1
-    for (int i0 = tid; i0 < 256 * 32; i0 += kSaThreads * kBatch) {
-        float4 v[kBatch];
-#pragma unroll
-        for (int j = 0; j < kBatch; ++j) {
-            const int i = i0 + j * kSaThreads;
-            v[j] = __ldg(reinterpret_cast<const float4 *>(k_base + (size_t)(i & 255) * row_stride) + (i >> 8));
-        }
-#pragma unroll
-        for (int j = 0; j < kBatch; ++j) {
-            const int i = i0 + j * kSaThreads;
-            *reinterpret_cast<float4 *>(sK + (size_t)(i >> 8) * kLboK + (i & 255) * 16) = to_tf32(v[j]);
-        }
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");                  // generic -> async proxy
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = *tmem_slot;                                              // lane 0, column base
-    const uint32_t tmem_S = tmem, tmem_O = tmem + 256;
-    const uint32_t lane_addr = (uint32_t)((warp & 3) * 32) << 16;                  // this warp's TMEM lane quarter
-    const int row = (warp & 3) * 32 + lane;                                        // query row inside the half
 
-    // ---- S = Q K^T
-    if (tid == 0) {
-        const uint32_t idesc = umma_idesc_tf32(128, 256);
-#pragma unroll 1
-        for (int k = 0; k < kSaD / 8; ++k) {
-            const uint64_t a = umma_desc(smem_u32(sQ) + k * 2 * kLboQ, kLboQ, 128);
-            const uint64_t b = umma_desc(smem_u32(sK) + k * 2 * kLboK, kLboK, 128);
-            mma_tf32_ss(tmem_S, a, b, idesc, k > 0);
-        }
-        umma_commit(smem_u32(bar));
-    }
-    mbar_wait(smem_u32(bar), 0);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (debug_mode == 1) {
-        if (warp < 4) {
-            float *dst = out + ((((size_t)img * n_heads + head) * 2 + half) * 128 + row) * 256;
-            for (int c = 0; c < 256; c += 32) {
-                float v[32];
-                tmem_ld32(tmem_S + lane_addr + c, v);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) dst[c + i] = v[i];
-            }
-        }
-    } else {
-        if (warp >= 4) {
-            // ---- warps 4-7: V^T into K's buffer (K is dead: the MMAs that read it have completed);
-            // one 16-byte chunk = 4 consecutive tokens of one channel, 16 scalar loads in flight
-            const int t4 = tid - 128;
-#pragma unroll 1
-            for (int i0 = t4; i0 < 128 * 64; i0 += 128 * 4) {
-                float4 v[4];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int i = i0 + j * 128;
-                    const float *src = v_base + (size_t)(4 * (i >> 7)) * row_stride + (i & 127);
-                    v[j].x = __ldg(src);
-                    v[j].y = __ldg(src + row_stride);
-                    v[j].z = __ldg(src + 2 * row_stride);
-                    v[j].w = __ldg(src + 3 * row_stride);
-                }
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    const int i = i0 + j * 128;
-                    *reinterpret_cast<float4 *>(sK + (size_t)(i >> 7) * kLboV + (i & 127) * 16) = to_tf32(v[j]);
-                }
-            }
-        } else {
-            // ---- warps 0-3: soft-max over the 256 keys of this thread's row, in place in TMEM
-            float m = -INFINITY;
-            for (int c = 0; c < 256; c += 32) {
-                float v[32];
-                tmem_ld32(tmem_S + lane_addr + c, v);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) m = fmaxf(m, v[i]);
-            }
-            float sum = 0.0f;
-            const float mb = m * scale_log2e;
-            for (int c = 0; c < 256; c += 32) {
-                float v[32];
-                tmem_ld32(tmem_S + lane_addr + c, v);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    v[i] = to_tf32(exp2f(v[i] * scale_log2e - mb));   // the row sum is over what the MMA will see
-                    sum += v[i];
-                }
-                tmem_st32(tmem_S + lane_addr + c, v);
-            }
-            s_inv[row] = 1.0f / sum;
-            if (stats) {   // what the backward needs to rebuild exactly these probabilities: (max * scale * log2 e, 1 / sum)
-                float2 *st = reinterpret_cast<float2 *>(stats) + ((size_t)img * n_heads + head) * kSaL + half * 128 + row;
-                *st = make_float2(mb, 1.0f / sum);
-            }
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        // ---- O = P V   (A = P from TMEM, B = V^T from shared memory)
-        if (tid == 0) {
-            const uint32_t idesc = umma_idesc_tf32(128, 128);
-#pragma unroll 1
-            for (int k = 0; k < kSaL / 8; ++k) {
-                const uint64_t b = umma_desc(smem_u32(sK) + k * 2 * kLboV, kLboV, 128);
-                mma_tf32_ts(tmem_O, tmem_S + k * 8, b, idesc, k > 0);
-            }
-            umma_commit(smem_u32(bar));
-        }
-        mbar_wait(smem_u32(bar), 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        // ---- epilogue: every warp takes its lane quarter x 64 of the 128 output channels
-        const float inv = s_inv[row];
-        const int c0 = (warp >> 2) * 64;
-        float *dst = out + ((size_t)img * kSaL + (size_t)half * 128 + row) * inner + (size_t)head * kSaD + c0;
-        for (int c = 0; c < 64; c += 32) {
-            float v[32];
-            tmem_ld32(tmem_O + lane_addr + c0 + c, v);
-#pragma unroll
-            for (int i = 0; i < 32; i += 4)
-                *reinterpret_cast<float4 *>(dst + c + i) = make_float4(v[i] * inv, v[i + 1] * inv, v[i + 2] * inv, v[i + 3] * inv);
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    stage_natural<128>(sQ, q_base, row_stride, tid, kSaThreads);
+    stage_natural<256>(sK, k_base, row_stride, tid, kSaThreads);
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");                  // generic -> async proxy
     __syncthreads();
-    if (warp == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem), "n"(kSaTmemCols) : "memory");
+
+    // ---- S = Q K^T, this warpgroup's 64 rows
+    float s[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) s[i] = 0.0f;
+    wgmma_fence();
+#pragma unroll 1
+    for (int k = 0; k < kSaD / 8; ++k)
+        wgmma_ss_n256(s, gmma_desc(smem_u32(sQ) + k * 2 * kLboQ + wg * 64 * 16, kLboQ, 128),
+                      gmma_desc(smem_u32(sK) + k * 2 * kLboK, kLboK, 128), k > 0);
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_operands(s);
+    if (debug_mode == 1) {
+        float *dst = out + ((((size_t)img * n_heads + head) * 2 + half) * 128 + row) * 256 + 2 * t;
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+            *reinterpret_cast<float2 *>(dst + 8 * j) = make_float2(s[4 * j], s[4 * j + 1]);
+            *reinterpret_cast<float2 *>(dst + 8 * 256 + 8 * j) = make_float2(s[4 * j + 2], s[4 * j + 3]);
+        }
+        return;
+    }
+    __syncthreads();                                   // both warpgroups' MMAs have completed: K is dead
+    stage_transposed<256>(sK, v_base, row_stride, tid, kSaThreads);
+
+    // ---- soft-max over the 256 keys of rows `row` (s[4 j], s[4 j + 1]) and `row + 8` (s[4 j + 2 / 3])
+    float m0 = -INFINITY, m1 = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+        m0 = fmaxf(m0, fmaxf(s[4 * j], s[4 * j + 1]));
+        m1 = fmaxf(m1, fmaxf(s[4 * j + 2], s[4 * j + 3]));
+    }
+#pragma unroll
+    for (int o = 1; o < 4; o <<= 1) {
+        m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, o));
+        m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, o));
+    }
+    const float mb0 = m0 * scale_log2e, mb1 = m1 * scale_log2e;
+    float sum0 = 0.0f, sum1 = 0.0f;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+        s[4 * j] = to_tf32(exp2f(s[4 * j] * scale_log2e - mb0));          // the row sum is over what the MMA will see
+        s[4 * j + 1] = to_tf32(exp2f(s[4 * j + 1] * scale_log2e - mb0));
+        s[4 * j + 2] = to_tf32(exp2f(s[4 * j + 2] * scale_log2e - mb1));
+        s[4 * j + 3] = to_tf32(exp2f(s[4 * j + 3] * scale_log2e - mb1));
+        sum0 += s[4 * j] + s[4 * j + 1];
+        sum1 += s[4 * j + 2] + s[4 * j + 3];
+    }
+#pragma unroll
+    for (int o = 1; o < 4; o <<= 1) {
+        sum0 += __shfl_xor_sync(0xffffffffu, sum0, o);
+        sum1 += __shfl_xor_sync(0xffffffffu, sum1, o);
+    }
+    const float inv0 = 1.0f / sum0, inv1 = 1.0f / sum1;
+    if (stats && t == 0) {   // what the backward needs to rebuild exactly these probabilities: (max * scale * log2 e, 1 / sum)
+        float2 *st = reinterpret_cast<float2 *>(stats) + ((size_t)img * n_heads + head) * kSaL + half * 128 + row;
+        st[0] = make_float2(mb0, inv0);
+        st[8] = make_float2(mb1, inv1);
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+
+    // ---- O = P V   (A = P from registers, B = V^T from shared memory)
+    float o[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) o[i] = 0.0f;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kSaL / 8; ++kk) {
+        uint32_t a[4];
+        acc_to_a(s, kk, a);
+        wgmma_rs_n128(o, a, gmma_desc(smem_u32(sK) + kk * 2 * kLboV, kLboV, 128), kk > 0);
+    }
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_operands(o);
+    // ---- epilogue
+    float *dst = out + ((size_t)img * kSaL + (size_t)half * 128 + row) * inner + (size_t)head * kSaD + 2 * t;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        *reinterpret_cast<float2 *>(dst + 8 * j) = make_float2(o[4 * j] * inv0, o[4 * j + 1] * inv0);
+        *reinterpret_cast<float2 *>(dst + 8 * (size_t)inner + 8 * j) = make_float2(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1);
+    }
 }
 
 }  // namespace ps
@@ -217,7 +141,7 @@ static int self_attention_forward_impl(int32_t n_images, int32_t tokens, int32_t
         return PS_ERR_UNSUPPORTED;
     }
     if (((uintptr_t)qkv | (uintptr_t)out) & 15) { set_error("ps_self_attention_forward: pointers must be 16-byte aligned"); return PS_ERR_INVALID_ARGUMENT; }
-    const size_t smem = 192 * 1024 + 64 + 128 * sizeof(float);
+    const size_t smem = 192 * 1024;
     static unsigned long long attr_devices = 0;
     if (first_use_on_device(attr_devices)) {
         PS_CUDA_CHECK(cudaFuncSetAttribute(k_self_attention_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

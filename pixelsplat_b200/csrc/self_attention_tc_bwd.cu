@@ -1,45 +1,42 @@
-// Backward of the dense per-image self-attention (self_attention_tc.cu) on the same tcgen05 / TMEM path:
-// autograd of softmax(Q K^T * scale) V for the ViT blocks of ImageSelfAttention
-// (/root/reference/src/model/encoder/epipolar/image_self_attention.py:57-79 ->
-//  /root/reference/src/model/transformer/attention.py:54-70 with z = None; SURVEY.md 8 row a14).
+// Backward of the dense per-image self-attention (self_attention_tc.cu) on the same wgmma path: autograd of
+// softmax(Q K^T * scale) V for the ViT blocks of ImageSelfAttention (reference: src/model/encoder/epipolar/
+// image_self_attention.py:57-79 -> src/model/transformer/attention.py:54-70 with z = None; SURVEY.md 8 row a14).
 //
 // Per (image, head), with Pn the forward's probabilities -- rebuilt from the saved per-row (max, 1 / sum) with
 // the same TF32 roundings, so the backward differentiates the forward that actually ran:
 //     dPn = dO V^T      D_i = dO_i . O_i      dS = Pn o (dPn - D) * scale
 //     dQ = dS K         dK = dS^T Q           dV = Pn^T dO
-// Two CTA roles (grid.x = 4), 8 warps, every contraction a tcgen05.mma with FP32 accumulation in TMEM:
-//   role 0/1 "query half I" -> dQ_I.  S = Q_I K^T (TMEM cols 0..255) and dPn = dO_I V^T (cols 256..511) with
-//            A / B staged K-major in shared memory; thread = query row turns S into dS in place; then
-//            dQ_I = dS K with A = dS read straight from TMEM and B = K^T staged transposed (the forward's P V
-//            step with other operands), accumulated over dPn's dead columns.
+// Two CTA roles (grid.x = 4), two warpgroups of 64 rows each, every contraction a wgmma with FP32 accumulators
+// in registers:
+//   role 0/1 "query half I" -> dQ_I.  S = Q_I K^T (m64n256, 128 registers) becomes Pn in place; dPn = dO_I V^T
+//            follows in two 128-key halves (64 registers each), each turned into dS over Pn's registers; then
+//            dQ_I = dS K with A = dS straight from registers and B = K^T staged transposed.
 //   role 2/3 "key half J"   -> dK_J, dV_J.  The transposed problem, so that the rows a CTA owns are the rows it
-//            sums over: S^T = K_J Q_I'^T and dPn^T = V_J dO_I'^T for the two query halves I' in turn (128 TMEM
-//            columns each), thread = key row builds Pn^T and dS^T in place (the per-query constants max, 1 / sum
-//            and D are per COLUMN here: 256-entry shared arrays), then dV_J += Pn^T dO_I' and dK_J += dS^T Q_I'
-//            with A from TMEM and B = dO_I'^T / Q_I'^T staged transposed; the two accumulators own the other 256
-//            TMEM columns across both I'.
-// Shared memory: 3 x 64 KB operand buffers (K_J, V_J persistent + one rotating buffer in role 2/3; Q/dO + K/V in
-// role 0/1) -- the forward's 192 KB; operands are rounded to the nearest TF32 on the way in, like the forward's.
-#include "umma_tf32.cuh"
+//            sums over: for the four 64-query chunks C in turn, S^T = K_J Q_C^T and dPn^T = V_J dO_C^T
+//            (m64n64), thread = key row builds Pn^T and dS^T in place (the per-query constants max, 1 / sum
+//            and D are per COLUMN here: 256-entry shared arrays), then dV_J += Pn^T dO_C and dK_J += dS^T Q_C
+//            with A from registers and B = dO_C^T / Q_C^T staged transposed over the chunk's natural copies.
+// Shared memory: 3 x 64 KB operand buffers (Q / dO + K / V in role 0/1; K_J, V_J + the chunk's two 32 KB
+// operands in role 2/3); operands are rounded to the nearest TF32 on the way in, like the forward's.
+#include "wgmma_tf32.cuh"
 
 namespace ps {
 
 namespace {
 
-constexpr uint32_t kLbo128 = 128 * 16;   // bytes between 16-byte K chunks of a 128-row tile
+constexpr uint32_t kLbo64 = 64 * 16;     // bytes between 16-byte K chunks of a 64-row tile
+constexpr uint32_t kLbo128 = 128 * 16;
 constexpr uint32_t kLbo256 = 256 * 16;
 
 __device__ __forceinline__ void sync_before_mma() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic -> async proxy (smem operands)
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
-__device__ __forceinline__ void wait_mma(uint32_t bar, uint32_t &phase) {
-    mbar_wait(bar, phase);
-    phase ^= 1u;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+template <int N>
+__device__ __forceinline__ void zero(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) d[i] = 0.0f;
 }
 
 }  // namespace
@@ -50,12 +47,12 @@ k_self_attention_tc_bwd(const float *__restrict__ qkv, const float *__restrict__
                         float scale_log2e) {
     extern __shared__ __align__(128) unsigned char s_sa[];
     unsigned char *buf0 = s_sa, *buf1 = s_sa + 64 * 1024, *buf2 = s_sa + 128 * 1024;
-    uint64_t *bar = reinterpret_cast<uint64_t *>(s_sa + 192 * 1024);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(s_sa + 192 * 1024 + 16);
-    float *s_mb = reinterpret_cast<float *>(s_sa + 192 * 1024 + 64);     // [256] row max * scale * log2 e
+    float *s_mb = reinterpret_cast<float *>(s_sa + 192 * 1024);          // [256] row max * scale * log2 e
     float *s_inv = s_mb + 256;                                            // [256] 1 / row sum
     float *s_D = s_inv + 256;                                             // [256] dO_i . O_i
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+    const int t = lane & 3;
+    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);              // first of this thread's rows (+8)
     const int role = blockIdx.x >> 1, half = blockIdx.x & 1, head = blockIdx.y, img = blockIdx.z;
     const int inner = n_heads * kSaD;
     const size_t rs3 = 3 * (size_t)inner, rs1 = (size_t)inner;            // floats per token in qkv / out
@@ -65,17 +62,8 @@ k_self_attention_tc_bwd(const float *__restrict__ qkv, const float *__restrict__
     const float *do_img = d_out + (size_t)img * kSaL * rs1 + (size_t)head * kSaD;
     float *dq_img = d_qkv + (size_t)img * kSaL * rs3 + (size_t)head * kSaD;
     float *dk_img = dq_img + inner, *dv_img = dq_img + 2 * inner;
-    const uint32_t bar_a = smem_u32(bar);
+    const uint32_t a_row = (uint32_t)wg * 64 * 16;                          // this warpgroup's rows in an A tile
 
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     :: "r"(smem_u32(tmem_slot)), "n"(kSaTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(bar_a) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
     // per-query constants of all 256 queries: (max, 1 / sum) saved by the forward, D = dO . O
     {
         const int i = tid;                                                  // kSaThreads == kSaL
@@ -92,9 +80,6 @@ k_self_attention_tc_bwd(const float *__restrict__ qkv, const float *__restrict__
         }
         s_D[i] = acc;
     }
-    uint32_t phase = 0;
-    const uint32_t lane_addr = (uint32_t)((warp & 3) * 32) << 16;             // this warp's TMEM lane quarter
-    const int row = (warp & 3) * 32 + lane;                                   // row of the CTA's 128-row half
 
     if (role == 0) {
         // ================================================================= dQ for query half `half`
@@ -102,165 +87,142 @@ k_self_attention_tc_bwd(const float *__restrict__ qkv, const float *__restrict__
         stage_natural<128>(sQ, q_img + (size_t)half * 128 * rs3, rs3, tid, kSaThreads);
         stage_natural<256>(sK, k_img, rs3, tid, kSaThreads);
         sync_before_mma();
-        const uint32_t tmem = *tmem_slot;
-        const uint32_t tmem_S = tmem, tmem_dP = tmem + 256, tmem_dQ = tmem + 256;
-        if (tid == 0) {
-            const uint32_t idesc = umma_idesc_tf32(128, 256);
+        float s[128];
+        zero(s);
+        wgmma_fence();
 #pragma unroll 1
-            for (int k = 0; k < kSaD / 8; ++k)
-                mma_tf32_ss(tmem_S, umma_desc(smem_u32(sQ) + k * 2 * kLbo128, kLbo128, 128),
-                            umma_desc(smem_u32(sK) + k * 2 * kLbo256, kLbo256, 128), idesc, k > 0);
-            umma_commit(bar_a);
+        for (int k = 0; k < kSaD / 8; ++k)
+            wgmma_ss_n256(s, gmma_desc(smem_u32(sQ) + k * 2 * kLbo128 + a_row, kLbo128, 128),
+                          gmma_desc(smem_u32(sK) + k * 2 * kLbo256, kLbo256, 128), k > 0);
+        wgmma_commit();
+        wgmma_wait_all();
+        fence_operands(s);
+        // S -> Pn in place (rows i0 = s[4 j + 0 / 1], i0 + 8 = s[4 j + 2 / 3])
+        const int i0 = half * 128 + row;
+        const float mb0 = s_mb[i0], inv0 = s_inv[i0], D0 = s_D[i0];
+        const float mb1 = s_mb[i0 + 8], inv1 = s_inv[i0 + 8], D1 = s_D[i0 + 8];
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+            s[4 * j] = to_tf32(exp2f(s[4 * j] * scale_log2e - mb0)) * inv0;
+            s[4 * j + 1] = to_tf32(exp2f(s[4 * j + 1] * scale_log2e - mb0)) * inv0;
+            s[4 * j + 2] = to_tf32(exp2f(s[4 * j + 2] * scale_log2e - mb1)) * inv1;
+            s[4 * j + 3] = to_tf32(exp2f(s[4 * j + 3] * scale_log2e - mb1)) * inv1;
         }
-        wait_mma(bar_a, phase);
-        // dPn = dO_I V^T
+        __syncthreads();                                                      // Q and K are dead
         stage_natural<128>(sQ, do_img + (size_t)half * 128 * rs1, rs1, tid, kSaThreads);
         stage_natural<256>(sK, v_img, rs3, tid, kSaThreads);
         sync_before_mma();
-        if (tid == 0) {
-            const uint32_t idesc = umma_idesc_tf32(128, 256);
+        // dPn = dO_I V^T one 128-key half at a time; Pn -> dS (TF32) in place
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            float dp[64];
+            zero(dp);
+            wgmma_fence();
 #pragma unroll 1
             for (int k = 0; k < kSaD / 8; ++k)
-                mma_tf32_ss(tmem_dP, umma_desc(smem_u32(sQ) + k * 2 * kLbo128, kLbo128, 128),
-                            umma_desc(smem_u32(sK) + k * 2 * kLbo256, kLbo256, 128), idesc, k > 0);
-            umma_commit(bar_a);
-        }
-        wait_mma(bar_a, phase);
-        if (warp >= 4) {
-            // K^T into the K/V buffer (V is dead: its MMAs have completed)
-            stage_transposed<256>(sK, k_img, rs3, tid - 128, 128);
-        } else {
-            // thread = query row: S -> dS in place (TF32)
-            const int i = half * 128 + row;
-            const float mb = s_mb[i], inv = s_inv[i], Di = s_D[i];
-            for (int c = 0; c < 256; c += 32) {
-                float sv[32], dp[32];
-                tmem_ld32(tmem_S + lane_addr + c, sv);
-                tmem_ld32(tmem_dP + lane_addr + c, dp);
+                wgmma_ss_n128(dp, gmma_desc(smem_u32(sQ) + k * 2 * kLbo128 + a_row, kLbo128, 128),
+                              gmma_desc(smem_u32(sK) + k * 2 * kLbo256 + h * 128 * 16, kLbo256, 128), k > 0);
+            wgmma_commit();
+            wgmma_wait_all();
+            fence_operands(dp);
 #pragma unroll
-                for (int x = 0; x < 32; ++x) {
-                    const float p = to_tf32(exp2f(sv[x] * scale_log2e - mb)) * inv;
-                    sv[x] = to_tf32(p * (dp[x] - Di) * scale);
-                }
-                tmem_st32(tmem_S + lane_addr + c, sv);
+            for (int x = 0; x < 64; ++x) {
+                float &p = s[64 * h + x];
+                p = to_tf32(p * (dp[x] - ((x & 2) ? D1 : D0)) * scale);
             }
-            asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
         }
+        __syncthreads();                                                      // dO and V are dead
+        stage_transposed<256>(sK, k_img, rs3, tid, kSaThreads);              // K^T (B of dQ)
         sync_before_mma();
-        if (tid == 0) {
-            const uint32_t idesc = umma_idesc_tf32(128, 128);
-#pragma unroll 1
-            for (int k = 0; k < kSaL / 8; ++k)
-                mma_tf32_ts(tmem_dQ, tmem_S + k * 8, umma_desc(smem_u32(sK) + k * 2 * kLbo128, kLbo128, 128), idesc, k > 0);
-            umma_commit(bar_a);
-        }
-        wait_mma(bar_a, phase);
-        {
-            const int c0 = (warp >> 2) * 64;
-            float *dst = dq_img + (size_t)(half * 128 + row) * rs3 + c0;
-            for (int c = 0; c < 64; c += 32) {
-                float v[32];
-                tmem_ld32(tmem_dQ + lane_addr + c0 + c, v);
+        float dq[64];
+        zero(dq);
+        wgmma_fence();
 #pragma unroll
-                for (int x = 0; x < 32; x += 4)
-                    *reinterpret_cast<float4 *>(dst + c + x) = make_float4(v[x], v[x + 1], v[x + 2], v[x + 3]);
-            }
+        for (int kk = 0; kk < kSaL / 8; ++kk) {
+            uint32_t a[4];
+            acc_to_a(s, kk, a);
+            wgmma_rs_n128(dq, a, gmma_desc(smem_u32(sK) + kk * 2 * kLbo128, kLbo128, 128), kk > 0);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        fence_operands(dq);
+        float *dst = dq_img + (size_t)i0 * rs3 + 2 * t;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            *reinterpret_cast<float2 *>(dst + 8 * j) = make_float2(dq[4 * j], dq[4 * j + 1]);
+            *reinterpret_cast<float2 *>(dst + 8 * rs3 + 8 * j) = make_float2(dq[4 * j + 2], dq[4 * j + 3]);
         }
     } else {
         // ================================================================= dK, dV for key half `half`
-        unsigned char *sKj = buf0, *sVj = buf1, *sC = buf2;
+        unsigned char *sKj = buf0, *sVj = buf1, *sQc = buf2, *sOc = buf2 + 32 * 1024;
         stage_natural<128>(sKj, k_img + (size_t)half * 128 * rs3, rs3, tid, kSaThreads);
         stage_natural<128>(sVj, v_img + (size_t)half * 128 * rs3, rs3, tid, kSaThreads);
-        sync_before_mma();
-        const uint32_t tmem = *tmem_slot;
-        const uint32_t tmem_ST = tmem, tmem_DPT = tmem + 128, tmem_dV = tmem + 256, tmem_dK = tmem + 384;
-        const uint32_t idesc = umma_idesc_tf32(128, 128);
+        float dv[64], dk[64];
+        zero(dv);
+        zero(dk);
 #pragma unroll 1
-        for (int ih = 0; ih < 2; ++ih) {
-            const float *q_i = q_img + (size_t)ih * 128 * rs3, *do_i = do_img + (size_t)ih * 128 * rs1;
-            // S^T = K_J Q_I'^T
-            stage_natural<128>(sC, q_i, rs3, tid, kSaThreads);
+        for (int q0 = 0; q0 < kSaL; q0 += 64) {
+            const float *q_c = q_img + (size_t)q0 * rs3, *do_c = do_img + (size_t)q0 * rs1;
+            stage_natural<64>(sQc, q_c, rs3, tid, kSaThreads);
+            stage_natural<64>(sOc, do_c, rs1, tid, kSaThreads);
             sync_before_mma();
-            if (tid == 0) {
+            // S^T = K_J Q_C^T, dPn^T = V_J dO_C^T
+            float st[32], dpt[32];
+            zero(st);
+            zero(dpt);
+            wgmma_fence();
 #pragma unroll 1
-                for (int k = 0; k < kSaD / 8; ++k)
-                    mma_tf32_ss(tmem_ST, umma_desc(smem_u32(sKj) + k * 2 * kLbo128, kLbo128, 128),
-                                umma_desc(smem_u32(sC) + k * 2 * kLbo128, kLbo128, 128), idesc, k > 0);
-                umma_commit(bar_a);
+            for (int k = 0; k < kSaD / 8; ++k) {
+                wgmma_ss_n64(st, gmma_desc(smem_u32(sKj) + k * 2 * kLbo128 + a_row, kLbo128, 128),
+                             gmma_desc(smem_u32(sQc) + k * 2 * kLbo64, kLbo64, 128), k > 0);
+                wgmma_ss_n64(dpt, gmma_desc(smem_u32(sVj) + k * 2 * kLbo128 + a_row, kLbo128, 128),
+                             gmma_desc(smem_u32(sOc) + k * 2 * kLbo64, kLbo64, 128), k > 0);
             }
-            wait_mma(bar_a, phase);
-            // dPn^T = V_J dO_I'^T
-            stage_natural<128>(sC, do_i, rs1, tid, kSaThreads);
-            sync_before_mma();
-            if (tid == 0) {
-#pragma unroll 1
-                for (int k = 0; k < kSaD / 8; ++k)
-                    mma_tf32_ss(tmem_DPT, umma_desc(smem_u32(sVj) + k * 2 * kLbo128, kLbo128, 128),
-                                umma_desc(smem_u32(sC) + k * 2 * kLbo128, kLbo128, 128), idesc, k > 0);
-                umma_commit(bar_a);
-            }
-            wait_mma(bar_a, phase);
-            if (warp >= 4) {
-                stage_transposed<128>(sC, do_i, rs1, tid - 128, 128);         // dO_I'^T (B of dV)
-            } else {
-                // thread = key row: S^T -> Pn^T, dPn^T -> dS^T, in place; the query constants are per column
-                for (int c = 0; c < 128; c += 32) {
-                    float sv[32], dp[32];
-                    tmem_ld32(tmem_ST + lane_addr + c, sv);
-                    tmem_ld32(tmem_DPT + lane_addr + c, dp);
+            wgmma_commit();
+            wgmma_wait_all();
+            fence_operands(st);
+            fence_operands(dpt);
+            // thread = key row: S^T -> Pn^T, dPn^T -> dS^T, in place; query i = column 8 j + 2 t (+1)
 #pragma unroll
-                    for (int x = 0; x < 32; ++x) {
-                        const int i = ih * 128 + c + x;
-                        const float p = to_tf32(exp2f(sv[x] * scale_log2e - s_mb[i])) * s_inv[i];
-                        sv[x] = to_tf32(p);
-                        dp[x] = to_tf32(p * (dp[x] - s_D[i]) * scale);
-                    }
-                    tmem_st32(tmem_ST + lane_addr + c, sv);
-                    tmem_st32(tmem_DPT + lane_addr + c, dp);
-                }
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+            for (int x = 0; x < 32; ++x) {
+                const int i = q0 + 8 * (x >> 2) + 2 * t + (x & 1);
+                const float p = to_tf32(exp2f(st[x] * scale_log2e - s_mb[i])) * s_inv[i];
+                st[x] = to_tf32(p);
+                dpt[x] = to_tf32(p * (dpt[x] - s_D[i]) * scale);
             }
+            __syncthreads();                                                  // Q_C, dO_C natural copies are dead
+            stage_transposed<64>(sOc, do_c, rs1, tid, kSaThreads);            // dO_C^T (B of dV)
+            stage_transposed<64>(sQc, q_c, rs3, tid, kSaThreads);             // Q_C^T (B of dK)
             sync_before_mma();
-            if (tid == 0) {                                                   // dV_J += Pn^T dO_I'
-#pragma unroll 1
-                for (int k = 0; k < 128 / 8; ++k)
-                    mma_tf32_ts(tmem_dV, tmem_ST + k * 8, umma_desc(smem_u32(sC) + k * 2 * kLbo128, kLbo128, 128), idesc,
-                                (ih > 0) || (k > 0));
-                umma_commit(bar_a);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 8; ++kk) {
+                uint32_t a[4];
+                acc_to_a(st, kk, a);
+                wgmma_rs_n128(dv, a, gmma_desc(smem_u32(sOc) + kk * 2 * kLbo128, kLbo128, 128), 1);
             }
-            wait_mma(bar_a, phase);
-            stage_transposed<128>(sC, q_i, rs3, tid, kSaThreads);            // Q_I'^T (B of dK)
-            sync_before_mma();
-            if (tid == 0) {                                                   // dK_J += dS^T Q_I'
-#pragma unroll 1
-                for (int k = 0; k < 128 / 8; ++k)
-                    mma_tf32_ts(tmem_dK, tmem_DPT + k * 8, umma_desc(smem_u32(sC) + k * 2 * kLbo128, kLbo128, 128), idesc,
-                                (ih > 0) || (k > 0));
-                umma_commit(bar_a);
+#pragma unroll
+            for (int kk = 0; kk < 8; ++kk) {
+                uint32_t a[4];
+                acc_to_a(dpt, kk, a);
+                wgmma_rs_n128(dk, a, gmma_desc(smem_u32(sQc) + kk * 2 * kLbo128, kLbo128, 128), 1);
             }
-            wait_mma(bar_a, phase);
+            wgmma_commit();
+            wgmma_wait_all();
+            fence_operands(dv);
+            fence_operands(dk);
+            __syncthreads();                                                  // before the next chunk restages
         }
-        {
-            const int c0 = (warp >> 2) * 64;
-            float *dk = dk_img + (size_t)(half * 128 + row) * rs3 + c0;
-            float *dv = dv_img + (size_t)(half * 128 + row) * rs3 + c0;
-            for (int c = 0; c < 64; c += 32) {
-                float v[32];
-                tmem_ld32(tmem_dK + lane_addr + c0 + c, v);
+        const size_t j0 = (size_t)half * 128 + row;
+        float *dkp = dk_img + j0 * rs3 + 2 * t, *dvp = dv_img + j0 * rs3 + 2 * t;
 #pragma unroll
-                for (int x = 0; x < 32; x += 4)
-                    *reinterpret_cast<float4 *>(dk + c + x) = make_float4(v[x], v[x + 1], v[x + 2], v[x + 3]);
-                tmem_ld32(tmem_dV + lane_addr + c0 + c, v);
-#pragma unroll
-                for (int x = 0; x < 32; x += 4)
-                    *reinterpret_cast<float4 *>(dv + c + x) = make_float4(v[x], v[x + 1], v[x + 2], v[x + 3]);
-            }
+        for (int j = 0; j < 16; ++j) {
+            *reinterpret_cast<float2 *>(dkp + 8 * j) = make_float2(dk[4 * j], dk[4 * j + 1]);
+            *reinterpret_cast<float2 *>(dkp + 8 * rs3 + 8 * j) = make_float2(dk[4 * j + 2], dk[4 * j + 3]);
+            *reinterpret_cast<float2 *>(dvp + 8 * j) = make_float2(dv[4 * j], dv[4 * j + 1]);
+            *reinterpret_cast<float2 *>(dvp + 8 * rs3 + 8 * j) = make_float2(dv[4 * j + 2], dv[4 * j + 3]);
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(*tmem_slot), "n"(kSaTmemCols) : "memory");
 }
 
 }  // namespace ps
@@ -281,7 +243,7 @@ extern "C" PS_API int ps_self_attention_backward(int32_t n_images, int32_t token
         set_error("ps_self_attention_backward: pointers must be 16-byte aligned");
         return PS_ERR_INVALID_ARGUMENT;
     }
-    const size_t smem = 192 * 1024 + 64 + 3 * 256 * sizeof(float);
+    const size_t smem = 192 * 1024 + 3 * 256 * sizeof(float);
     static unsigned long long attr_devices = 0;
     if (first_use_on_device(attr_devices)) {
         PS_CUDA_CHECK(cudaFuncSetAttribute(k_self_attention_tc_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -1,4 +1,4 @@
-"""Host side of the tcgen05 self-attention kernel (csrc/self_attention_tc.cu): softmax(q k^T * scale) v
+"""Host side of the wgmma self-attention kernel (csrc/self_attention_tc.cu): softmax(q k^T * scale) v
 for ImageSelfAttention's ViT blocks, TF32 operands / FP32 accumulation on the tensor cores.
 
 Reference semantics: /root/reference/src/model/transformer/attention.py:54-70 (z = None).  Forward AND

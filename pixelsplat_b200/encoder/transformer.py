@@ -10,7 +10,7 @@ encoder_visualizer_epipolar.py:53-56) the module falls back to the explicit soft
 hook sees the [(b v r), head, 1, s*ov] attention tensor it expects.
 
 With z = None (ImageSelfAttention's ViT blocks) and the shape the kernel is written for (256 tokens,
-128-dim heads) the soft-max attention runs on the tcgen05 tensor cores
+128-dim heads) the soft-max attention runs on the tensor cores (wgmma)
 (pixelsplat_b200/encoder/self_attention_tc.py); other shapes use torch's fp32 matmul + softmax.
 """
 from __future__ import annotations

@@ -146,8 +146,10 @@ def test_bench_roofline_object_is_built_from_the_profile_file():
     assert r["kernel"] == "composite_bwd" and r["unit"] == "GB/s" and 0 < r["frac"] < 1
     assert r["algorithmic_bytes_per_launch"] == 399057 * (48 + 36) + 65536 * 20
     prof_path = ROOT / "profiles" / "kernel_metrics_V1.json"
-    prof = _json.loads(prof_path.read_text())
-    if prof["csrc_sha"] == bench.csrc_sha():
+    prof = _json.loads(prof_path.read_text()) if prof_path.exists() else None
+    if prof is None:        # no profile of this build stored: nothing from it is reported, and the note says why
+        assert r["traffic"] is None and r["issue_frac"] is None and "absent" in r["profile"]
+    elif prof["csrc_sha"] == bench.csrc_sha():
         kp = prof["k_composite_bwd2"]
         assert r["traffic"] == kp["dram_bytes"] and r["bound"] == "issue"
         assert abs(r["issue_frac"] - kp["warp_inst"] / 0.080e-3 / bench.ISSUE_PEAK) < 1e-12 and 0 < r["issue_frac"] < 1

@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 self-attention kernels (csrc/self_attention_tc.cu and _bwd.cu, SURVEY.md 8 row a14)
+"""GPU tests of the wgmma self-attention kernels (csrc/self_attention_tc.cu and _bwd.cu, SURVEY.md 8 row a14)
 against the reference's formula softmax(q k^T * scale) v
 (/root/reference/src/model/transformer/attention.py:54-70, z = None) evaluated in float64 by torch.
 
@@ -81,7 +81,7 @@ def test_structured_input_catches_layout_errors():
 
 @pytest.mark.parametrize("n,heads", [(2, 4), (1, 1), (3, 8)])
 def test_gradients_match_float64(n, heads, monkeypatch):
-    """The tcgen05 backward (csrc/self_attention_tc_bwd.cu): dq, dk, dv separately against float64 autograd of the
+    """The wgmma backward (csrc/self_attention_tc_bwd.cu): dq, dk, dv separately against float64 autograd of the
     reference formula.  Stated tolerance: TF32 operands (q, k, v, dO, probabilities and d score rounded to 10
     mantissa bits) -> 3e-3 relative (max-norm) per tensor; the round-1 torch backward (fp32 GEMMs) is kept under
     PIXELSPLAT_B200_SELF_ATTENTION_BWD=torch and must sit at 1e-4."""

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Times the tcgen05 self-attention kernel (csrc/self_attention_tc.cu) against torch's own paths for
+"""Times the wgmma self-attention kernel (csrc/self_attention_tc.cu) against torch's own paths for
 the same contraction -- fp32 matmul + softmax (what the reference runs, attention.py:54-70), the
 same with TF32 matmuls allowed, and F.scaled_dot_product_attention -- at ImageSelfAttention's shape
 (256 tokens, 4 heads x 128) for a range of image counts.  CUDA events, L2 not flushed (the whole
@@ -36,7 +36,7 @@ def main():
     heads, L, d = 4, 256, 128
     scale = d ** -0.5
     rows = []
-    for n in (2, 14, 37, 148):
+    for n in (2, 14, 37, 132):
         qkv = torch.randn(n, L, 3 * heads * d, device=dev)
 
         def explicit():
@@ -55,7 +55,7 @@ def main():
         t_tf32 = timed(explicit)
         torch.backends.cuda.matmul.allow_tf32 = False
         t_sdpa = timed(sdpa)
-        # forward + backward: the tcgen05 pair vs the round-1 backward (fp32 torch GEMMs) behind the same forward
+        # forward + backward: the wgmma pair vs the round-1 backward (fp32 torch GEMMs) behind the same forward
         import os
         qg = qkv.clone().requires_grad_(True)
         wgt = torch.randn(n, L, heads * d, device=dev)
@@ -72,9 +72,9 @@ def main():
         ref = explicit().double()
         err = float((sa.self_attention_tc(qkv, heads, scale).double() - ref).abs().max() / ref.abs().max())
         flops = n * heads * 2 * (2.0 * L * L * d)
-        rows.append({"images": n, "ctas": 2 * heads * n, "tcgen05_us": t_tc, "torch_fp32_us": t_fp32,
+        rows.append({"images": n, "ctas": 2 * heads * n, "wgmma_us": t_tc, "torch_fp32_us": t_fp32,
                      "torch_tf32_us": t_tf32, "torch_sdpa_us": t_sdpa,
-                     "fwd_bwd_tcgen05_us": t_fb_tc, "fwd_bwd_torch_backward_us": t_fb_torch, "tcgen05_tflops": flops / t_tc * 1e-6,
+                     "fwd_bwd_wgmma_us": t_fb_tc, "fwd_bwd_torch_backward_us": t_fb_torch, "wgmma_tflops": flops / t_tc * 1e-6,
                      "rel_err_vs_torch_fp32": err})
     print(json.dumps({"what": "self-attention 256 tokens x 4 heads x 128; forward, and forward + backward (incl. the loss ops)", "rows": rows}))
 

@@ -1,6 +1,6 @@
 """Summarise an `ncu --csv` launch list (tools/ncu_raster_launches.sh): per kernel name, launches, mean device time,
-share of the total, and the mean of the other collected metrics (issue% = warp instructions / duration / (148 SMs x 4
-schedulers x 1965 MHz), computed here).  usage: python tools/summarize_launches.py FILE [skip_first_n] [--json OUT]
+share of the total, and the mean of the other collected metrics (issue% = warp instructions / duration / (132 SMs x 4
+schedulers x 1980 MHz), computed here).  usage: python tools/summarize_launches.py FILE [skip_first_n] [--json OUT]
 --json writes {kernel: {us, warp_inst, dram_bytes, ...}, "csrc_sha": <hash of the CUDA sources the capture was built
 from>} -- the file bench.py reads `roofline.traffic` / `issue_frac` from (never a literal in bench.py)."""
 import csv
@@ -10,7 +10,7 @@ import sys
 from pathlib import Path
 from collections import OrderedDict, defaultdict
 
-ISSUE_PEAK = 148 * 4 * 1.965e9     # warp instructions / s
+ISSUE_PEAK = 132 * 4 * 1.98e9      # warp instructions / s (H100 SXM)
 argv = [a for a in sys.argv[1:]]
 json_out = None
 if "--json" in argv:
