@@ -162,9 +162,12 @@ PS_API int ps_timing_read(float *ms);
 
 /* Process-wide tunables of the compositor, for A/B measurements and tests (defaults are automatic):
  *   "composite_impl"      2 = warp-task compositor (default), 1 = round-1 CTA-per-tile compositor;
- *   "composite_segments"  0 = automatic (default), 1 | 2 | 4 = list runs per warp task.
- * Takes effect for forwards issued afterwards (a backward uses the split its forward used only if the option is
- * unchanged in between).  Also read once from PIXELSPLAT_B200_COMPOSITE / PIXELSPLAT_B200_SEGMENTS. */
+ *   "composite_segments"  0 = automatic (default), 1 | 2 | 4 = list runs per warp task;
+ *   "composite_hit_lists" 2 = automatic (default: kept while 64 x instance_capacity <= 512 MB), 0 = never keep,
+ *                         1 = always keep the forward's per-block hit lists for the backward (binning_bytes grows).
+ * Takes effect for forwards issued afterwards (a backward uses the split and the hit lists its forward used only if
+ * the options are unchanged in between).  Also read once from PIXELSPLAT_B200_COMPOSITE / PIXELSPLAT_B200_SEGMENTS /
+ * PIXELSPLAT_B200_HIT_LISTS. */
 PS_API int ps_set_option(const char *name, int value);
 
 /* Workspace sizes / layout for a descriptor. */

@@ -138,7 +138,8 @@ int launch_composite_backward_v1(const Dims &d, const Inputs &in, const Geom &g,
                                  const unsigned long long *keys, const ImageState &img,
                                  const float *d_color, const ViewGrads &vg, cudaStream_t st);
 int composite_impl();   // 1 = legacy, 2 = warp-task compositor (env PIXELSPLAT_B200_COMPOSITE, default 2)
-int set_composite_option(int which, int value);   // 0: impl (1 | 2), 1: segments (0 = auto | 1 | 2 | 4)
+int set_composite_option(int which, int value);   // 0: impl (1 | 2), 1: segments (0 = auto | 1 | 2 | 4),
+                                                  // 2: hit lists (0 = never | 1 = always | 2 = auto)
 int composite_segments(long long tasks);
 bool composite_hit_lists(long long capacity);      // keep the forward's hit lists for the backward?   // list runs per task (1, 2, 4) for a batch of `tasks` warp tasks
 int launch_preprocess_backward(const Dims &d, const Inputs &in, const Geom &g, const ViewGrads &vg,

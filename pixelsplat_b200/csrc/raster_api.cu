@@ -270,6 +270,7 @@ PS_API int ps_set_option(const char *name, int value) {
     int rc = PS_ERR_INVALID_ARGUMENT;
     if (!strcmp(name, "composite_impl")) rc = set_composite_option(0, value);
     else if (!strcmp(name, "composite_segments")) rc = set_composite_option(1, value);
+    else if (!strcmp(name, "composite_hit_lists")) rc = set_composite_option(2, value);
     if (rc) set_error("ps_set_option: unknown option or bad value: %s = %d", name, value);
     return rc;
 }

@@ -612,6 +612,7 @@ k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
 // Tunables (A/B measurements, tests): initialised from the environment once, changeable through ps_set_option.
 static int g_impl = 0;        // 1 = legacy CTA-per-tile compositor, 2 = warp tasks
 static int g_segments = -1;   // 0 = automatic, else 1 | 2 | 4 list runs per task
+static int g_hit_lists = -1;  // 0 = never keep, 1 = always keep, 2 = automatic
 
 int composite_impl() {
     if (g_impl == 0) {
@@ -624,6 +625,7 @@ int composite_impl() {
 int set_composite_option(int which, int value) {
     if (which == 0 && (value == 1 || value == 2)) { g_impl = value; return PS_OK; }
     if (which == 1 && (value == 0 || value == 1 || value == 2 || value == 4)) { g_segments = value; return PS_OK; }
+    if (which == 2 && (value == 0 || value == 1 || value == 2)) { g_hit_lists = value; return PS_OK; }
     return PS_ERR_INVALID_ARGUMENT;
 }
 
@@ -698,13 +700,12 @@ int composite_segments(long long tasks) {
 // 512 MB (every configuration of BASELINE.json at batch 1-2), dropped beyond (the backward then culls for itself).
 // PIXELSPLAT_B200_HIT_LISTS = 0 | 1 forces it (A/B runs); the legacy compositor never uses them.
 bool composite_hit_lists(long long capacity) {
-    static int forced = -1;
-    if (forced < 0) {
+    if (g_hit_lists < 0) {
         const char *e = getenv("PIXELSPLAT_B200_HIT_LISTS");
-        forced = (e && (e[0] == '0' || e[0] == '1') && e[1] == 0) ? (e[0] - '0') : 2;
+        g_hit_lists = (e && (e[0] == '0' || e[0] == '1') && e[1] == 0) ? (e[0] - '0') : 2;
     }
     if (composite_impl() == 1) return false;
-    if (forced != 2) return forced == 1;
+    if (g_hit_lists != 2) return g_hit_lists == 1;
     return capacity * 64 <= (512ll << 20);
 }
 

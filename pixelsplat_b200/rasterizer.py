@@ -166,6 +166,7 @@ class RasterOutputState:
             return buf[off:off + nbytes].view(dtype).reshape(shape)
 
         P = d.n_gaussians
+        hw = d.height * d.width
         return dict(
             depth=view(self.geom, lay.depth, torch.float32, vp, (vt, P)),
             radii=view(self.geom, lay.radii, torch.int32, vp, (vt, P)),
@@ -177,10 +178,11 @@ class RasterOutputState:
             tile_count=view(self.geom, lay.tile_count, torch.int32, vt * tiles, (vt, tiles)),
             tile_start=view(self.geom, lay.tile_start, torch.int32, vt * tiles, (vt, tiles)),
             keys=view(self.binning, lay.keys, torch.int64, n, (n,)),
-            final_T=view(self.image, lay.final_T, torch.float32, vt * d.height * d.width,
-                         (vt, d.height, d.width)),
-            n_contrib=view(self.image, lay.n_contrib, torch.int32, vt * d.height * d.width,
-                           (vt, d.height, d.width)),
+            final_T=view(self.image, lay.final_T, torch.float32, vt * hw, (vt, d.height, d.width)),
+            n_contrib=view(self.image, lay.n_contrib, torch.int32, vt * hw, (vt, d.height, d.width)),
+            color=view(self.image, lay.color, torch.float32, vt * 3 * hw, (vt, 3, d.height, d.width)),
+            # (T, Cr, Cg, Cb) in front of list runs 1..3; written only when the forward cut lists into runs
+            run_state=view(self.image, lay.run_state, torch.float32, vt * 3 * hw * 4, (vt, 3, d.height, d.width, 4)),
             num_instances=n,
         )
 

@@ -80,6 +80,35 @@ def test_sizes_layout_and_validation_without_gpu():
     assert rc == 1 and b"NULL" in _lib.lib.ps_last_error()
 
 
+def test_hit_list_option_without_gpu():
+    """ps_set_option("composite_hit_lists", 0 | 1 | 2) decides whether the binning state holds the forward's hit
+    lists: 2 (automatic) keeps them while 64 bytes x capacity <= 512 MB; other values are rejected."""
+    from pixelsplat_b200 import _lib
+    small = _lib.RasterDesc(1, 1, 1000, 25, 4, 0, 0, 256, 256, 0, 0, 100_000)
+    big = _lib.RasterDesc(1, 1, 1000, 25, 4, 0, 0, 256, 256, 0, 0, (512 << 20) // 64 + 1)
+    try:
+        for bad in (-1, 3, 4):
+            with pytest.raises(ValueError, match="PS_ERR_INVALID_ARGUMENT.*unknown option or bad value: "
+                                                 f"composite_hit_lists = {bad}"):
+                _lib.set_option("composite_hit_lists", bad)
+        binning, hits = {}, {}
+        for v in (0, 1, 2):
+            _lib.set_option("composite_hit_lists", v)
+            binning[v] = {n: _lib.sizes(d).binning_bytes for n, d in (("small", small), ("big", big))}
+            hits[v] = {n: _lib.layout(d).block_hits for n, d in (("small", small), ("big", big))}
+        assert binning[0]["small"] < binning[1]["small"] == binning[2]["small"]
+        assert binning[0]["big"] == binning[2]["big"] < binning[1]["big"]
+        assert binning[1]["small"] - binning[0]["small"] >= 100_000 * 64
+        assert hits[0] == {"small": 0, "big": 0} and hits[2]["small"] != 0 and hits[2]["big"] == 0
+        assert hits[1]["small"] != 0 and hits[1]["big"] != 0
+        _lib.set_option("composite_impl", 1)          # the legacy compositor never keeps them
+        assert _lib.layout(small).block_hits == 0
+    finally:
+        _lib.set_option("composite_impl", 2)
+        _lib.set_option("composite_hit_lists", 2)
+    assert _lib.layout(small).block_hits != 0
+
+
 def test_no_cpu_fallback():
     """CPU tensors are rejected; a missing library is an ImportError, not a silent fallback."""
     from pixelsplat_b200.rasterizer import rasterize_gaussians

@@ -16,8 +16,26 @@ def _decoder():
                                 type("D", (), {"background_color": [0.1, 0.0, 0.2]})()).to(DEV)
 
 
+# the warp-task compositor variants: (composite_impl, composite_segments, composite_hit_lists)
+VARIANTS = {"k1": (2, 1, 1), "k1-nohl": (2, 1, 0), "k2": (2, 2, 1), "k2-nohl": (2, 2, 0), "k4": (2, 4, 1),
+            "k4-nohl": (2, 4, 0)}
+
+
 @pytest.mark.parametrize("hw,views", [((64, 64), 1), ((48, 80), 3), ((256, 256), 4)])
 def test_fused_mse_and_psnr_equal_the_unfused_route(hw, views):
+    """The compositor variant the shape selects automatically."""
+    _fused_equals_unfused(hw, views)
+
+
+@pytest.mark.parametrize("variant", list(VARIANTS))
+def test_fused_mse_and_psnr_equal_the_unfused_route_under_every_variant(variant):
+    """The (48, 80) x 3 case with each warp-task variant forced; both routes run under the same variant."""
+    from tests import util
+    with util.composite_variant(*VARIANTS[variant]):
+        _fused_equals_unfused((48, 80), 3)
+
+
+def _fused_equals_unfused(hw, views):
     from pixelsplat_b200 import loss as L
     from pixelsplat_b200.decoder import Gaussians
     S = 2
@@ -67,6 +85,28 @@ def test_fused_mse_and_psnr_equal_the_unfused_route(hw, views):
     (((out_e.color - target) ** 2).sum(dim=(2, 3, 4)) * wv).sum().backward()
     assert (gd.means.grad - ge.means.grad).norm() <= 2e-5 * ge.means.grad.norm()
     assert (gd.harmonics.grad - ge.harmonics.grad).norm() <= 2e-5 * ge.harmonics.grad.norm()
+
+
+def test_fused_gradients_agree_across_list_runs():
+    """The fused loss's gradients with K = 2 list runs per task against K = 1 (one warp walks the whole list)."""
+    from pixelsplat_b200.decoder import Gaussians
+    from tests import util
+    S, views, hw = 2, 3, (48, 80)
+    scs = [synthetic.scene_re10k_like(seed=70 + i, image_hw=(32, 32), target_views=views) for i in range(S)]
+    st = lambda name: torch.stack([getattr(s, name).to(DEV) for s in scs])
+    cams = (st("extrinsics"), st("intrinsics"), st("near"), st("far"), hw)
+    target = (torch.rand((S, views, 3, *hw), generator=torch.Generator().manual_seed(3)) * 1.4 - 0.2).to(DEV)
+    dec = _decoder()
+    grads = {}
+    for K in (1, 2):
+        g = Gaussians(st("means").requires_grad_(True), st("covariances").requires_grad_(True),
+                      st("harmonics").requires_grad_(True), st("opacities").requires_grad_(True))
+        with util.composite_variant(2, K, 2):
+            _, sse, _ = dec.forward_mse(g, *cams, target)
+            sse.sum().backward()
+        grads[K] = {n: getattr(g, n).grad for n in ("means", "covariances", "harmonics", "opacities")}
+    for n, a in grads[1].items():
+        assert (grads[2][n] - a).norm() <= 1e-4 * a.norm(), n
 
 
 def test_legacy_compositor_rejects_the_loss_epilogue():
