@@ -75,8 +75,18 @@ typedef struct ps_raster_desc {
     int64_t instance_capacity; /* room, in (tile,Gaussian) instances, summed over all S*V views */
     /* appended in round 2 (struct grows at the end only) */
     int32_t sh_basis;        /* PS_SH_BASIS_*: the convention the SH coefficients are evaluated in    */
-    int32_t reserved;        /* must be 0                                                      */
+    int32_t depth_mode;      /* PS_DEPTH_*: also composite a depth channel (0 = colour only)    */
 } ps_raster_desc;
+
+/* depth_mode: the per-(view, Gaussian) value d composited into the depth image sum_i w_i d_i (background 0, no
+ * clamp) with the colour pass's alphas, from z = the camera-space depth in WORLD units (view-space z / scene_scale);
+ * the "colour" render_depth_cuda composites (/root/reference/src/model/decoder/cuda_splatting.py:238-251).
+ * near / far are ps_raster_inputs.near_far (world units), eps = 1e-10. */
+#define PS_DEPTH_NONE 0
+#define PS_DEPTH_Z 1                 /* d = z                                                                */
+#define PS_DEPTH_DISPARITY 2         /* d = 1 / z                                                            */
+#define PS_DEPTH_RELATIVE_DISPARITY 3 /* d = 1 - (1/(z+eps) - 1/(far+eps)) / (1/(near+eps) - 1/(far+eps) + eps) */
+#define PS_DEPTH_LOG 4               /* d = log(max(min(z, near), far)), as the reference writes it         */
 
 /* Per-call inputs. Camera arrays are indexed by flat view id  vid = scene * V + view. */
 typedef struct ps_raster_inputs {
@@ -91,6 +101,9 @@ typedef struct ps_raster_inputs {
     const float *background; /* [S*V, 3]                                                       */
     const float *scene_scale; /* [S*V] or NULL: means*=s, cov*=s*s before use -- the
                                  scale_invariant rescale of cuda_splatting.py:64-71, fused     */
+    /* appended with depth_mode */
+    const float *near_far;    /* [S*V, 2] (near, far) in world units; required for PS_DEPTH_RELATIVE_DISPARITY
+                                 and PS_DEPTH_LOG, unused otherwise (may be NULL)               */
 } ps_raster_inputs;
 
 /* Opaque state that lives from forward to backward (the analogue of upstream's geomBuffer /
@@ -139,6 +152,9 @@ typedef struct ps_raster_layout {
     size_t run_hits;      /* binning: u32 [S*V*tiles*8*4] their lengths                                        */
     size_t run_state;     /* image: f32x4 [S*V*3*H*W] (T, Cr, Cg, Cb) in front of list runs 1..3 when the
                              compositor cuts a tile's list into runs (small batches)            */
+    /* appended with depth_mode (both 0 and not allocated when depth_mode == 0) */
+    size_t depth_image;   /* image: f32 [S*V*H*W] the composited depth channel                                  */
+    size_t run_depth;     /* image: f32 [S*V*3*H*W] depth in front of list runs 1..3 (next to run_state)        */
 } ps_raster_layout;
 
 typedef struct ps_raster_grads {
@@ -169,6 +185,9 @@ PS_API int ps_timing_read(float *ms);
  * the options are unchanged in between).  Also read once from PIXELSPLAT_B200_COMPOSITE / PIXELSPLAT_B200_SEGMENTS /
  * PIXELSPLAT_B200_HIT_LISTS. */
 PS_API int ps_set_option(const char *name, int value);
+/* The value of an option above as it is in force (the environment included): composite_impl 1 | 2,
+ * composite_segments 0 | 1 | 2 | 4, composite_hit_lists 0 | 1 | 2. */
+PS_API int ps_get_option(const char *name, int *value);
 
 /* Workspace sizes / layout for a descriptor. */
 PS_API int ps_raster_sizes_query(const ps_raster_desc *desc, ps_raster_sizes *out);
@@ -211,6 +230,20 @@ PS_API int ps_raster_backward(const ps_raster_desc *desc, const ps_raster_inputs
                        const ps_raster_state *state, const float *d_color /* [S*V,3,H,W] */,
                        void *scratch, size_t scratch_bytes, const ps_raster_grads *grads,
                        void *stream);
+
+/* With desc->depth_mode != 0, ps_raster_forward / ps_raster_forward_loss also composite the depth channel into
+ * the image state (ps_raster_layout.depth_image; the colour, radii and every other output are unchanged).  The
+ * legacy compositor (composite_impl = 1) has no depth channel: PS_ERR_UNSUPPORTED before anything is enqueued.
+ * ps_raster_backward / ps_raster_backward_loss after such a forward take dL/dD = 0. */
+
+/* Backward of a depth forward with a depth gradient d_depth [S*V, H, W]: dL/dD reaches the Gaussians through the
+ * alphas and through d (the means, summed over the V views).  d_color [S*V, 3, H, W], or NULL: then dL/dC comes
+ * from the fused loss as in ps_raster_backward_loss (loss_target, grad_scale). */
+PS_API int ps_raster_backward_depth(const ps_raster_desc *desc, const ps_raster_inputs *in,
+                                    const ps_raster_state *state, const float *d_color /* or NULL */,
+                                    const float *loss_target, const float *grad_scale, const float *d_depth,
+                                    void *scratch, size_t scratch_bytes, const ps_raster_grads *grads,
+                                    void *stream);
 
 /* ---- fused loss epilogue (SURVEY.md 8 row f-4) --------------------------------------------------
  * The training loss the reference applies to the render, LossMse (/root/reference/src/loss/loss_mse.py:30-31,

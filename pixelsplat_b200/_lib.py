@@ -16,6 +16,9 @@ PS_OK = 0
 PS_SH_M3, PS_SH_3M = 0, 1
 PS_COV_TRIU6, PS_COV_3X3 = 0, 1
 PS_SH_BASIS_3DGS, PS_SH_BASIS_E3NN = 0, 1
+PS_ERR_UNSUPPORTED = 3
+# ps_raster_desc.depth_mode
+DEPTH_MODES = {None: 0, "depth": 1, "disparity": 2, "relative_disparity": 3, "log": 4}
 TILE = 16
 
 _ERR_NAMES = {1: "PS_ERR_INVALID_ARGUMENT", 2: "PS_ERR_CUDA", 3: "PS_ERR_UNSUPPORTED"}
@@ -29,14 +32,14 @@ class RasterDesc(ctypes.Structure):
         ("cov_layout", ctypes.c_int32), ("height", ctypes.c_int32), ("width", ctypes.c_int32),
         ("sort_impl", ctypes.c_int32), ("sort_segment_hint", ctypes.c_int32),
         ("instance_capacity", ctypes.c_int64),
-        ("sh_basis", ctypes.c_int32), ("reserved", ctypes.c_int32),
+        ("sh_basis", ctypes.c_int32), ("depth_mode", ctypes.c_int32),
     ]
 
 
 class RasterInputs(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in (
         "means", "cov", "opacities", "sh", "viewmatrix", "projmatrix", "campos", "tanfov",
-        "background", "scene_scale")]
+        "background", "scene_scale", "near_far")]
 
 
 class RasterState(ctypes.Structure):
@@ -54,7 +57,7 @@ class RasterLayout(ctypes.Structure):
     _fields_ = [(n, ctypes.c_size_t) for n in (
         "depth", "radii", "xy", "conic_opacity", "rgb", "rect", "clamped", "tile_count",
         "tile_start", "tile_cursor", "n_instances", "vis_pairs", "vis_any", "keys", "keys_alt", "final_T",
-        "n_contrib", "cull", "color", "block_hits", "run_hits", "run_state")]
+        "n_contrib", "cull", "color", "block_hits", "run_hits", "run_state", "depth_image", "run_depth")]
 
 
 class EpipolarDesc(ctypes.Structure):
@@ -97,7 +100,8 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_epipolar_attention_forward", "ps_epipolar_attention_backward",
            "ps_self_attention_forward", "ps_gaussian_adapter_forward", "ps_gaussian_adapter_backward",
            "ps_sh_rotation_matrices", "ps_set_option", "ps_raster_forward_loss", "ps_raster_backward_loss",
-           "ps_self_attention_forward_stats", "ps_self_attention_backward")
+           "ps_self_attention_forward_stats", "ps_self_attention_backward", "ps_get_option",
+           "ps_raster_backward_depth")
 
 
 class NativeLibraryMissing(ImportError):
@@ -124,6 +128,9 @@ def _load() -> ctypes.CDLL:
     lib.ps_raster_backward_loss.argtypes = [P(RasterDesc), P(RasterInputs), P(RasterState), ctypes.c_void_p,
                                             ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, P(RasterGrads),
                                             ctypes.c_void_p]
+    lib.ps_raster_backward_depth.argtypes = [P(RasterDesc), P(RasterInputs), P(RasterState)] + [ctypes.c_void_p] * 5 + \
+        [ctypes.c_size_t, P(RasterGrads), ctypes.c_void_p]
+    lib.ps_raster_backward_depth.restype = ctypes.c_int
     lib.ps_raster_forward_loss.restype = ctypes.c_int
     lib.ps_raster_backward_loss.restype = ctypes.c_int
     lib.ps_camera_setup.argtypes = [ctypes.c_int32] + [ctypes.c_void_p] * 4 + [ctypes.c_int32] + \
@@ -157,6 +164,8 @@ def _load() -> ctypes.CDLL:
     lib.ps_sh_rotation_matrices.restype = ctypes.c_int
     lib.ps_set_option.argtypes = [ctypes.c_char_p, ctypes.c_int]
     lib.ps_set_option.restype = ctypes.c_int
+    lib.ps_get_option.argtypes = [ctypes.c_char_p, ctypes.POINTER(ctypes.c_int)]
+    lib.ps_get_option.restype = ctypes.c_int
     for f in ("ps_raster_sizes_query", "ps_raster_layout_query", "ps_raster_forward", "ps_raster_backward"):
         getattr(lib, f).restype = ctypes.c_int
     return lib
@@ -187,6 +196,13 @@ def on_device(device, fn, *args) -> int:
 
 def set_option(name: str, value: int) -> None:
     check(lib.ps_set_option(name.encode(), int(value)), "ps_set_option")
+
+
+def get_option(name: str) -> int:
+    """The value of a compositor option in force (set through set_option or the environment)."""
+    v = ctypes.c_int()
+    check(lib.ps_get_option(name.encode(), ctypes.byref(v)), "ps_get_option")
+    return v.value
 
 
 def sizes(desc: RasterDesc) -> RasterSizes:

@@ -34,6 +34,8 @@ struct ImageState {
     uint32_t *n_contrib;      // [S*V*H*W]
     float *color;             // [S*V*3*H*W] copy of the rendered colour (backward's forward-order prefix form)
     float4 *run_state;        // [S*V*(kMaxSegments-1)*H*W] (T, Cr, Cg, Cb) in front of list runs 1.. (segK > 1)
+    float *depth_image;       // [S*V*H*W] composited depth channel (depth_mode != 0, else null)
+    float *run_depth;         // [S*V*(kMaxSegments-1)*H*W] depth in front of list runs 1.. (depth_mode != 0)
 };
 
 // Fused loss epilogue of the compositor (SURVEY.md 8 row f-4): squared error against a target image summed per
@@ -57,19 +59,57 @@ struct HitLists {
 
 struct Dims {
     int S, V, P, M, deg, sh_layout, cov_layout, H, W, gx, gy, tiles, sh_basis, segK, hit_lists;
+    int depth_mode;           // PS_DEPTH_*; in a backward, 0 unless a depth gradient is given
     long long capacity;
 };
 
 struct Inputs {
     const float *means, *cov, *opac, *sh, *view, *proj, *campos, *tanfov, *bg, *scale;
+    const float *near_far;    // [S*V, 2] world units (depth modes 3, 4)
 };
 
 // Per-(view,Gaussian) gradient scratch written by the composite backward.
 struct ViewGrads {
     float2 *d_mean2d;  // NDC-scaled like upstream (x * 0.5 W, y * 0.5 H)
     float4 *d_conic;   // x, y (half-weighted B), z, w = d_opacity
-    float4 *d_color;   // r, g, b, unused
+    float4 *d_color;   // r, g, b, depth value d (the latter only with a depth gradient)
 };
+
+// Depth channel (PS_DEPTH_*): the value d composited for a Gaussian at view-space depth vz of a view whose
+// scene_scale is `sc` (null scale = 1).  z = vz / sc is the depth in world units.  Compiled into the preprocess
+// (--fmad=false, both producers of d give the same bits) and the preprocess backward (depth_value_grad).
+constexpr float kDepthEps = 1e-10f;
+
+__device__ __forceinline__ float depth_value(int mode, float vz, const float *scale, const float *near_far, int vid) {
+    const float z = scale ? vz / scale[vid] : vz;
+    if (mode == PS_DEPTH_DISPARITY) return 1.0f / z;
+    if (mode == PS_DEPTH_RELATIVE_DISPARITY) {
+        const float dn = 1.0f / (near_far[2 * vid] + kDepthEps), df = 1.0f / (near_far[2 * vid + 1] + kDepthEps);
+        return 1.0f - (1.0f / (z + kDepthEps) - df) / (dn - df + kDepthEps);
+    }
+    if (mode == PS_DEPTH_LOG) return logf(fmaxf(fminf(z, near_far[2 * vid]), near_far[2 * vid + 1]));
+    return z;
+}
+
+// dd/dz of depth_value.  The log mode follows torch's minimum / maximum backward (a tie splits the gradient in
+// half): for near < far, max(min(z, near), far) = far and the derivative is 0, as in the reference.
+__device__ __forceinline__ float depth_value_grad(int mode, float vz, const float *scale, const float *near_far, int vid) {
+    const float z = scale ? vz / scale[vid] : vz;
+    if (mode == PS_DEPTH_DISPARITY) return -1.0f / (z * z);
+    if (mode == PS_DEPTH_RELATIVE_DISPARITY) {
+        const float dn = 1.0f / (near_far[2 * vid] + kDepthEps), df = 1.0f / (near_far[2 * vid + 1] + kDepthEps);
+        const float iz = 1.0f / (z + kDepthEps);
+        return iz * iz / (dn - df + kDepthEps);
+    }
+    if (mode == PS_DEPTH_LOG) {
+        const float nr = near_far[2 * vid], fr = near_far[2 * vid + 1];
+        const float m = fminf(z, nr);
+        const float gm = z < nr ? 1.0f : (z == nr ? 0.5f : 0.0f);
+        const float gr = m > fr ? 1.0f : (m == fr ? 0.5f : 0.0f);
+        return gm * gr / fmaxf(m, fr);
+    }
+    return 1.0f;
+}
 
 // Half-extents (pixels) of the axis-aligned box outside of which a splat's alpha is certainly
 // < 1/255: alpha = o exp(-0.5 d^T Sigma^-1 d) >= 1/255  <=>  d^T Sigma^-1 d <= 2 ln(255 o), whose bounding
@@ -128,8 +168,8 @@ int launch_composite_forward(const Dims &d, const Inputs &in, const Geom &g,
                              float *out_color, const LossEpilogue &loss, const HitLists &hl, cudaStream_t st);
 int launch_composite_backward(const Dims &d, const Inputs &in, const Geom &g,
                               const unsigned long long *keys, const ImageState &img,
-                              const float *d_color, const ViewGrads &vg, const LossEpilogue &loss, const HitLists &hl,
-                              cudaStream_t st);
+                              const float *d_color, const float *d_depth, const ViewGrads &vg,
+                              const LossEpilogue &loss, const HitLists &hl, cudaStream_t st);
 // legacy CTA-per-tile compositor (round 1), kept selectable for A/B measurements
 int launch_composite_forward_v1(const Dims &d, const Inputs &in, const Geom &g,
                                 const unsigned long long *keys, const ImageState &img,
@@ -140,8 +180,9 @@ int launch_composite_backward_v1(const Dims &d, const Inputs &in, const Geom &g,
 int composite_impl();   // 1 = legacy, 2 = warp-task compositor (env PIXELSPLAT_B200_COMPOSITE, default 2)
 int set_composite_option(int which, int value);   // 0: impl (1 | 2), 1: segments (0 = auto | 1 | 2 | 4),
                                                   // 2: hit lists (0 = never | 1 = always | 2 = auto)
+int get_composite_option(int which);              // the value in force (environment included)
 int composite_segments(long long tasks);
-bool composite_hit_lists(long long capacity);      // keep the forward's hit lists for the backward?   // list runs per task (1, 2, 4) for a batch of `tasks` warp tasks
+bool composite_hit_lists(long long capacity);      // keep the forward's hit lists for the backward?
 int launch_preprocess_backward(const Dims &d, const Inputs &in, const Geom &g, const ViewGrads &vg,
                                const ps_raster_grads &out, cudaStream_t st);
 int launch_gradient_fill(const Dims &d, const ps_raster_grads &out, cudaStream_t st);

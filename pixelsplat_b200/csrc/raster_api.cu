@@ -97,7 +97,7 @@ static int validate(const ps_raster_desc *d) {
     }
     if (d->sh_layout != PS_SH_M3 && d->sh_layout != PS_SH_3M) { set_error("bad sh_layout %d", d->sh_layout); return PS_ERR_INVALID_ARGUMENT; }
     if (d->sh_basis != PS_SH_BASIS_3DGS && d->sh_basis != PS_SH_BASIS_E3NN) { set_error("bad sh_basis %d", d->sh_basis); return PS_ERR_INVALID_ARGUMENT; }
-    if (d->reserved != 0) { set_error("ps_raster_desc.reserved must be 0 (got %d): caller built against an older header?", d->reserved); return PS_ERR_INVALID_ARGUMENT; }
+    if (d->depth_mode < PS_DEPTH_NONE || d->depth_mode > PS_DEPTH_LOG) { set_error("bad depth_mode %d (PS_DEPTH_*: 0..4)", d->depth_mode); return PS_ERR_INVALID_ARGUMENT; }
     if (d->cov_layout != PS_COV_TRIU6 && d->cov_layout != PS_COV_3X3) { set_error("bad cov_layout %d", d->cov_layout); return PS_ERR_INVALID_ARGUMENT; }
     if (d->instance_capacity < 1 || d->instance_capacity > 0x7fffffffll) {
         set_error("instance_capacity must be in [1, 2^31-1], got %lld", (long long)d->instance_capacity);
@@ -128,6 +128,7 @@ static Dims make_dims(const ps_raster_desc *d) {
     r.sh_basis = d->sh_basis;
     r.segK = composite_segments((long long)r.S * r.V * r.tiles * 8);
     r.hit_lists = composite_hit_lists(r.capacity) ? 1 : 0;
+    r.depth_mode = d->depth_mode;
     return r;
 }
 
@@ -170,6 +171,11 @@ static Layout make_layout(const ps_raster_desc *d) {
     L.off.n_contrib = take(px * 4);
     L.off.color = take(px * 12);
     L.off.run_state = take(px * 16 * (kMaxSegments - 1));
+    L.off.depth_image = L.off.run_depth = 0;
+    if (m.depth_mode) {
+        L.off.depth_image = take(px * 4);
+        L.off.run_depth = take(px * 4 * (kMaxSegments - 1));
+    }
     L.sizes.image_bytes = o;
     // backward scratch: d_mean2d (8) + d_conic (16) + d_color (16) per (view, Gaussian)
     L.sizes.backward_bytes = align_up(vp * 8) + align_up(vp * 16) + align_up(vp * 16);
@@ -203,6 +209,8 @@ static ImageState make_image(const Layout &L, void *image) {
     im.n_contrib = reinterpret_cast<uint32_t *>(b + L.off.n_contrib);
     im.color = reinterpret_cast<float *>(b + L.off.color);
     im.run_state = reinterpret_cast<float4 *>(b + L.off.run_state);
+    im.depth_image = L.off.depth_image ? reinterpret_cast<float *>(b + L.off.depth_image) : nullptr;
+    im.run_depth = L.off.run_depth ? reinterpret_cast<float *>(b + L.off.run_depth) : nullptr;
     return im;
 }
 
@@ -226,7 +234,14 @@ static int check_common(const ps_raster_desc *desc, const ps_raster_inputs *in, 
         set_error("state buffers must be 16-byte aligned");
         return PS_ERR_INVALID_ARGUMENT;
     }
-    (void)desc;
+    if ((desc->depth_mode == PS_DEPTH_RELATIVE_DISPARITY || desc->depth_mode == PS_DEPTH_LOG) && !in->near_far) {
+        set_error("depth_mode %d needs ps_raster_inputs.near_far", desc->depth_mode);
+        return PS_ERR_INVALID_ARGUMENT;
+    }
+    if (desc->depth_mode && composite_impl() == 1) {
+        set_error("the legacy compositor (composite_impl = 1) has no depth channel");
+        return PS_ERR_UNSUPPORTED;
+    }
     return PS_OK;
 }
 
@@ -234,7 +249,7 @@ static Inputs make_inputs(const ps_raster_inputs *in) {
     Inputs r;
     r.means = in->means; r.cov = in->cov; r.opac = in->opacities; r.sh = in->sh;
     r.view = in->viewmatrix; r.proj = in->projmatrix; r.campos = in->campos; r.tanfov = in->tanfov;
-    r.bg = in->background; r.scale = in->scene_scale;
+    r.bg = in->background; r.scale = in->scene_scale; r.near_far = in->near_far;
     return r;
 }
 
@@ -273,6 +288,17 @@ PS_API int ps_set_option(const char *name, int value) {
     else if (!strcmp(name, "composite_hit_lists")) rc = set_composite_option(2, value);
     if (rc) set_error("ps_set_option: unknown option or bad value: %s = %d", name, value);
     return rc;
+}
+
+PS_API int ps_get_option(const char *name, int *value) {
+    if (!name || !value) { set_error("ps_get_option: name / value is NULL"); return PS_ERR_INVALID_ARGUMENT; }
+    int which = -1;
+    if (!strcmp(name, "composite_impl")) which = 0;
+    else if (!strcmp(name, "composite_segments")) which = 1;
+    else if (!strcmp(name, "composite_hit_lists")) which = 2;
+    if (which < 0) { set_error("ps_get_option: unknown option %s", name); return PS_ERR_INVALID_ARGUMENT; }
+    *value = get_composite_option(which);
+    return PS_OK;
 }
 
 PS_API int ps_raster_sizes_query(const ps_raster_desc *desc, ps_raster_sizes *out) {
@@ -366,8 +392,9 @@ PS_API int ps_raster_forward_loss(const ps_raster_desc *desc, const ps_raster_in
 }  // extern "C"
 
 static int raster_backward_impl(const ps_raster_desc *desc, const ps_raster_inputs *in, const ps_raster_state *state,
-                                const float *d_color, const float *target, const float *grad_scale, void *scratch,
-                                size_t scratch_bytes, const ps_raster_grads *grads, void *stream) {
+                                const float *d_color, const float *target, const float *grad_scale,
+                                const float *d_depth, void *scratch, size_t scratch_bytes,
+                                const ps_raster_grads *grads, void *stream) {
     int rc = validate(desc);
     if (rc) return rc;
     const Layout L = make_layout(desc);
@@ -387,7 +414,8 @@ static int raster_backward_impl(const ps_raster_desc *desc, const ps_raster_inpu
         return PS_ERR_INVALID_ARGUMENT;
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const Dims d = make_dims(desc);
+    Dims d = make_dims(desc);
+    if (!d_depth) d.depth_mode = 0;     // no depth gradient: the colour-only kernels, dL/dD = 0
     const Inputs I = make_inputs(in);
     const Geom g = make_geom(L, state->geom);
     const unsigned long long *keys = reinterpret_cast<const unsigned long long *>(static_cast<char *>(state->binning) + L.off.keys);
@@ -414,7 +442,7 @@ static int raster_backward_impl(const ps_raster_desc *desc, const ps_raster_inpu
         hl.hits = reinterpret_cast<uint2 *>(static_cast<char *>(state->binning) + L.off.block_hits);
         hl.run_hits = reinterpret_cast<uint32_t *>(static_cast<char *>(state->binning) + L.off.run_hits);
     }
-    if ((rc = launch_composite_backward(d, I, g, keys, img, d_color, vg, le, hl, st))) return rc;
+    if ((rc = launch_composite_backward(d, I, g, keys, img, d_color, d_depth, vg, le, hl, st))) return rc;
     mark(kMarkCompositeBwd, st);
     PS_CUDA_CHECK(cudaStreamWaitEvent(st, sc->join, 0));   // join
     if ((rc = launch_preprocess_backward(d, I, g, vg, *grads, st))) return rc;
@@ -428,14 +456,30 @@ PS_API int ps_raster_backward(const ps_raster_desc *desc, const ps_raster_inputs
                               const float *d_color, void *scratch, size_t scratch_bytes,
                               const ps_raster_grads *grads, void *stream) {
     if (!d_color) { set_error("d_color is NULL"); return PS_ERR_INVALID_ARGUMENT; }
-    return raster_backward_impl(desc, in, state, d_color, nullptr, nullptr, scratch, scratch_bytes, grads, stream);
+    return raster_backward_impl(desc, in, state, d_color, nullptr, nullptr, nullptr, scratch, scratch_bytes, grads,
+                                stream);
 }
 
 PS_API int ps_raster_backward_loss(const ps_raster_desc *desc, const ps_raster_inputs *in, const ps_raster_state *state,
                                    const float *target, const float *grad_scale, void *scratch, size_t scratch_bytes,
                                    const ps_raster_grads *grads, void *stream) {
     if (!target || !grad_scale) { set_error("target / grad_scale is NULL"); return PS_ERR_INVALID_ARGUMENT; }
-    return raster_backward_impl(desc, in, state, nullptr, target, grad_scale, scratch, scratch_bytes, grads, stream);
+    return raster_backward_impl(desc, in, state, nullptr, target, grad_scale, nullptr, scratch, scratch_bytes, grads,
+                                stream);
+}
+
+PS_API int ps_raster_backward_depth(const ps_raster_desc *desc, const ps_raster_inputs *in, const ps_raster_state *state,
+                                    const float *d_color, const float *loss_target, const float *grad_scale,
+                                    const float *d_depth, void *scratch, size_t scratch_bytes,
+                                    const ps_raster_grads *grads, void *stream) {
+    if (!d_depth) { set_error("d_depth is NULL"); return PS_ERR_INVALID_ARGUMENT; }
+    if (desc && desc->depth_mode == PS_DEPTH_NONE) {
+        set_error("ps_raster_backward_depth needs the depth_mode of a depth forward (got 0)");
+        return PS_ERR_INVALID_ARGUMENT;
+    }
+    if (!d_color && !(loss_target && grad_scale)) { set_error("d_color, or loss_target + grad_scale, is NULL"); return PS_ERR_INVALID_ARGUMENT; }
+    return raster_backward_impl(desc, in, state, d_color, d_color ? nullptr : loss_target, d_color ? nullptr : grad_scale,
+                                d_depth, scratch, scratch_bytes, grads, stream);
 }
 
 }  // extern "C"

@@ -86,7 +86,7 @@ __device__ __forceinline__ void red_add_v2(float2 *addr, float a, float b) {
 struct HitQueue {
     float4 r0[kQ];   // A, B, C, opacity
     float4 r1[kQ];   // qa, qb, qc, list position (bits)
-    float4 r2[kQ];   // r, g, b, Gaussian id (bits)
+    float4 r2[kQ];   // r, g, b, Gaussian id (bits) -- forward with a depth channel: r, g, b, depth value d
 };
 
 // log2 of the Gaussian falloff at block-local pixel (fi, fj)
@@ -168,8 +168,11 @@ __device__ __forceinline__ void cull_prologue(CullPipe &p, const Geom &geo, cons
 
 // Parks the hit found in the previous iteration (its gathers have had a whole iteration to land): forms the
 // polynomial coefficients of the hit about the block origin.  D0 = also keep (dx0, dy0) for the backward.
-template <bool D0>
-__device__ __forceinline__ void cull_park(CullPipe &p, HitQueue &q, float2 *d0, const TaskGeom &t) {
+// DEPTH: the forward carries the depth value in r2.w instead of the id (it never reads the id); the backward keeps
+// the id there and parks the depth value in dd[].
+template <bool D0, bool DEPTH = false>
+__device__ __forceinline__ void cull_park(CullPipe &p, HitQueue &q, float2 *d0, const TaskGeom &t,
+                                          float *dd = nullptr) {
     if (p.h_pending) {
         const float qa = -0.5f * kLog2e * p.h_co.x, qb = -kLog2e * p.h_co.y, qc = -0.5f * kLog2e * p.h_co.z;
         const float dx0 = p.h_xy.x - t.rx0, dy0 = p.h_xy.y - t.ry0;
@@ -179,21 +182,25 @@ __device__ __forceinline__ void cull_park(CullPipe &p, HitQueue &q, float2 *d0, 
         const float C = -(2.0f * cy + qb * dx0);
         q.r0[p.h_slot] = make_float4(A, B, C, p.h_co.w);
         q.r1[p.h_slot] = make_float4(qa, qb, qc, __uint_as_float(p.h_pos));
-        q.r2[p.h_slot] = make_float4(p.h_rgb.x, p.h_rgb.y, p.h_rgb.z, __uint_as_float(p.h_g));
+        q.r2[p.h_slot] = make_float4(p.h_rgb.x, p.h_rgb.y, p.h_rgb.z,
+                                     (DEPTH && !D0) ? p.h_rgb.w : __uint_as_float(p.h_g));
         if (D0) d0[p.h_slot] = make_float2(dx0, dy0);
+        if (D0 && DEPTH) dd[p.h_slot] = p.h_rgb.w;
     }
     p.h_pending = false;
     __syncwarp();
 }
 
-// Zero-opacity records up to the next multiple of four (they can never contribute: alpha = 0 < 1/255).
-__device__ __forceinline__ uint32_t queue_pad(HitQueue &q, uint32_t tail, int lane) {
+// Zero-opacity records up to the next multiple of four (they can never contribute: alpha = 0 < 1/255).  Their
+// colour (and depth value, dd) is zero too, so that a weight of zero never meets an uninitialised value.
+__device__ __forceinline__ uint32_t queue_pad(HitQueue &q, uint32_t tail, int lane, float *dd = nullptr) {
     const uint32_t padded = (tail + 3u) & ~3u;
     if ((uint32_t)lane < padded - tail) {
         const uint32_t slot = (tail + (uint32_t)lane) & (kQ - 1);
         q.r0[slot] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
         q.r1[slot] = make_float4(0.0f, 0.0f, 0.0f, __uint_as_float(0xffffffffu));   // position beyond any `last`
         q.r2[slot] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (dd) dd[slot] = 0.0f;
     }
     __syncwarp();
     return padded;
@@ -243,15 +250,18 @@ constexpr float kStopGuard = 1.01e-4f;     // a run is folded without replay onl
 
 struct FwdPixel {
     float T, Cr, Cg, Cb;
+    float D;            // depth channel (DEPTH instantiations only)
     uint32_t last;      // 1 + list position of the last blended entry (0 = none)
     bool done;          // no further blending for this lane (stopped, or outside the image / masked)
     bool stopped;       // the early-exit test fired
 };
 
-// Four queued hits (an aligned group) onto the lane's pixel, front to back.
+// Four queued hits (an aligned group) onto the lane's pixel, front to back.  DEPTH: D accumulates r2.w with the
+// colour's weights (an independent chain; the colour arithmetic is unchanged).
+template <bool DEPTH>
 __device__ __forceinline__ void fwd_blend4(const HitQueue &q, uint32_t base, const TaskGeom &t, float &T, float &Cr,
-                                           float &Cg, float &Cb, uint32_t &last, bool &done, bool &stopped) {
-    float pw[4], al[4];
+                                           float &Cg, float &Cb, float &D, uint32_t &last, bool &done, bool &stopped) {
+    float pw[4], al[4], dv[4];
     float3 col[4];
     uint32_t ps[4];
 #pragma unroll
@@ -260,6 +270,7 @@ __device__ __forceinline__ void fwd_blend4(const HitQueue &q, uint32_t base, con
         pw[k] = hit_power2(a0, a1, t.fi, t.fj);
         al[k] = fminf(0.99f, a0.w * fast_exp2(pw[k]));
         col[k] = make_float3(a2.x, a2.y, a2.z);
+        dv[k] = a2.w;
         ps[k] = __float_as_uint(a1.w);
     }
 #pragma unroll
@@ -270,6 +281,7 @@ __device__ __forceinline__ void fwd_blend4(const HitQueue &q, uint32_t base, con
         const bool blend = contrib && !stop;
         const float w = blend ? al[k] * T : 0.0f;
         Cr = fmaf(col[k].x, w, Cr); Cg = fmaf(col[k].y, w, Cg); Cb = fmaf(col[k].z, w, Cb);
+        if (DEPTH) D = fmaf(dv[k], w, D);
         T = blend ? test_T : T;
         last = blend ? ps[k] + 1u : last;
         done = done || stop;
@@ -278,10 +290,11 @@ __device__ __forceinline__ void fwd_blend4(const HitQueue &q, uint32_t base, con
 }
 
 // Front-to-back blend of the warp's run [t.run_begin, t.run_begin + t.run_len) onto the per-lane state px.
+template <bool DEPTH>
 __device__ __forceinline__ uint32_t fwd_run(const Geom &geo, const TaskGeom &t, const unsigned long long *__restrict__ keys,
                                             HitQueue &q, FwdPixel &px, int lane, uint2 *__restrict__ hit_out = nullptr) {
     const uint32_t n = t.run_len;
-    float T = px.T, Cr = px.Cr, Cg = px.Cg, Cb = px.Cb;
+    float T = px.T, Cr = px.Cr, Cg = px.Cg, Cb = px.Cb, D = px.D;
     uint32_t last = px.last;
     bool done = px.done, stopped = px.stopped;
     CullPipe p;
@@ -289,29 +302,32 @@ __device__ __forceinline__ uint32_t fwd_run(const Geom &geo, const TaskGeom &t, 
     uint32_t head = 0, tail = 0;
     const uint32_t nchunks = (n + 31u) >> 5;
     for (uint32_t c = 0; c <= nchunks; ++c) {          // one extra iteration drains the last parked hits
-        cull_park<false>(p, q, nullptr, t);
+        cull_park<false, DEPTH>(p, q, nullptr, t);
         uint32_t avail = tail;                         // parked so far
         if (c < nchunks) tail += (uint32_t)cull_step(p, geo, t, keys, n, c, tail, lane, hit_out);
         else avail = queue_pad(q, tail, lane);
         // whole groups of four (their power / exp evaluations are independent, only the transmittance chains)
         while (avail - head >= 4u) {
-            fwd_blend4(q, head & (kQ - 1), t, T, Cr, Cg, Cb, last, done, stopped);
+            fwd_blend4<DEPTH>(q, head & (kQ - 1), t, T, Cr, Cg, Cb, D, last, done, stopped);
             head += 4u;
         }
         if (__all_sync(0xffffffffu, done)) break;     // (hits beyond this point are behind every pixel's last contributor)
         __syncwarp();
     }
     __syncwarp();
-    px.T = T; px.Cr = Cr; px.Cg = Cg; px.Cb = Cb; px.last = last; px.done = done; px.stopped = stopped;
+    px.T = T; px.Cr = Cr; px.Cg = Cg; px.Cb = Cb; px.D = D; px.last = last; px.done = done; px.stopped = stopped;
     return tail;
 }
 
-template <int K>
-__global__ void __launch_bounds__(kFwdWarps * 32, PS_FWD_MIN_CTAS)
+// DEPTH instantiations carry one more accumulator through the same loop (and the fold of the K > 1 runs); they are
+// built for fewer resident CTAs (5, or 4 with runs) so that it does not spill.
+template <int K, bool DEPTH>
+__global__ void __launch_bounds__(kFwdWarps * 32, DEPTH ? (K > 1 ? 4 : 5) : PS_FWD_MIN_CTAS)
 k_composite_fwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsigned long long *__restrict__ keys,
                  ImageState img, float *__restrict__ out_color, LossEpilogue loss, HitLists hl) {
     __shared__ HitQueue s_q[kFwdWarps];
     __shared__ float4 s_ct[K > 1 ? kFwdWarps : 1][32];      // a run's (Cr, Cg, Cb, T)
+    __shared__ float s_d[K > 1 && DEPTH ? kFwdWarps : 1][32];   // its depth
     __shared__ uint32_t s_last[K > 1 ? kFwdWarps : 1][32];   // its last contributor | stopped << 31
     constexpr int kTasksPerCta = kFwdWarps / K;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -326,7 +342,7 @@ k_composite_fwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
     if (K > 1) run_bounds(count, K, run, t.run_begin, t.run_len);
 
     FwdPixel px;
-    px.T = 1.0f; px.Cr = px.Cg = px.Cb = 0.0f;
+    px.T = 1.0f; px.Cr = px.Cg = px.Cb = 0.0f; px.D = 0.0f;
     px.last = 0; px.stopped = false;
     px.done = !valid || !t.inside;
     if (valid) {
@@ -334,20 +350,23 @@ k_composite_fwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
         uint2 *hit_out = nullptr;
         if (hl.hits)   // this run's slice of the block's region (a run has at most run_len hits)
             hit_out = hl.hits + ((size_t)t.start * 8 + (size_t)(task & 7) * t.count + t.run_begin);
-        const uint32_t nh = fwd_run(geo, t, keys, q, px, lane, hit_out);
+        const uint32_t nh = fwd_run<DEPTH>(geo, t, keys, q, px, lane, hit_out);
         if (hl.run_hits && lane == 0) hl.run_hits[task * kMaxSegments + run] = nh;
     }
 
     if (K > 1) {
         s_ct[warp][lane] = make_float4(px.Cr, px.Cg, px.Cb, px.T);
+        if (DEPTH) s_d[warp][lane] = px.D;
         s_last[warp][lane] = px.last | (px.stopped ? 0x80000000u : 0u);
         __syncthreads();
         if (run != 0 || !valid) return;
         // fold the runs in list order; px is run 0's result, i.e. the exact sequential state after run 0
         for (int j = 1; j < K; ++j) {
-            if (t.inside)   // state in front of run j: what the backward's run j starts from
-                img.run_state[((size_t)t.vid * (kMaxSegments - 1) + (j - 1)) * t.hw + t.pix] =
-                    make_float4(px.T, px.Cr, px.Cg, px.Cb);
+            if (t.inside) {  // state in front of run j: what the backward's run j starts from
+                const size_t o = ((size_t)t.vid * (kMaxSegments - 1) + (j - 1)) * t.hw + t.pix;
+                img.run_state[o] = make_float4(px.T, px.Cr, px.Cg, px.Cb);
+                if (DEPTH) img.run_depth[o] = px.D;
+            }
             const float4 r = s_ct[warp + j][lane];
             const uint32_t rl = s_last[warp + j][lane];
             const bool replay = !px.done && ((rl >> 31) != 0u || px.T * r.w < kStopGuard);
@@ -357,11 +376,12 @@ k_composite_fwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
                 run_bounds(count, K, j, tj.run_begin, tj.run_len);
                 FwdPixel pj = px;
                 pj.done = px.done || !replay;
-                fwd_run(geo, tj, keys, q, pj, lane);
+                fwd_run<DEPTH>(geo, tj, keys, q, pj, lane);
                 if (replay) px = pj;
             }
             if (!replay && !px.done) {
                 px.Cr = fmaf(px.T, r.x, px.Cr); px.Cg = fmaf(px.T, r.y, px.Cg); px.Cb = fmaf(px.T, r.z, px.Cb);
+                if (DEPTH) px.D = fmaf(px.T, s_d[warp + j][lane], px.D);
                 px.T *= r.w;
                 const uint32_t r_last = rl & 0x7fffffffu;
                 px.last = r_last ? r_last : px.last;
@@ -375,6 +395,7 @@ k_composite_fwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
         const size_t o1 = (size_t)t.vid * t.hw + t.pix;
         img.final_T[o1] = px.T;
         img.n_contrib[o1] = px.last;
+        if (DEPTH) img.depth_image[o1] = px.D;     // background 0: nothing behind the last contributor
         const float *bg = bg_all + 3 * t.vid;
         const float r = px.Cr + px.T * bg[0], g = px.Cg + px.T * bg[1], b = px.Cb + px.T * bg[2];
         const size_t o3 = (size_t)t.vid * 3 * t.hw + t.pix;
@@ -413,23 +434,25 @@ static_assert(kBatch == 32 || kBatch == 16, "phase 2 maps lanes to (entry, pixel
 constexpr int kHalves = 32 / kBatch;    // lanes per entry in phase 2
 constexpr int kRowsPerLane = 4 / kHalves;   // pixel rows (of 8) each phase-2 lane sums
 
+template <bool DEPTH>
 struct BwdSmem {
     HitQueue q;
     float2 d0[kQ];                      // (dx0, dy0): the hit's centre relative to the block origin
     float su[kBatch][33];               // u = G dL/dalpha   [entry][pixel], +1 pad: conflict-free both ways
     float sw[kBatch][33];               // w = alpha T
-    float4 dp[32];                      // dL/dC of the block's pixels (r, g, b, -)
+    float4 dp[32];                      // dL/dC of the block's pixels (r, g, b, dL/dD)
+    float dd[DEPTH ? kQ : 1];           // depth value d of each queued hit (r2.w holds the id)
 };
 
 struct BwdPixel {
-    float dpr, dpg, dpb, Q, T, S;
+    float dpr, dpg, dpb, dpd, Q, T, S;  // dpd = dL/dD (DEPTH instantiations only)
     uint32_t last;
 };
 
 // Phase 1 + phase 2 for the queue entries [head, head + cnt), head a multiple of kBatch, cnt <= kBatch
 // (warp-uniform; entries up to the next multiple of four exist as zero-opacity padding).
-template <bool FULL>
-__device__ __forceinline__ void bwd_batch(BwdSmem &sm, BwdPixel &px, const TaskGeom &t, const ViewGrads &vg,
+template <bool FULL, bool DEPTH>
+__device__ __forceinline__ void bwd_batch(BwdSmem<DEPTH> &sm, BwdPixel &px, const TaskGeom &t, const ViewGrads &vg,
                                           uint32_t head, int cnt, float kx, float ky, int lane) {
     // ---- phase 1: lane = pixel, entries front to back
     const uint32_t base = head & (kQ - 1);
@@ -443,7 +466,8 @@ __device__ __forceinline__ void bwd_batch(BwdSmem &sm, BwdPixel &px, const TaskG
         const bool active = __float_as_uint(a1.w) < px.last && !(p2 > kPowerEps) && !(al < kAlphaMin);
         const float a = active ? al : 0.0f;
         const float Gs = active ? G : 0.0f;        // also keeps an overflowed exp2 out of 0 * inf
-        const float cdp = fmaf(a2.z, px.dpb, fmaf(a2.y, px.dpg, a2.x * px.dpr));
+        float cdp = fmaf(a2.z, px.dpb, fmaf(a2.y, px.dpg, a2.x * px.dpr));
+        if (DEPTH) cdp = fmaf(sm.dd[base + j], px.dpd, cdp);     // c . dL/dC + d dL/dD
         const float w = a * px.T;
         px.S = fmaf(w, cdp, px.S);
         const float om = 1.0f - a;
@@ -456,6 +480,7 @@ __device__ __forceinline__ void bwd_batch(BwdSmem &sm, BwdPixel &px, const TaskG
     // ---- phase 2: lane = (entry e, pixel half h); raw moments over the lane's rows, i / j literals
     const int e = lane & (kBatch - 1), h = lane / kBatch;
     float m00 = 0.0f, m10 = 0.0f, m01 = 0.0f, m20 = 0.0f, m11 = 0.0f, m02 = 0.0f, s_r = 0.0f, s_g = 0.0f, s_b = 0.0f;
+    float s_d = 0.0f;
 #pragma unroll
     for (int jr = 0; jr < kRowsPerLane; ++jr) {
 #pragma unroll
@@ -468,6 +493,7 @@ __device__ __forceinline__ void bwd_batch(BwdSmem &sm, BwdPixel &px, const TaskG
             if (jr) { m01 = fmaf(u, (float)jr, m01); m02 = fmaf(u, (float)(jr * jr), m02); }
             if (i && jr) m11 = fmaf(u, (float)(i * jr), m11);
             s_r = fmaf(w, dpp.x, s_r); s_g = fmaf(w, dpp.y, s_g); s_b = fmaf(w, dpp.z, s_b);
+            if (DEPTH) s_d = fmaf(w, dpp.w, s_d);
         }
     }
     // shift to the Gaussian's centre: dx = ca - i, dy = cb - jr, (ca, cb) = centre relative to this lane's first row
@@ -486,9 +512,10 @@ __device__ __forceinline__ void bwd_batch(BwdSmem &sm, BwdPixel &px, const TaskG
         s_xy += __shfl_xor_sync(0xffffffffu, s_xy, 16); s_yy += __shfl_xor_sync(0xffffffffu, s_yy, 16);
         s_r += __shfl_xor_sync(0xffffffffu, s_r, 16); s_g += __shfl_xor_sync(0xffffffffu, s_g, 16);
         s_b += __shfl_xor_sync(0xffffffffu, s_b, 16);
+        if (DEPTH) s_d += __shfl_xor_sync(0xffffffffu, s_d, 16);
     }
     const bool any = (s_u != 0.0f) | (s_x != 0.0f) | (s_y != 0.0f) | (s_xx != 0.0f) | (s_xy != 0.0f) |
-                     (s_yy != 0.0f) | (s_r != 0.0f) | (s_g != 0.0f) | (s_b != 0.0f);
+                     (s_yy != 0.0f) | (s_r != 0.0f) | (s_g != 0.0f) | (s_b != 0.0f) | (DEPTH && s_d != 0.0f);
     if (h == 0 && e < cnt && any) {
         const float4 b0 = sm.q.r0[slot], b1 = sm.q.r1[slot], b2 = sm.q.r2[slot];
         const float o = b0.w;
@@ -497,27 +524,29 @@ __device__ __forceinline__ void bwd_batch(BwdSmem &sm, BwdPixel &px, const TaskG
         const float ox = o * s_x, oy = o * s_y;
         red_add_v2(vg.d_mean2d + rec, kx * (2.0f * b1.x * ox + b1.y * oy), ky * (2.0f * b1.z * oy + b1.y * ox));
         red_add_v4(vg.d_conic + rec, -0.5f * o * s_xx, -0.5f * o * s_xy, -0.5f * o * s_yy, s_u);
-        red_add_v4(vg.d_color + rec, s_r, s_g, s_b, 0.0f);
+        red_add_v4(vg.d_color + rec, s_r, s_g, s_b, DEPTH ? s_d : 0.0f);
     }
     __syncwarp();
 }
 
-template <int K>
-__global__ void __launch_bounds__(kBwdWarps * 32, 6)
+// DEPTH: dL/dD = d_depth rides along (see bwd_batch); built for 5 resident CTAs so that it does not spill.
+template <int K, bool DEPTH>
+__global__ void __launch_bounds__(kBwdWarps * 32, DEPTH ? 5 : 6)
 k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsigned long long *__restrict__ keys,
-                 ImageState img, const float *__restrict__ d_color, ViewGrads vg, LossEpilogue loss, HitLists hl) {
+                 ImageState img, const float *__restrict__ d_color, const float *__restrict__ d_depth, ViewGrads vg,
+                 LossEpilogue loss, HitLists hl) {
     extern __shared__ __align__(16) unsigned char s_raw[];
     constexpr int kTasksPerCta = kBwdWarps / K;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int run = warp % K;
-    BwdSmem &sm = reinterpret_cast<BwdSmem *>(s_raw)[warp];
+    BwdSmem<DEPTH> &sm = reinterpret_cast<BwdSmem<DEPTH> *>(s_raw)[warp];
     if (*geo.n_instances > d.capacity) return;
     TaskGeom t;
     if (!task_setup(d, geo, (long long)blockIdx.x * kTasksPerCta + warp / K, lane, t)) return;
 
     BwdPixel px;
     px.T = 1.0f; px.S = 0.0f;
-    px.last = 0; px.dpr = px.dpg = px.dpb = 0.0f; px.Q = 0.0f;
+    px.last = 0; px.dpr = px.dpg = px.dpb = px.dpd = 0.0f; px.Q = 0.0f;
     if (t.inside) {
         const size_t o1 = (size_t)t.vid * t.hw + t.pix, o3 = (size_t)t.vid * 3 * t.hw + t.pix;
         px.last = img.n_contrib[o1];
@@ -531,8 +560,12 @@ k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
             px.dpb = sc * (c_b - loss.target[o3 + 2 * t.hw]);
         }
         px.Q = c_r * px.dpr + c_g * px.dpg + c_b * px.dpb;
+        if (DEPTH) {   // Q = C . dL/dC + D dL/dD (the background adds nothing to the depth channel)
+            px.dpd = d_depth[o1];
+            px.Q = fmaf(img.depth_image[o1], px.dpd, px.Q);
+        }
     }
-    sm.dp[lane] = make_float4(px.dpr, px.dpg, px.dpb, 0.0f);
+    sm.dp[lane] = make_float4(px.dpr, px.dpg, px.dpb, px.dpd);
     // nothing beyond the block's last contributor; the run split is the forward's (on the full count)
     const uint32_t nmax = min(t.count, __reduce_max_sync(0xffffffffu, px.last));
     if (K > 1) {
@@ -542,6 +575,8 @@ k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
             const float4 st = img.run_state[((size_t)t.vid * (kMaxSegments - 1) + (run - 1)) * t.hw + t.pix];
             px.T = st.x;
             px.S = st.y * px.dpr + st.z * px.dpg + st.w * px.dpb;
+            if (DEPTH)
+                px.S = fmaf(img.run_depth[((size_t)t.vid * (kMaxSegments - 1) + (run - 1)) * t.hw + t.pix], px.dpd, px.S);
         }
     }
     const uint32_t run_end = min(t.run_begin + t.run_len, nmax);
@@ -579,11 +614,12 @@ k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
                 sm.q.r1[slot] = make_float4(qa, qb, qc, __uint_as_float(hcur.x));
                 sm.q.r2[slot] = make_float4(rgb.x, rgb.y, rgb.z, __uint_as_float(hcur.y));
                 sm.d0[slot] = make_float2(dx0, dy0);
+                if (DEPTH) sm.dd[slot] = rgb.w;
             }
             tail += (uint32_t)__popc(m);
             __syncwarp();
             while (tail - head >= (uint32_t)kBatch) {
-                bwd_batch<true>(sm, px, t, vg, head, kBatch, kx, ky, lane);
+                bwd_batch<true, DEPTH>(sm, px, t, vg, head, kBatch, kx, ky, lane);
                 head += kBatch;
             }
             if (m != 0xffffffffu) break;                                      // the list is ordered by position
@@ -593,18 +629,18 @@ k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
         cull_prologue(p, geo, t, keys, n, lane);
         const uint32_t nchunks = (n + 31u) >> 5;
         for (uint32_t c = 0; c <= nchunks; ++c) {
-            cull_park<true>(p, sm.q, sm.d0, t);
+            cull_park<true, DEPTH>(p, sm.q, sm.d0, t, sm.dd);
             const uint32_t avail = tail;
             if (c < nchunks) tail += (uint32_t)cull_step(p, geo, t, keys, n, c, tail, lane);
             while (avail - head >= (uint32_t)kBatch) {
-                bwd_batch<true>(sm, px, t, vg, head, kBatch, kx, ky, lane);
+                bwd_batch<true, DEPTH>(sm, px, t, vg, head, kBatch, kx, ky, lane);
                 head += kBatch;
             }
         }
     }
     if (tail != head) {
-        queue_pad(sm.q, tail, lane);
-        bwd_batch<false>(sm, px, t, vg, head, (int)(tail - head), kx, ky, lane);
+        queue_pad(sm.q, tail, lane, DEPTH ? sm.dd : nullptr);
+        bwd_batch<false, DEPTH>(sm, px, t, vg, head, (int)(tail - head), kx, ky, lane);
     }
 }
 
@@ -622,6 +658,13 @@ int composite_impl() {
     return g_impl;
 }
 
+int get_composite_option(int which) {
+    if (which == 0) return composite_impl();
+    composite_segments(0);           // reads the environment once
+    composite_hit_lists(0);
+    return which == 1 ? g_segments : g_hit_lists;
+}
+
 int set_composite_option(int which, int value) {
     if (which == 0 && (value == 1 || value == 2)) { g_impl = value; return PS_OK; }
     if (which == 1 && (value == 0 || value == 1 || value == 2 || value == 4)) { g_segments = value; return PS_OK; }
@@ -629,15 +672,23 @@ int set_composite_option(int which, int value) {
     return PS_ERR_INVALID_ARGUMENT;
 }
 
-template <int K>
+template <int K, bool DEPTH>
 static int launch_fwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
                       const ImageState &img, float *out_color, const LossEpilogue &loss, const HitLists &hl,
                       cudaStream_t st) {
     const long long tasks = (long long)d.S * d.V * d.tiles * 8;
     constexpr int per_cta = kFwdWarps / K;
-    k_composite_fwd2<K><<<(unsigned)((tasks + per_cta - 1) / per_cta), kFwdWarps * 32, 0, st>>>(d, g, in.bg, keys, img, out_color, loss, hl);
+    k_composite_fwd2<K, DEPTH><<<(unsigned)((tasks + per_cta - 1) / per_cta), kFwdWarps * 32, 0, st>>>(d, g, in.bg, keys, img, out_color, loss, hl);
     PS_LAUNCH_CHECK("k_composite_fwd2");
     return PS_OK;
+}
+
+template <int K>
+static int launch_fwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
+                      const ImageState &img, float *out_color, const LossEpilogue &loss, const HitLists &hl,
+                      cudaStream_t st) {
+    return d.depth_mode ? launch_fwd<K, true>(d, in, g, keys, img, out_color, loss, hl, st)
+                        : launch_fwd<K, false>(d, in, g, keys, img, out_color, loss, hl, st);
 }
 
 int launch_composite_forward(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
@@ -654,33 +705,42 @@ int launch_composite_forward(const Dims &d, const Inputs &in, const Geom &g, con
     }
 }
 
-template <int K>
+template <int K, bool DEPTH>
 static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
-                      const ImageState &img, const float *d_color, const ViewGrads &vg, const LossEpilogue &loss,
-                      const HitLists &hl, cudaStream_t st) {
+                      const ImageState &img, const float *d_color, const float *d_depth, const ViewGrads &vg,
+                      const LossEpilogue &loss, const HitLists &hl, cudaStream_t st) {
     const long long tasks = (long long)d.S * d.V * d.tiles * 8;
     constexpr int per_cta = kBwdWarps / K;
-    const size_t smem = sizeof(BwdSmem) * kBwdWarps;
+    const size_t smem = sizeof(BwdSmem<DEPTH>) * kBwdWarps;
     static unsigned long long attr_devices = 0;
     if (first_use_on_device(attr_devices)) {
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_composite_bwd2<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PS_CUDA_CHECK(cudaFuncSetAttribute(k_composite_bwd2<K, DEPTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
-    k_composite_bwd2<K><<<(unsigned)((tasks + per_cta - 1) / per_cta), kBwdWarps * 32, smem, st>>>(d, g, in.bg, keys, img, d_color, vg, loss, hl);
+    k_composite_bwd2<K, DEPTH><<<(unsigned)((tasks + per_cta - 1) / per_cta), kBwdWarps * 32, smem, st>>>(
+        d, g, in.bg, keys, img, d_color, d_depth, vg, loss, hl);
     PS_LAUNCH_CHECK("k_composite_bwd2");
     return PS_OK;
 }
 
+template <int K>
+static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
+                      const ImageState &img, const float *d_color, const float *d_depth, const ViewGrads &vg,
+                      const LossEpilogue &loss, const HitLists &hl, cudaStream_t st) {
+    return d_depth ? launch_bwd<K, true>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st)
+                   : launch_bwd<K, false>(d, in, g, keys, img, d_color, nullptr, vg, loss, hl, st);
+}
+
 int launch_composite_backward(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
-                              const ImageState &img, const float *d_color, const ViewGrads &vg,
+                              const ImageState &img, const float *d_color, const float *d_depth, const ViewGrads &vg,
                               const LossEpilogue &loss, const HitLists &hl, cudaStream_t st) {
     if (composite_impl() == 1) {
         if (!d_color) { set_error("the legacy compositor has no loss epilogue"); return PS_ERR_UNSUPPORTED; }
         return launch_composite_backward_v1(d, in, g, keys, img, d_color, vg, st);
     }
     switch (d.segK) {
-        case 4: return launch_bwd<4>(d, in, g, keys, img, d_color, vg, loss, hl, st);
-        case 2: return launch_bwd<2>(d, in, g, keys, img, d_color, vg, loss, hl, st);
-        default: return launch_bwd<1>(d, in, g, keys, img, d_color, vg, loss, hl, st);
+        case 4: return launch_bwd<4>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
+        case 2: return launch_bwd<2>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
+        default: return launch_bwd<1>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
     }
 }
 

@@ -123,7 +123,8 @@ k_preprocess(Dims d, Inputs in, Geom geo, int use_smem_hist) {
                                                 (unsigned short)maxx, (unsigned short)maxy);
                     if (d.M == 0) {
                         const float *__restrict__ col = in.sh + sg * 3;
-                        geo.rgb[vg] = make_float4(col[0], col[1], col[2], 0.0f);
+                        const float dv = d.depth_mode ? depth_value(d.depth_mode, vz, in.scale, in.near_far, vid) : 0.0f;
+                        geo.rgb[vg] = make_float4(col[0], col[1], col[2], dv);
                         geo.clamped[vg] = 0;
                     }
                     for (int ty = miny; ty < maxy; ++ty)
@@ -201,7 +202,9 @@ k_sh_color(Dims d, Inputs in, Geom geo, int row_stride) {
         if (a < 0.0f) clamp_bits |= (uint8_t)(1u << ch);
         rgb[ch] = fmaxf(a, 0.0f);
     }
-    geo.rgb[vg] = make_float4(rgb[0], rgb[1], rgb[2], 0.0f);
+    // depth channel in the spare lane (the same function of the same vz as the colors_precomp branch above)
+    const float dv = d.depth_mode ? depth_value(d.depth_mode, geo.depth[vg], in.scale, in.near_far, (int)vid) : 0.0f;
+    geo.rgb[vg] = make_float4(rgb[0], rgb[1], rgb[2], dv);
     geo.clamped[vg] = clamp_bits;
 }
 

@@ -19,7 +19,10 @@ constexpr int kPreBwdThreads = 128;
 // launch_gradient_fill (plain memsets, issued on a side stream so that they overlap the
 // compute-bound composite backward).  SH rows are staged per warp in shared memory: coefficients
 // come in with coalesced row-wise loads, dL/dSH goes out the same way.
-__global__ void __launch_bounds__(kPreBwdThreads, 5)
+// DEPTH: the depth value's chain to the means is added (a depth gradient was given); built for 4 resident CTAs so
+// that it does not spill.
+template <bool DEPTH>
+__global__ void __launch_bounds__(kPreBwdThreads, DEPTH ? 4 : 5)
 k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, ps_raster_grads out, int row_stride) {
     extern __shared__ float s_dsh[];   // [warps][32][row_stride] coefficients (V == 1: reused for the gradient)
     if (*geo.n_instances > d.capacity) return;
@@ -178,6 +181,13 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, ps_raster_grads out
             dcol[0] += gcol.x; dcol[1] += gcol.y; dcol[2] += gcol.z;
         }
         dmx += gx * sc; dmy += gy * sc; dmz += gz * sc;
+        if (DEPTH && vis) {
+            // depth channel: d = f(z), z = vz / sc = (vm[2], vm[6], vm[10]) . mean + vm[14] / sc, so the chain to the
+            // (unscaled) mean carries no scale factor.  Re-read here, after the SH part, to keep registers free there.
+            const float *__restrict__ vm = in.view + 16 * vid;
+            const float dz = vgr.d_color[vg].w * depth_value_grad(d.depth_mode, geo.depth[vg], in.scale, in.near_far, vid);
+            dmx += dz * vm[2]; dmy += dz * vm[6]; dmz += dz * vm[10];
+        }
     }
 
     if (live) {
@@ -223,11 +233,15 @@ int launch_preprocess_backward(const Dims &d, const Inputs &in, const Geom &g, c
     const size_t smem = d.M > 0 ? sizeof(float) * kPreBwdThreads * row_stride * (d.V == 1 ? 1 : 2) : 0;
     static unsigned long long attr_devices = 0;
     if (first_use_on_device(attr_devices)) {
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_preprocess_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        PS_CUDA_CHECK(cudaFuncSetAttribute(k_preprocess_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+        PS_CUDA_CHECK(cudaFuncSetAttribute(k_preprocess_bwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     }
     const long long sp = (long long)d.S * d.P;               // worst case; surplus warps exit at once
-    k_preprocess_bwd<<<(unsigned)((sp + kPreBwdThreads - 1) / kPreBwdThreads), kPreBwdThreads, smem, st>>>(
-        d, in, g, vg, out, row_stride);
+    const unsigned blocks = (unsigned)((sp + kPreBwdThreads - 1) / kPreBwdThreads);
+    if (d.depth_mode)
+        k_preprocess_bwd<true><<<blocks, kPreBwdThreads, smem, st>>>(d, in, g, vg, out, row_stride);
+    else
+        k_preprocess_bwd<false><<<blocks, kPreBwdThreads, smem, st>>>(d, in, g, vg, out, row_stride);
     PS_LAUNCH_CHECK("k_preprocess_bwd");
     return PS_OK;
 }

@@ -19,7 +19,7 @@ import torch
 from torch import Tensor
 
 from .. import _lib
-from ..rasterizer import rasterize_gaussians, rasterize_gaussians_mse
+from ..rasterizer import rasterize_gaussians, rasterize_gaussians_mse, rasterize_gaussians_with_depth
 
 DepthRenderingMode = Literal["depth", "disparity", "relative_disparity", "log"]
 
@@ -121,6 +121,69 @@ def render_views_mse(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: 
         image_shape=(h, w), views_per_scene=v, sh_degree=isqrt(n) - 1, use_sh=True, sh_layout=_lib.PS_SH_3M,
         scene_scale=cams["scene_scale"] if scale_invariant else None, want_color=want_color)
     return sse.reshape(s, v), sse_clipped.reshape(s, v), (color.reshape(s, v, 3, h, w) if want_color else None)
+
+
+def _legacy_compositor() -> bool:
+    """The legacy CTA-per-tile compositor (composite_impl = 1) has no depth channel."""
+    return _lib.get_option("composite_impl") == 1
+
+
+def render_views_with_depth(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor,
+                            image_shape: tuple[int, int], background_color: Tensor, gaussian_means: Tensor,
+                            gaussian_covariances: Tensor, gaussian_sh_coefficients: Tensor, gaussian_opacities: Tensor,
+                            scale_invariant: bool = True, mode: DepthRenderingMode = "depth",
+                            state_out: Optional[list] = None) -> tuple[Tensor, Tensor]:
+    """render_views and render_depth_views in one pass: the depth map is a fourth channel of the colour
+    compositor (same visibility, sort order and alphas), not a second rasterization over per-view copies of the
+    Gaussians.  -> (color [s, v, 3, h, w], depth [s, v, h, w]), both differentiable.  Under the legacy compositor
+    the two are rendered separately, as render_views + render_depth_views."""
+    if _legacy_compositor():
+        color = render_views(extrinsics, intrinsics, near, far, image_shape, background_color, gaussian_means,
+                             gaussian_covariances, gaussian_sh_coefficients, gaussian_opacities, scale_invariant,
+                             state_out=state_out)
+        return color, render_depth_views(extrinsics, intrinsics, near, far, image_shape, gaussian_means,
+                                         gaussian_covariances, gaussian_opacities, scale_invariant, mode)
+    s, v = extrinsics.shape[:2]
+    n = gaussian_sh_coefficients.shape[-1]
+    cams = camera_setup(extrinsics.reshape(s * v, 4, 4), intrinsics.reshape(s * v, 3, 3),
+                        near.reshape(s * v), far.reshape(s * v), scale_invariant)
+    h, w = image_shape
+    color, depth, _ = rasterize_gaussians_with_depth(
+        gaussian_means, gaussian_covariances, gaussian_opacities, gaussian_sh_coefficients,
+        viewmatrix=cams["viewmatrix"], projmatrix=cams["projmatrix"], campos=cams["campos"],
+        tanfov=cams["tanfov"], background=background_color.reshape(s * v, 3).to(torch.float32),
+        image_shape=(h, w), views_per_scene=v, sh_degree=isqrt(n) - 1, use_sh=True, sh_layout=_lib.PS_SH_3M,
+        scene_scale=cams["scene_scale"] if scale_invariant else None, depth_mode=mode,
+        near_far=_near_far_world(near, far, s * v), state_out=state_out)
+    return color.reshape(s, v, 3, h, w), depth.reshape(s, v, h, w)
+
+
+def render_views_mse_with_depth(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor,
+                                image_shape: tuple[int, int], background_color: Tensor, gaussian_means: Tensor,
+                                gaussian_covariances: Tensor, gaussian_sh_coefficients: Tensor,
+                                gaussian_opacities: Tensor, target: Tensor, scale_invariant: bool = True,
+                                mode: DepthRenderingMode = "depth", want_color: bool = True):
+    """render_views_mse with the depth channel of render_views_with_depth: -> (sse [s, v], sse_clipped [s, v],
+    color [s, v, 3, h, w] detached or None, depth [s, v, h, w] differentiable)."""
+    s, v = extrinsics.shape[:2]
+    n = gaussian_sh_coefficients.shape[-1]
+    cams = camera_setup(extrinsics.reshape(s * v, 4, 4), intrinsics.reshape(s * v, 3, 3),
+                        near.reshape(s * v), far.reshape(s * v), scale_invariant)
+    h, w = image_shape
+    sse, sse_clipped, color, depth, _ = rasterize_gaussians_with_depth(
+        gaussian_means, gaussian_covariances, gaussian_opacities, gaussian_sh_coefficients,
+        viewmatrix=cams["viewmatrix"], projmatrix=cams["projmatrix"], campos=cams["campos"],
+        tanfov=cams["tanfov"], background=background_color.reshape(s * v, 3).to(torch.float32),
+        image_shape=(h, w), views_per_scene=v, sh_degree=isqrt(n) - 1, use_sh=True, sh_layout=_lib.PS_SH_3M,
+        scene_scale=cams["scene_scale"] if scale_invariant else None, depth_mode=mode,
+        near_far=_near_far_world(near, far, s * v), target=target.reshape(s * v, 3, h, w).to(torch.float32),
+        want_color=want_color)
+    return (sse.reshape(s, v), sse_clipped.reshape(s, v),
+            color.reshape(s, v, 3, h, w) if want_color else None, depth.reshape(s, v, h, w))
+
+
+def _near_far_world(near: Tensor, far: Tensor, n: int) -> Tensor:
+    return torch.stack([near.reshape(n), far.reshape(n)], -1).to(torch.float32).contiguous()
 
 
 def render_cuda(

@@ -10,7 +10,8 @@ from typing import Any, Literal, Optional
 import torch
 from torch import Tensor, nn
 
-from .cuda_splatting import DepthRenderingMode, render_depth_views, render_views, render_views_mse
+from .cuda_splatting import (DepthRenderingMode, render_depth_views, render_views, render_views_mse,
+                             render_views_mse_with_depth, render_views_with_depth)
 
 
 @dataclass
@@ -49,18 +50,27 @@ class DecoderSplattingCUDA(nn.Module):
                 far: Tensor, image_shape: tuple[int, int],
                 depth_mode: DepthRenderingMode | None = None) -> DecoderOutput:
         b, v, _, _ = extrinsics.shape
-        color = render_views(extrinsics, intrinsics, near, far, image_shape,
-                             self.background_color.expand(b, v, 3), gaussians.means,
-                             gaussians.covariances, gaussians.harmonics, gaussians.opacities)
-        return DecoderOutput(color, None if depth_mode is None else self.render_depth(
-            gaussians, extrinsics, intrinsics, near, far, image_shape, depth_mode))
+        args = (extrinsics, intrinsics, near, far, image_shape, self.background_color.expand(b, v, 3),
+                gaussians.means, gaussians.covariances, gaussians.harmonics, gaussians.opacities)
+        if depth_mode is None:
+            return DecoderOutput(render_views(*args), None)
+        # the depth map is a channel of the colour pass (two passes under the legacy compositor)
+        return DecoderOutput(*render_views_with_depth(*args, mode=depth_mode))
 
     def forward_mse(self, gaussians: Gaussians, extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor,
-                    image_shape: tuple[int, int], target: Tensor, want_color: bool = True):
+                    image_shape: tuple[int, int], target: Tensor, want_color: bool = True,
+                    depth_mode: DepthRenderingMode | None = None):
         """`forward` with LossMse / PSNR sums taken in the compositor's epilogue (row f-4):
         -> (DecoderOutput (color detached, or None when want_color=False), sse [b, v], sse_clipped [b, v]).
-        pixelsplat_b200.loss.mse_from_sse / psnr_from_sse turn the sums into the reference's numbers."""
+        pixelsplat_b200.loss.mse_from_sse / psnr_from_sse turn the sums into the reference's numbers.
+        With `depth_mode`, DecoderOutput.depth is the (differentiable) depth channel of the same pass."""
         b, v, _, _ = extrinsics.shape
+        if depth_mode is not None:
+            sse, sse_clipped, color, depth = render_views_mse_with_depth(
+                extrinsics, intrinsics, near, far, image_shape, self.background_color.expand(b, v, 3),
+                gaussians.means, gaussians.covariances, gaussians.harmonics, gaussians.opacities, target,
+                mode=depth_mode, want_color=want_color)
+            return DecoderOutput(color, depth), sse, sse_clipped
         sse, sse_clipped, color = render_views_mse(
             extrinsics, intrinsics, near, far, image_shape, self.background_color.expand(b, v, 3), gaussians.means,
             gaussians.covariances, gaussians.harmonics, gaussians.opacities, target, want_color=want_color)

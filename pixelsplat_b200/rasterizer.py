@@ -183,28 +183,52 @@ class RasterOutputState:
             color=view(self.image, lay.color, torch.float32, vt * 3 * hw, (vt, 3, d.height, d.width)),
             # (T, Cr, Cg, Cb) in front of list runs 1..3; written only when the forward cut lists into runs
             run_state=view(self.image, lay.run_state, torch.float32, vt * 3 * hw * 4, (vt, 3, d.height, d.width, 4)),
+            # depth channel and the depth in front of list runs 1..3 (None when the forward had no depth channel)
+            depth_image=view(self.image, lay.depth_image, torch.float32, vt * hw, (vt, d.height, d.width))
+            if d.depth_mode else None,
+            run_depth=view(self.image, lay.run_depth, torch.float32, vt * 3 * hw, (vt, 3, d.height, d.width))
+            if d.depth_mode else None,
             num_instances=n,
         )
 
+    def depth_image(self) -> Tensor:
+        """The composited depth channel [S*V, H, W] (a view of the image state; depth forwards only)."""
+        d = self.desc
+        off = _lib.layout(d).depth_image
+        n = d.n_scenes * d.views_per_scene * d.height * d.width
+        return self.image[off:off + 4 * n].view(torch.float32).reshape(-1, d.height, d.width)
+
 
 def _make_desc(S, V, P, M, deg, sh_layout, cov_layout, H, W, capacity, sort_impl, seg_hint=0,
-               sh_basis=0) -> _lib.RasterDesc:
+               sh_basis=0, depth_mode=0) -> _lib.RasterDesc:
     return _lib.RasterDesc(S, V, P, M, deg, sh_layout, cov_layout, H, W, sort_impl, seg_hint, capacity,
-                           sh_basis, 0)
+                           sh_basis, depth_mode)
+
+
+def _raster_inputs(means, cov, opac, sh, cams) -> _lib.RasterInputs:
+    opt = lambda k: cams[k].data_ptr() if cams.get(k) is not None else None
+    return _lib.RasterInputs(
+        means.data_ptr(), cov.data_ptr(), opac.data_ptr(), sh.data_ptr(),
+        cams["viewmatrix"].data_ptr(), cams["projmatrix"].data_ptr(), cams["campos"].data_ptr(),
+        cams["tanfov"].data_ptr(), cams["background"].data_ptr(), opt("scene_scale"), opt("near_far"))
 
 
 def _forward_native(means, cov, opac, sh, cams, S, V, P, M, deg, sh_layout, cov_layout, H, W,
-                    sort_impl, want_radii, sh_basis=0, backward_follows=False, loss_target=None, want_color=True):
+                    sort_impl, want_radii, sh_basis=0, backward_follows=False, loss_target=None, want_color=True,
+                    depth_mode=0):
     """Returns (color | None, radii | None, state) and, with `loss_target`, a 4th element: the
-    [S*V, 2, LOSS_SLOTS] partial sums of the fused loss epilogue."""
+    [S*V, 2, LOSS_SLOTS] partial sums of the fused loss epilogue.  With depth_mode != 0 the state also holds the
+    depth channel (RasterOutputState.depth_image)."""
     dev = means.device
     with torch.cuda.device(dev):            # the library works on the CURRENT device
         return _forward_on_device(means, cov, opac, sh, cams, S, V, P, M, deg, sh_layout, cov_layout, H, W,
-                                  sort_impl, want_radii, sh_basis, backward_follows, loss_target, want_color)
+                                  sort_impl, want_radii, sh_basis, backward_follows, loss_target, want_color,
+                                  depth_mode)
 
 
 def _forward_on_device(means, cov, opac, sh, cams, S, V, P, M, deg, sh_layout, cov_layout, H, W,
-                       sort_impl, want_radii, sh_basis, backward_follows, loss_target=None, want_color=True):
+                       sort_impl, want_radii, sh_basis, backward_follows, loss_target=None, want_color=True,
+                       depth_mode=0):
     dev = means.device
     key = (dev.index, S, V, P, H, W)
     capturing = torch.cuda.is_current_stream_capturing()
@@ -219,7 +243,7 @@ def _forward_on_device(means, cov, opac, sh, cams, S, V, P, M, deg, sh_layout, c
     stream = torch.cuda.current_stream(dev)
     while True:
         desc = _make_desc(S, V, P, M, deg, sh_layout, cov_layout, H, W, capacity, sort_impl,
-                          min(_segment_hint.get(key, 0), 1 << 30), sh_basis)
+                          min(_segment_hint.get(key, 0), 1 << 30), sh_basis, depth_mode)
         sz = _lib.sizes(desc)
         geom = torch.empty(sz.geom_bytes, dtype=torch.uint8, device=dev)
         binning = torch.empty(sz.binning_bytes, dtype=torch.uint8, device=dev)
@@ -229,11 +253,7 @@ def _forward_on_device(means, cov, opac, sh, cams, S, V, P, M, deg, sh_layout, c
         sums = (torch.empty((S * V, 2, _lib.LOSS_SLOTS), dtype=torch.float32, device=dev)
                 if loss_target is not None else None)
         n_host = _pinned_slot()
-        inputs = _lib.RasterInputs(
-            means.data_ptr(), cov.data_ptr(), opac.data_ptr(), sh.data_ptr(),
-            cams["viewmatrix"].data_ptr(), cams["projmatrix"].data_ptr(), cams["campos"].data_ptr(),
-            cams["tanfov"].data_ptr(), cams["background"].data_ptr(),
-            cams["scene_scale"].data_ptr() if cams.get("scene_scale") is not None else None)
+        inputs = _raster_inputs(means, cov, opac, sh, cams)
         state = _lib.RasterState(geom.data_ptr(), geom.numel(), binning.data_ptr(), binning.numel(),
                                  image.data_ptr(), image.numel())
         if loss_target is None:
@@ -409,6 +429,120 @@ class _RasterizeMseFn(torch.autograd.Function):
                                                   ctypes.byref(grads), ctypes.c_void_p(stream.cuda_stream))
         _lib.check(rc, "ps_raster_backward_loss")
         return (d_means, d_cov, d_opac, d_sh) + (None,) * 15
+
+
+class _RasterizeDepthFn(torch.autograd.Function):
+    """_RasterizeFn (target None) or _RasterizeMseFn (target given) with the depth channel composited in the same
+    pass.  Outputs (color, depth [S*V, H, W], radii, sse, sse_clipped); sse / sse_clipped are empty without a
+    target, and with one the colour is detached (as in _RasterizeMseFn).  When no gradient reaches `depth` the
+    backward is the colour-only one (ps_raster_backward / ps_raster_backward_loss)."""
+
+    @staticmethod
+    def forward(ctx, means, cov, opac, sh, target, cams, S, V, P, M, deg, sh_layout, cov_layout, H, W, sort_impl,
+                state_out, sh_basis, depth_mode, want_color):
+        ctx.set_materialize_grads(False)
+        backward_follows = any(ctx.needs_input_grad[:4])
+        out = _forward_native(means, cov, opac, sh, cams, S, V, P, M, deg, sh_layout, cov_layout, H, W, sort_impl,
+                              True, sh_basis, backward_follows, loss_target=target,
+                              want_color=want_color or target is None, depth_mode=depth_mode)
+        color, radii, st = out[:3]
+        depth = st.depth_image().clone()
+        ctx.save_for_backward(means, cov, opac, sh, target)
+        ctx.cams, ctx.st = cams, st
+        if state_out is not None:
+            state_out.append(st)
+        if target is None:
+            sse = sse_clipped = torch.empty(0, device=means.device)
+        else:
+            totals = out[3].sum(dim=-1)                              # [S*V, 2]
+            sse, sse_clipped = totals[:, 0].contiguous(), totals[:, 1].contiguous()
+            if color is None:
+                color = torch.empty(0, device=means.device)
+            ctx.mark_non_differentiable(color)
+        ctx.mark_non_differentiable(radii, sse_clipped)
+        return color, depth, radii, sse, sse_clipped
+
+    @staticmethod
+    def backward(ctx, d_color, d_depth, _d_radii, d_sse, _d_clip):
+        means, cov, opac, sh, target = ctx.saved_tensors
+        st: RasterOutputState = ctx.st
+        st.verify()
+        desc, cams = st.desc, ctx.cams
+        dev = means.device
+        VT = desc.n_scenes * desc.views_per_scene
+        f32 = lambda t: t.to(torch.float32).contiguous()
+        if target is None:
+            d_color = (torch.zeros((VT, 3, desc.height, desc.width), dtype=torch.float32, device=dev)
+                       if d_color is None else f32(d_color))
+        else:
+            scale = 2.0 * (torch.zeros(VT, dtype=torch.float32, device=dev) if d_sse is None else f32(d_sse))
+        sz = _lib.sizes(desc)
+        scratch = torch.empty(sz.backward_bytes, dtype=torch.uint8, device=dev)
+        d_means, d_cov = torch.empty_like(means), torch.empty_like(cov)
+        d_opac, d_sh = torch.empty_like(opac), torch.empty_like(sh)
+        inputs = _raster_inputs(means, cov, opac, sh, cams)
+        grads = _lib.RasterGrads(d_means.data_ptr(), d_cov.data_ptr(), d_opac.data_ptr(), d_sh.data_ptr(), None)
+        state = st.raw_state()
+        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
+        L = _lib.lib
+        with torch.cuda.device(dev):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            sc = (ctypes.c_void_p(scratch.data_ptr()), scratch.numel(), ctypes.byref(grads), stream)
+            if d_depth is not None:
+                d_depth = f32(d_depth)
+                rc = L.ps_raster_backward_depth(ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state),
+                                                p(d_color if target is None else None), p(target),
+                                                p(scale if target is not None else None), p(d_depth), *sc)
+                what = "ps_raster_backward_depth"
+            elif target is None:
+                rc = L.ps_raster_backward(ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state),
+                                          p(d_color), *sc)
+                what = "ps_raster_backward"
+            else:
+                rc = L.ps_raster_backward_loss(ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state),
+                                               p(target), p(scale), *sc)
+                what = "ps_raster_backward_loss"
+        _lib.check(rc, what)
+        return (d_means, d_cov, d_opac, d_sh) + (None,) * 16
+
+
+def _near_far(near_far: Optional[Tensor], depth_mode: int, VT: int) -> Optional[Tensor]:
+    if depth_mode == 0:
+        raise ValueError(f"depth_mode must be one of {[k for k in _lib.DEPTH_MODES if k]}")
+    if near_far is None:
+        if depth_mode in (3, 4):
+            raise ValueError("depth modes relative_disparity and log need near_far [S*V, 2]")
+        return None
+    return _req(near_far, "near_far", (VT, 2))
+
+
+def rasterize_gaussians_with_depth(
+        means: Tensor, covariances: Tensor, opacities: Tensor, colors: Tensor, *, viewmatrix: Tensor,
+        projmatrix: Tensor, campos: Tensor, tanfov: Tensor, background: Tensor, image_shape: tuple[int, int],
+        views_per_scene: int, sh_degree: int, depth_mode: str, near_far: Optional[Tensor] = None,
+        use_sh: bool = True, sh_layout: int = PS_SH_M3, scene_scale: Optional[Tensor] = None, sort_impl: int = 0,
+        state_out: Optional[list] = None, sh_basis=None, target: Optional[Tensor] = None, want_color: bool = True):
+    """rasterize_gaussians with a depth channel composited in the same pass: the Gaussians' camera-space depth in
+    world units (view-space z / scene_scale), as `depth_mode` "depth" | "disparity" | "relative_disparity" | "log"
+    (the values render_depth_cuda composites), blended with the colour's alphas over a zero background.
+    `near_far` [S*V, 2] (world units) is needed by the last two modes.
+    Returns (color [S*V, 3, H, W], depth [S*V, H, W], radii), both images differentiable.  With `target`
+    [S*V, 3, H, W] the loss epilogue of rasterize_gaussians_mse runs too and the result is (sse [S*V]
+    differentiable, sse_clipped, color detached (empty when want_color=False), depth differentiable, radii)."""
+    means, covariances, opacities, colors, cams, S, V, P, M, cov_layout, H, W = _prepare(
+        means, covariances, opacities, colors, viewmatrix, projmatrix, campos, tanfov, background, image_shape,
+        views_per_scene, use_sh, sh_layout, scene_scale)
+    mode = _lib.DEPTH_MODES.get(depth_mode, 0)
+    cams["near_far"] = _near_far(near_far, mode, S * V)
+    if target is not None:
+        target = _req(target, "target", (S * V, 3, H, W))
+    color, depth, radii, sse, sse_clipped = _RasterizeDepthFn.apply(
+        means, covariances, opacities, colors, target, cams, S, V, P, M, int(sh_degree), sh_layout, cov_layout,
+        H, W, int(sort_impl), state_out, _SH_BASIS if sh_basis is None else convention_id(sh_basis), mode,
+        bool(want_color))
+    if target is None:
+        return color, depth, radii
+    return sse, sse_clipped, color, depth, radii
 
 
 def _prepare(means, covariances, opacities, colors, viewmatrix, projmatrix, campos, tanfov, background, image_shape,

@@ -45,12 +45,16 @@ def main():
     ap.add_argument("--bucket-mb", type=float, default=8.0)
     ap.add_argument("--legacy-allreduce", action="store_true", help="round-1 path: all-reduce after backward (A/B)")
     ap.add_argument("--unfused-loss", action="store_true", help="render an image, then torch MSE (A/B of the loss epilogue)")
+    ap.add_argument("--depth-loss", action="store_true",
+                    help="add LossDepth (re10k_depth_loss: weight 0.25, sigma 12, second derivative) on the fused depth")
+    ap.add_argument("--two-pass-depth", action="store_true",
+                    help="with --depth-loss: render the depth as a second pass (render_depth) instead (A/B)")
     args = ap.parse_args()
     from pixelsplat_b200 import parallel, synthetic
     from pixelsplat_b200.decoder import DecoderSplattingCUDA, DecoderSplattingCUDACfg
     from pixelsplat_b200.encoder import EpipolarTransformer, EpipolarTransformerCfg, ImageSelfAttentionCfg
     from pixelsplat_b200.encoder.encoder_tail import EncoderEpipolarTail, EncoderTailCfg
-    from pixelsplat_b200.loss import mse_from_sse
+    from pixelsplat_b200.loss import LossDepth, LossDepthCfg, LossDepthCfgWrapper, mse_from_sse
     rank, world, local = parallel.init_distributed()
     dev = torch.device("cuda", local)
     torch.cuda.set_device(dev)
@@ -78,6 +82,8 @@ def main():
     near_t, far_t = torch.full((B, T), near_v, device=dev), torch.full((B, T), far_v, device=dev)
 
     context = dict(image=images, extrinsics=ctx_e, intrinsics=ctx_k, near=near_c, far=far_c)
+    loss_depth = LossDepth(LossDepthCfgWrapper(LossDepthCfg(0.25, 12.0, True)))
+    depth_batch = {"target": {"near": near_t, "far": far_t, "image": target}}
     phases = ["encoder", "head", "render", "backward", "allreduce", "optimizer"]
     acc = {p: 0.0 for p in phases}
 
@@ -93,12 +99,18 @@ def main():
             opt.zero_grad(set_to_none=True)
         f, _ = enc(feats, ctx_e, ctx_k, near_c, far_c); mark(1)
         gs = head(f, context, global_step=0); mark(2)
+        fused_depth = "depth" if args.depth_loss and not args.two_pass_depth else None
         if args.unfused_loss:
-            out = dec(gs, tgt_e, tgt_k, near_t, far_t, (HW, HW)); mark(3)
+            out = dec(gs, tgt_e, tgt_k, near_t, far_t, (HW, HW), depth_mode=fused_depth)
             loss = (out.color - target).square().mean()
         else:   # LossMse from the compositor's epilogue: no image tensor, no dL/dC tensor (row f-4)
-            _, sse, _ = dec.forward_mse(gs, tgt_e, tgt_k, near_t, far_t, (HW, HW), target, want_color=False); mark(3)
+            out, sse, _ = dec.forward_mse(gs, tgt_e, tgt_k, near_t, far_t, (HW, HW), target, want_color=False,
+                                          depth_mode=fused_depth)
             loss = mse_from_sse(sse, (HW, HW))
+        if args.depth_loss:
+            depth = out.depth if fused_depth else dec.render_depth(gs, tgt_e, tgt_k, near_t, far_t, (HW, HW))
+            loss = loss + loss_depth(type("O", (), {"depth": depth})(), depth_batch)
+        mark(3)
         loss.backward(); mark(4)
         if reducer is not None:
             reducer.finish()                       # only the tail that backward did not hide
@@ -163,6 +175,8 @@ def main():
             "ms_per_step": 1e3 * sec / args.steps,
             "phase_ms": ({p: acc[p] / len(timeline) for p in phases} if timeline else None),
             "launch": launch, "loss_path": "torch MSE on the rendered image" if args.unfused_loss else "fused compositor epilogue",
+            "depth_loss": None if not args.depth_loss else ("two-pass render_depth" if args.two_pass_depth
+                                                            else "fused depth channel"),
             "allreduce": ("after backward, torch.cat buckets (round-1 path)" if reducer is None else
                           f"{len(reducer.buckets)} flat buckets of <= {args.bucket_mb} MB, issued from backward hooks "
                           "(overlapped); phase 'allreduce' is the exposed tail only"),
