@@ -399,6 +399,31 @@ PS_API int ps_sh_rotation_matrices(int32_t n_views, int32_t sh_coeffs, int32_t n
                                    const float *extrinsics, const float *fit_dirs, const float *fit_pinv,
                                    float *out, void *stream);
 
+/* ---- SSIM of image planes (csrc/ssim.cu) ------------------------------------------------------------------
+ * Replaces the skimage call of /root/reference/src/evaluation/metrics.py:36-52, structural_similarity(win_size=11,
+ * gaussian_weights=True, data_range=1.0) with skimage's defaults (K1 = 0.01, K2 = 0.03, sigma = 1.5, truncate =
+ * 3.5, use_sample_covariance), one plane at a time.  For x (ground truth) and y (prediction) [n_planes, H, W] and
+ * G the normalised 11 x 11 Gaussian window (sigma 1.5):
+ *   mu_x = G*x, mu_y = G*y,  var_x = n (G*x^2 - mu_x^2),  var_y alike,  cov = n (G*xy - mu_x mu_y),  n = 121/120,
+ *   S = (2 mu_x mu_y + C1)(2 cov + C2) / ((mu_x^2 + mu_y^2 + C1)(var_x + var_y + C2)),  C1 = 0.01^2, C2 = 0.03^2,
+ * and the plane's score is the mean of S over the crop [5, H-5) x [5, W-5), where every window lies inside the
+ * image (so no padding mode is involved).  Nothing is clipped.  The constants are fixed; H, W >= 11.
+ * No call synchronises the host; the forward's sum is in a fixed order (the same bits every run).  Every entry point
+ * rejects n_planes < 1, H < 11, W < 11, NULL pointers and a short workspace with PS_ERR_INVALID_ARGUMENT before
+ * anything is enqueued. */
+PS_API int ps_ssim_workspace_bytes(int32_t n_planes, int32_t H, int32_t W, size_t *out);
+
+/* out_mean [n_planes] = the planes' scores.  The workspace (ps_ssim_workspace_bytes) holds per-tile partial sums. */
+PS_API int ps_ssim_forward(int32_t n_planes, int32_t H, int32_t W, const float *x, const float *y, float *out_mean,
+                           void *workspace, size_t workspace_bytes, void *stream);
+
+/* Given d_mean [n_planes] = dL/d(score), writes d_y = dL/dy and, when d_x is not NULL, d_x = dL/dx ([n_planes, H, W],
+ * fully written: no zero-fill needed).  The filtered moments are recomputed, not stored.  The workspace is the
+ * forward's (same size check, so one buffer serves both); the backward does not write it. */
+PS_API int ps_ssim_backward(int32_t n_planes, int32_t H, int32_t W, const float *x, const float *y,
+                            const float *d_mean, float *d_x /* or NULL */, float *d_y, void *workspace,
+                            size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

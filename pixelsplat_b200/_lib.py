@@ -101,7 +101,7 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_self_attention_forward", "ps_gaussian_adapter_forward", "ps_gaussian_adapter_backward",
            "ps_sh_rotation_matrices", "ps_set_option", "ps_raster_forward_loss", "ps_raster_backward_loss",
            "ps_self_attention_forward_stats", "ps_self_attention_backward", "ps_get_option",
-           "ps_raster_backward_depth")
+           "ps_raster_backward_depth", "ps_ssim_workspace_bytes", "ps_ssim_forward", "ps_ssim_backward")
 
 
 class NativeLibraryMissing(ImportError):
@@ -166,6 +166,12 @@ def _load() -> ctypes.CDLL:
     lib.ps_set_option.restype = ctypes.c_int
     lib.ps_get_option.argtypes = [ctypes.c_char_p, ctypes.POINTER(ctypes.c_int)]
     lib.ps_get_option.restype = ctypes.c_int
+    lib.ps_ssim_workspace_bytes.argtypes = [ctypes.c_int32] * 3 + [P(ctypes.c_size_t)]
+    lib.ps_ssim_workspace_bytes.restype = ctypes.c_int
+    lib.ps_ssim_forward.argtypes = [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 4 + [ctypes.c_size_t, ctypes.c_void_p]
+    lib.ps_ssim_forward.restype = ctypes.c_int
+    lib.ps_ssim_backward.argtypes = [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 6 + [ctypes.c_size_t, ctypes.c_void_p]
+    lib.ps_ssim_backward.restype = ctypes.c_int
     for f in ("ps_raster_sizes_query", "ps_raster_layout_query", "ps_raster_forward", "ps_raster_backward"):
         getattr(lib, f).restype = ctypes.c_int
     return lib

@@ -10,12 +10,19 @@ epilogue already returns, per view, sse = sum (C - t)^2 and sse_clipped = sum (c
 
 with the rendered image never re-read for the loss and dL/dC never written as a tensor.
 
+`ssim` / `compute_ssim` score renders as /root/reference/src/evaluation/metrics.py:36-52 does (skimage's
+structural_similarity with an 11-tap Gaussian window, sigma 1.5, data_range 1, sample covariance), on the GPU: the
+sm_90a kernels of csrc/ssim.cu (`ps_ssim_forward` / `ps_ssim_backward`) instead of a device-to-host copy and a CPU
+loop over images.  `ssim` is differentiable in both images (1 - ssim is the usual partner of the photometric loss);
+`compute_ssim` is the no-grad metric.
+
 `LossDepth` / `LossDepthCfg` / `LossDepthCfgWrapper` are the drop-in for /root/reference/src/loss/loss_depth.py: an
 edge-aware smoothness penalty on the rendered depth map (`DecoderOutput.depth`), which the fused depth channel
 (`DecoderSplattingCUDA.forward(depth_mode=...)`) provides.
 """
 from __future__ import annotations
 
+import ctypes
 from dataclasses import dataclass, fields
 
 import torch
@@ -69,6 +76,76 @@ def compute_psnr(ground_truth: Tensor, predicted: Tensor) -> Tensor:
 def psnr_from_sse(sse_clipped: Tensor, image_shape: tuple[int, int], channels: int = 3) -> Tensor:
     h, w = image_shape
     return -10 * (sse_clipped / (channels * h * w)).log10()
+
+
+def _ssim_check(ground_truth: Tensor, predicted: Tensor) -> None:
+    if ground_truth.dim() != 4 or ground_truth.shape != predicted.shape:
+        raise ValueError(f"ssim: expected two [batch, channel, height, width] tensors of one shape, got "
+                         f"{tuple(ground_truth.shape)} and {tuple(predicted.shape)}")
+    if ground_truth.dtype != torch.float32 or predicted.dtype != torch.float32:
+        raise ValueError(f"ssim: expected float32 images, got {ground_truth.dtype} and {predicted.dtype}")
+    if ground_truth.shape[-2] < 11 or ground_truth.shape[-1] < 11:
+        raise ValueError(f"ssim: images must be at least 11 x 11 (the window), got {tuple(ground_truth.shape[-2:])}")
+    if not (ground_truth.is_cuda and predicted.is_cuda) or ground_truth.device != predicted.device:
+        raise ValueError(f"ssim: expected CUDA tensors on one device, got {ground_truth.device} and "
+                         f"{predicted.device}; there is no CPU path")
+
+
+def _ssim_workspace(n: int, h: int, w: int, device) -> Tensor:
+    from . import _lib
+    size = ctypes.c_size_t()
+    _lib.check(_lib.lib.ps_ssim_workspace_bytes(n, h, w, ctypes.byref(size)), "ps_ssim_workspace_bytes")
+    return torch.empty(size.value, dtype=torch.uint8, device=device)
+
+
+class _SsimPlanes(torch.autograd.Function):
+    """[n, h, w] x 2 -> [n] per-plane scores (x = ground truth, y = prediction)."""
+
+    @staticmethod
+    def forward(ctx, x: Tensor, y: Tensor) -> Tensor:
+        from . import _lib
+        n, h, w = x.shape
+        ws = _ssim_workspace(n, h, w, x.device)
+        out = torch.empty(n, dtype=torch.float32, device=x.device)
+        stream = torch.cuda.current_stream(x.device).cuda_stream
+        rc = _lib.on_device(x.device, _lib.lib.ps_ssim_forward, n, h, w, x.data_ptr(), y.data_ptr(), out.data_ptr(),
+                            ws.data_ptr(), ws.numel(), stream)
+        _lib.check(rc, "ps_ssim_forward")
+        ctx.save_for_backward(x, y)
+        return out
+
+    @staticmethod
+    def backward(ctx, d_out: Tensor):
+        from . import _lib
+        x, y = ctx.saved_tensors
+        n, h, w = x.shape
+        d_out = d_out.contiguous().float()
+        d_x = torch.empty_like(x) if ctx.needs_input_grad[0] else None
+        d_y = torch.empty_like(y)
+        ws = _ssim_workspace(n, h, w, x.device)
+        stream = torch.cuda.current_stream(x.device).cuda_stream
+        rc = _lib.on_device(x.device, _lib.lib.ps_ssim_backward, n, h, w, x.data_ptr(), y.data_ptr(),
+                            d_out.data_ptr(), None if d_x is None else d_x.data_ptr(), d_y.data_ptr(), ws.data_ptr(),
+                            ws.numel(), stream)
+        _lib.check(rc, "ps_ssim_backward")
+        return d_x, (d_y if ctx.needs_input_grad[1] else None)
+
+
+def ssim(ground_truth: Tensor, predicted: Tensor) -> Tensor:
+    """SSIM of each image, [batch, channel, h, w] x 2 float32 CUDA -> [batch]: the mean over channels of each
+    plane's mean SSIM map on the crop [5, h-5) x [5, w-5), as skimage's structural_similarity(win_size=11,
+    gaussian_weights=True, channel_axis=0, data_range=1.0) computes it.  Differentiable in both images (the ground
+    truth gets a gradient only when it requires one).  Inputs are not clipped."""
+    _ssim_check(ground_truth, predicted)
+    b, c, h, w = predicted.shape
+    planes = _SsimPlanes.apply(ground_truth.contiguous().view(b * c, h, w), predicted.contiguous().view(b * c, h, w))
+    return planes.view(b, c).mean(dim=1)
+
+
+@torch.no_grad()
+def compute_ssim(ground_truth: Tensor, predicted: Tensor) -> Tensor:
+    """[batch, c, h, w] x 2 -> [batch] (metrics.py:36-52), on the prediction's device, without a host copy."""
+    return ssim(ground_truth, predicted).to(predicted.dtype)
 
 
 @dataclass
