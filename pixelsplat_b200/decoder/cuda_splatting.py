@@ -19,7 +19,7 @@ import torch
 from torch import Tensor
 
 from .. import _lib
-from ..rasterizer import rasterize_gaussians, rasterize_gaussians_mse, rasterize_gaussians_with_depth
+from ..rasterizer import _rasterize, rasterize_gaussians
 
 DepthRenderingMode = Literal["depth", "disparity", "relative_disparity", "log"]
 
@@ -64,6 +64,39 @@ def camera_setup(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tens
     return dict(viewmatrix=view, projmatrix=proj, campos=campos, tanfov=tanfov, scene_scale=scale)
 
 
+def _render(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor, image_shape: tuple[int, int],
+            background_color: Tensor, gaussian_means: Tensor, gaussian_covariances: Tensor,
+            gaussian_sh_coefficients: Tensor, gaussian_opacities: Tensor, scale_invariant: bool, use_sh: bool = True,
+            state_out: Optional[list] = None, target: Optional[Tensor] = None,
+            mode: Optional[DepthRenderingMode] = None, want_color: bool = True):
+    """One rasterizer call for [s, v] cameras over [s, g] Gaussians, with the loss epilogue when `target`
+    [s, v, 3, h, w] is given and the depth channel when `mode` is.  -> (color [s, v, 3, h, w] or None when
+    want_color=False, depth [s, v, h, w] | None, sse [s, v] | None, sse_clipped [s, v] | None)."""
+    s, v = extrinsics.shape[:2]
+    n = s * v
+    h, w = image_shape
+    cams = camera_setup(extrinsics.reshape(n, 4, 4), intrinsics.reshape(n, 3, 3), near.reshape(n), far.reshape(n),
+                        scale_invariant)
+    if use_sh:
+        colors, layout = gaussian_sh_coefficients, _lib.PS_SH_3M
+    else:
+        colors, layout = gaussian_sh_coefficients[..., 0], _lib.PS_SH_M3
+    color, depth, _, sse, sse_clipped = _rasterize(
+        gaussian_means, gaussian_covariances, gaussian_opacities, colors,
+        viewmatrix=cams["viewmatrix"], projmatrix=cams["projmatrix"], campos=cams["campos"],
+        tanfov=cams["tanfov"], background=background_color.reshape(n, 3).to(torch.float32),
+        image_shape=(h, w), views_per_scene=v, sh_degree=isqrt(gaussian_sh_coefficients.shape[-1]) - 1,
+        use_sh=use_sh, sh_layout=layout, scene_scale=cams["scene_scale"] if scale_invariant else None,
+        state_out=state_out, target=None if target is None else target.reshape(n, 3, h, w).to(torch.float32),
+        depth_mode=mode,
+        near_far=None if mode is None else torch.stack([near.reshape(n), far.reshape(n)], -1).to(torch.float32),
+        want_color=want_color)
+    return (color.reshape(s, v, 3, h, w) if want_color else None,
+            None if depth is None else depth.reshape(s, v, h, w),
+            None if sse is None else sse.reshape(s, v),
+            None if sse_clipped is None else sse_clipped.reshape(s, v))
+
+
 def render_views(
     extrinsics: Tensor,            # [s, v, 4, 4]
     intrinsics: Tensor,            # [s, v, 3, 3]
@@ -81,23 +114,10 @@ def render_views(
 ) -> Tensor:                       # [s, v, 3, h, w]
     """V cameras per scene share the scene's Gaussians (no `repeat`)."""
     assert use_sh or gaussian_sh_coefficients.shape[-1] == 1
-    s, v = extrinsics.shape[:2]
-    n = gaussian_sh_coefficients.shape[-1]
-    degree = isqrt(n) - 1
-    cams = camera_setup(extrinsics.reshape(s * v, 4, 4), intrinsics.reshape(s * v, 3, 3),
-                        near.reshape(s * v), far.reshape(s * v), scale_invariant)
-    if use_sh:
-        colors, layout = gaussian_sh_coefficients, _lib.PS_SH_3M
-    else:
-        colors, layout = gaussian_sh_coefficients[..., 0], _lib.PS_SH_M3
-    h, w = image_shape
-    color, _ = rasterize_gaussians(
-        gaussian_means, gaussian_covariances, gaussian_opacities, colors,
-        viewmatrix=cams["viewmatrix"], projmatrix=cams["projmatrix"], campos=cams["campos"],
-        tanfov=cams["tanfov"], background=background_color.reshape(s * v, 3).to(torch.float32),
-        image_shape=(h, w), views_per_scene=v, sh_degree=degree, use_sh=use_sh, sh_layout=layout,
-        scene_scale=cams["scene_scale"] if scale_invariant else None, state_out=state_out)
-    return color.reshape(s, v, 3, h, w)
+    color, _, _, _ = _render(extrinsics, intrinsics, near, far, image_shape, background_color, gaussian_means,
+                             gaussian_covariances, gaussian_sh_coefficients, gaussian_opacities, scale_invariant,
+                             use_sh=use_sh, state_out=state_out)
+    return color
 
 
 def render_views_mse(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor, image_shape: tuple[int, int],
@@ -108,19 +128,10 @@ def render_views_mse(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: 
     [s, v, 3, h, w] -> (sse [s, v] differentiable sum of squared errors, sse_clipped [s, v] the same on images
     clipped to [0, 1] (what compute_psnr needs), color [s, v, 3, h, w] detached or None).  See
     pixelsplat_b200/loss.py for the LossMse / PSNR built on top."""
-    s, v = extrinsics.shape[:2]
-    n = gaussian_sh_coefficients.shape[-1]
-    cams = camera_setup(extrinsics.reshape(s * v, 4, 4), intrinsics.reshape(s * v, 3, 3),
-                        near.reshape(s * v), far.reshape(s * v), scale_invariant)
-    h, w = image_shape
-    sse, sse_clipped, color, _ = rasterize_gaussians_mse(
-        gaussian_means, gaussian_covariances, gaussian_opacities, gaussian_sh_coefficients,
-        target.reshape(s * v, 3, h, w).to(torch.float32),
-        viewmatrix=cams["viewmatrix"], projmatrix=cams["projmatrix"], campos=cams["campos"],
-        tanfov=cams["tanfov"], background=background_color.reshape(s * v, 3).to(torch.float32),
-        image_shape=(h, w), views_per_scene=v, sh_degree=isqrt(n) - 1, use_sh=True, sh_layout=_lib.PS_SH_3M,
-        scene_scale=cams["scene_scale"] if scale_invariant else None, want_color=want_color)
-    return sse.reshape(s, v), sse_clipped.reshape(s, v), (color.reshape(s, v, 3, h, w) if want_color else None)
+    color, _, sse, sse_clipped = _render(extrinsics, intrinsics, near, far, image_shape, background_color,
+                                         gaussian_means, gaussian_covariances, gaussian_sh_coefficients,
+                                         gaussian_opacities, scale_invariant, target=target, want_color=want_color)
+    return sse, sse_clipped, color
 
 
 def _legacy_compositor() -> bool:
@@ -143,19 +154,10 @@ def render_views_with_depth(extrinsics: Tensor, intrinsics: Tensor, near: Tensor
                              state_out=state_out)
         return color, render_depth_views(extrinsics, intrinsics, near, far, image_shape, gaussian_means,
                                          gaussian_covariances, gaussian_opacities, scale_invariant, mode)
-    s, v = extrinsics.shape[:2]
-    n = gaussian_sh_coefficients.shape[-1]
-    cams = camera_setup(extrinsics.reshape(s * v, 4, 4), intrinsics.reshape(s * v, 3, 3),
-                        near.reshape(s * v), far.reshape(s * v), scale_invariant)
-    h, w = image_shape
-    color, depth, _ = rasterize_gaussians_with_depth(
-        gaussian_means, gaussian_covariances, gaussian_opacities, gaussian_sh_coefficients,
-        viewmatrix=cams["viewmatrix"], projmatrix=cams["projmatrix"], campos=cams["campos"],
-        tanfov=cams["tanfov"], background=background_color.reshape(s * v, 3).to(torch.float32),
-        image_shape=(h, w), views_per_scene=v, sh_degree=isqrt(n) - 1, use_sh=True, sh_layout=_lib.PS_SH_3M,
-        scene_scale=cams["scene_scale"] if scale_invariant else None, depth_mode=mode,
-        near_far=_near_far_world(near, far, s * v), state_out=state_out)
-    return color.reshape(s, v, 3, h, w), depth.reshape(s, v, h, w)
+    color, depth, _, _ = _render(extrinsics, intrinsics, near, far, image_shape, background_color, gaussian_means,
+                                 gaussian_covariances, gaussian_sh_coefficients, gaussian_opacities, scale_invariant,
+                                 state_out=state_out, mode=mode)
+    return color, depth
 
 
 def render_views_mse_with_depth(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor,
@@ -165,25 +167,11 @@ def render_views_mse_with_depth(extrinsics: Tensor, intrinsics: Tensor, near: Te
                                 mode: DepthRenderingMode = "depth", want_color: bool = True):
     """render_views_mse with the depth channel of render_views_with_depth: -> (sse [s, v], sse_clipped [s, v],
     color [s, v, 3, h, w] detached or None, depth [s, v, h, w] differentiable)."""
-    s, v = extrinsics.shape[:2]
-    n = gaussian_sh_coefficients.shape[-1]
-    cams = camera_setup(extrinsics.reshape(s * v, 4, 4), intrinsics.reshape(s * v, 3, 3),
-                        near.reshape(s * v), far.reshape(s * v), scale_invariant)
-    h, w = image_shape
-    sse, sse_clipped, color, depth, _ = rasterize_gaussians_with_depth(
-        gaussian_means, gaussian_covariances, gaussian_opacities, gaussian_sh_coefficients,
-        viewmatrix=cams["viewmatrix"], projmatrix=cams["projmatrix"], campos=cams["campos"],
-        tanfov=cams["tanfov"], background=background_color.reshape(s * v, 3).to(torch.float32),
-        image_shape=(h, w), views_per_scene=v, sh_degree=isqrt(n) - 1, use_sh=True, sh_layout=_lib.PS_SH_3M,
-        scene_scale=cams["scene_scale"] if scale_invariant else None, depth_mode=mode,
-        near_far=_near_far_world(near, far, s * v), target=target.reshape(s * v, 3, h, w).to(torch.float32),
-        want_color=want_color)
-    return (sse.reshape(s, v), sse_clipped.reshape(s, v),
-            color.reshape(s, v, 3, h, w) if want_color else None, depth.reshape(s, v, h, w))
-
-
-def _near_far_world(near: Tensor, far: Tensor, n: int) -> Tensor:
-    return torch.stack([near.reshape(n), far.reshape(n)], -1).to(torch.float32).contiguous()
+    color, depth, sse, sse_clipped = _render(extrinsics, intrinsics, near, far, image_shape, background_color,
+                                             gaussian_means, gaussian_covariances, gaussian_sh_coefficients,
+                                             gaussian_opacities, scale_invariant, target=target, mode=mode,
+                                             want_color=want_color)
+    return sse, sse_clipped, color, depth
 
 
 def render_cuda(

@@ -65,16 +65,13 @@ class DecoderSplattingCUDA(nn.Module):
         pixelsplat_b200.loss.mse_from_sse / psnr_from_sse turn the sums into the reference's numbers.
         With `depth_mode`, DecoderOutput.depth is the (differentiable) depth channel of the same pass."""
         b, v, _, _ = extrinsics.shape
-        if depth_mode is not None:
-            sse, sse_clipped, color, depth = render_views_mse_with_depth(
-                extrinsics, intrinsics, near, far, image_shape, self.background_color.expand(b, v, 3),
-                gaussians.means, gaussians.covariances, gaussians.harmonics, gaussians.opacities, target,
-                mode=depth_mode, want_color=want_color)
-            return DecoderOutput(color, depth), sse, sse_clipped
-        sse, sse_clipped, color = render_views_mse(
-            extrinsics, intrinsics, near, far, image_shape, self.background_color.expand(b, v, 3), gaussians.means,
-            gaussians.covariances, gaussians.harmonics, gaussians.opacities, target, want_color=want_color)
-        return DecoderOutput(color, None), sse, sse_clipped
+        args = (extrinsics, intrinsics, near, far, image_shape, self.background_color.expand(b, v, 3),
+                gaussians.means, gaussians.covariances, gaussians.harmonics, gaussians.opacities, target)
+        if depth_mode is None:
+            sse, sse_clipped, color = render_views_mse(*args, want_color=want_color)
+            return DecoderOutput(color, None), sse, sse_clipped
+        sse, sse_clipped, color, depth = render_views_mse_with_depth(*args, mode=depth_mode, want_color=want_color)
+        return DecoderOutput(color, depth), sse, sse_clipped
 
     def render_depth(self, gaussians: Gaussians, extrinsics: Tensor, intrinsics: Tensor, near: Tensor,
                      far: Tensor, image_shape: tuple[int, int],

@@ -199,10 +199,22 @@ class RasterOutputState:
         return self.image[off:off + 4 * n].view(torch.float32).reshape(-1, d.height, d.width)
 
 
-def _make_desc(S, V, P, M, deg, sh_layout, cov_layout, H, W, capacity, sort_impl, seg_hint=0,
-               sh_basis=0, depth_mode=0) -> _lib.RasterDesc:
-    return _lib.RasterDesc(S, V, P, M, deg, sh_layout, cov_layout, H, W, sort_impl, seg_hint, capacity,
-                           sh_basis, depth_mode)
+class _Config(NamedTuple):
+    """The non-tensor settings of one rasterizer call: the ps_raster_desc fields the caller chooses, and whether
+    the colour image is written."""
+    S: int
+    V: int
+    P: int
+    M: int
+    degree: int
+    sh_layout: int
+    cov_layout: int
+    H: int
+    W: int
+    sort_impl: int
+    sh_basis: int
+    depth_mode: int
+    want_color: bool
 
 
 def _raster_inputs(means, cov, opac, sh, cams) -> _lib.RasterInputs:
@@ -213,253 +225,103 @@ def _raster_inputs(means, cov, opac, sh, cams) -> _lib.RasterInputs:
         cams["tanfov"].data_ptr(), cams["background"].data_ptr(), opt("scene_scale"), opt("near_far"))
 
 
-def _forward_native(means, cov, opac, sh, cams, S, V, P, M, deg, sh_layout, cov_layout, H, W,
-                    sort_impl, want_radii, sh_basis=0, backward_follows=False, loss_target=None, want_color=True,
-                    depth_mode=0):
-    """Returns (color | None, radii | None, state) and, with `loss_target`, a 4th element: the
-    [S*V, 2, LOSS_SLOTS] partial sums of the fused loss epilogue.  With depth_mode != 0 the state also holds the
-    depth channel (RasterOutputState.depth_image)."""
+def _forward(means, cov, opac, sh, cams, cfg: _Config, backward_follows: bool, target: Optional[Tensor]):
+    """Enqueues the forward on the current stream of the Gaussians' device.  Returns (color | None, radii, state,
+    sums | None): `sums` are the [S*V, 2, LOSS_SLOTS] partial sums of the loss epilogue, run when a `target` is
+    given.  With cfg.depth_mode != 0 the state also holds the depth channel (RasterOutputState.depth_image)."""
     dev = means.device
-    with torch.cuda.device(dev):            # the library works on the CURRENT device
-        return _forward_on_device(means, cov, opac, sh, cams, S, V, P, M, deg, sh_layout, cov_layout, H, W,
-                                  sort_impl, want_radii, sh_basis, backward_follows, loss_target, want_color,
-                                  depth_mode)
-
-
-def _forward_on_device(means, cov, opac, sh, cams, S, V, P, M, deg, sh_layout, cov_layout, H, W,
-                       sort_impl, want_radii, sh_basis, backward_follows, loss_target=None, want_color=True,
-                       depth_mode=0):
-    dev = means.device
+    S, V, P, H, W = cfg.S, cfg.V, cfg.P, cfg.H, cfg.W
     key = (dev.index, S, V, P, H, W)
-    capturing = torch.cuda.is_current_stream_capturing()
-    prev = _pending.pop(key, None)
-    if prev is not None and not capturing:
-        prev = prev()
-        if prev is not None:
-            prev.verify()                   # deferred check of the previous forward of this shape
-    capacity = _capacity_hint.get(key)
-    if capacity is None:
-        capacity = max(4096, 3 * S * V * P)
-    stream = torch.cuda.current_stream(dev)
-    while True:
-        desc = _make_desc(S, V, P, M, deg, sh_layout, cov_layout, H, W, capacity, sort_impl,
-                          min(_segment_hint.get(key, 0), 1 << 30), sh_basis, depth_mode)
-        sz = _lib.sizes(desc)
-        geom = torch.empty(sz.geom_bytes, dtype=torch.uint8, device=dev)
-        binning = torch.empty(sz.binning_bytes, dtype=torch.uint8, device=dev)
-        image = torch.empty(sz.image_bytes, dtype=torch.uint8, device=dev)
-        color = torch.empty((S * V, 3, H, W), dtype=torch.float32, device=dev) if want_color else None
-        radii = torch.empty((S * V, P), dtype=torch.int32, device=dev) if want_radii else None
-        sums = (torch.empty((S * V, 2, _lib.LOSS_SLOTS), dtype=torch.float32, device=dev)
-                if loss_target is not None else None)
-        n_host = _pinned_slot()
-        inputs = _raster_inputs(means, cov, opac, sh, cams)
-        state = _lib.RasterState(geom.data_ptr(), geom.numel(), binning.data_ptr(), binning.numel(),
-                                 image.data_ptr(), image.numel())
-        if loss_target is None:
-            rc = _lib.lib.ps_raster_forward(ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state),
-                                            _ptr(color), _ptr(radii), ctypes.c_void_p(n_host.data_ptr()),
-                                            ctypes.c_void_p(stream.cuda_stream))
-            _lib.check(rc, "ps_raster_forward")
-            ret = lambda st_: (color, radii, st_)
-        else:
-            loss = _lib.RasterLoss(loss_target.data_ptr(), sums.data_ptr())
-            rc = _lib.lib.ps_raster_forward_loss(ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state),
-                                                 ctypes.byref(loss), _ptr(color), _ptr(radii),
-                                                 ctypes.c_void_p(n_host.data_ptr()), ctypes.c_void_p(stream.cuda_stream))
-            _lib.check(rc, "ps_raster_forward_loss")
-            ret = lambda st_: (color, radii, st_, sums)
-        if torch.cuda.is_current_stream_capturing():
-            # CUDA-graph capture: shapes and capacity are frozen into the graph; the count still
-            # lands in pinned memory on every replay and is checked by the caller afterwards
-            if key not in _capacity_hint:
-                raise RuntimeError("run this shape once eagerly before capturing it in a CUDA graph "
-                                   "(the binning capacity must be known)")
-            return ret(RasterOutputState(desc, geom, binning, image, n_host, None, key))
-        event = torch.cuda.Event()
-        event.record(stream)
-        st = RasterOutputState(desc, geom, binning, image, n_host, event, key)
-        if _CHECK_MODE == "deferred" and key in _capacity_hint and backward_follows:
-            _pending[key] = weakref.ref(st)
-            return ret(st)
-        n = st.num_instances()
-        if n <= capacity:
-            st.verified = True
-            # keep ~25 % head-room for the next call of the same shape
-            _capacity_hint[key] = max(_capacity_hint.get(key, 0), int(n * _HEADROOM) + 4096)
-            return ret(st)
-        capacity = int(n * _HEADROOM) + 4096
-        _capacity_hint[key] = capacity
+    with torch.cuda.device(dev):            # the library works on the CURRENT device
+        capturing = torch.cuda.is_current_stream_capturing()
+        prev = _pending.pop(key, None)
+        if prev is not None and not capturing:
+            prev = prev()
+            if prev is not None:
+                prev.verify()               # deferred check of the previous forward of this shape
+        capacity = _capacity_hint.get(key)
+        if capacity is None:
+            capacity = max(4096, 3 * S * V * P)
+        stream = torch.cuda.current_stream(dev)
+        while True:
+            desc = _lib.RasterDesc(S, V, P, cfg.M, cfg.degree, cfg.sh_layout, cfg.cov_layout, H, W, cfg.sort_impl,
+                                   min(_segment_hint.get(key, 0), 1 << 30), capacity, cfg.sh_basis, cfg.depth_mode)
+            sz = _lib.sizes(desc)
+            geom = torch.empty(sz.geom_bytes, dtype=torch.uint8, device=dev)
+            binning = torch.empty(sz.binning_bytes, dtype=torch.uint8, device=dev)
+            image = torch.empty(sz.image_bytes, dtype=torch.uint8, device=dev)
+            color = torch.empty((S * V, 3, H, W), dtype=torch.float32, device=dev) if cfg.want_color else None
+            radii = torch.empty((S * V, P), dtype=torch.int32, device=dev)
+            n_host = _pinned_slot()
+            inputs = _raster_inputs(means, cov, opac, sh, cams)
+            state = _lib.RasterState(geom.data_ptr(), geom.numel(), binning.data_ptr(), binning.numel(),
+                                     image.data_ptr(), image.numel())
+            args = [ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state)]
+            if target is None:
+                fn, sums = _lib.lib.ps_raster_forward, None
+            else:
+                fn = _lib.lib.ps_raster_forward_loss
+                sums = torch.empty((S * V, 2, _lib.LOSS_SLOTS), dtype=torch.float32, device=dev)
+                loss = _lib.RasterLoss(target.data_ptr(), sums.data_ptr())
+                args.append(ctypes.byref(loss))
+            rc = fn(*args, _ptr(color), _ptr(radii), ctypes.c_void_p(n_host.data_ptr()),
+                    ctypes.c_void_p(stream.cuda_stream))
+            _lib.check(rc, fn.__name__)
+            if torch.cuda.is_current_stream_capturing():
+                # CUDA-graph capture: shapes and capacity are frozen into the graph; the count still
+                # lands in pinned memory on every replay and is checked by the caller afterwards
+                if key not in _capacity_hint:
+                    raise RuntimeError("run this shape once eagerly before capturing it in a CUDA graph "
+                                       "(the binning capacity must be known)")
+                return color, radii, RasterOutputState(desc, geom, binning, image, n_host, None, key), sums
+            event = torch.cuda.Event()
+            event.record(stream)
+            st = RasterOutputState(desc, geom, binning, image, n_host, event, key)
+            if _CHECK_MODE == "deferred" and key in _capacity_hint and backward_follows:
+                _pending[key] = weakref.ref(st)
+                return color, radii, st, sums
+            n = st.num_instances()
+            if n <= capacity:
+                st.verified = True
+                # keep ~25 % head-room for the next call of the same shape
+                _capacity_hint[key] = max(_capacity_hint.get(key, 0), int(n * _HEADROOM) + 4096)
+                return color, radii, st, sums
+            capacity = int(n * _HEADROOM) + 4096
+            _capacity_hint[key] = capacity
 
 
-class _RasterizeFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, means, cov, opac, sh, means2d, cams, S, V, P, M, deg, sh_layout, cov_layout,
-                H, W, sort_impl, state_out, sh_basis):
-        backward_follows = any(ctx.needs_input_grad[:5])
-        color, radii, st = _forward_native(means, cov, opac, sh, cams, S, V, P, M, deg, sh_layout,
-                                           cov_layout, H, W, sort_impl, True, sh_basis, backward_follows)
-        ctx.save_for_backward(means, cov, opac, sh)
-        ctx.cams, ctx.st = cams, st
-        ctx.want_m2d = means2d is not None and means2d.requires_grad
-        if state_out is not None:
-            state_out.append(st)
-        ctx.mark_non_differentiable(radii)
-        return color, radii
+class _Rasterize(torch.autograd.Function):
+    """One forward (+ backward) of S scenes x V views.  Optional parts of the same pass: the squared-error epilogue
+    against `target` [S*V, 3, H, W] (SURVEY.md 8 row f-4) and the depth channel (cfg.depth_mode != 0).
+    Outputs (color, depth, radii, sse, sse_clipped):
+      color [S*V, 3, H, W]  differentiable without a target; detached with one (empty when not cfg.want_color);
+      depth [S*V, H, W]     differentiable; None without the depth channel;
+      sse [S*V]             sum over the view's pixels and channels of (C - target)^2, differentiable; its gradient
+                            g reaches the composite backward as the per-view scale 2 g of (C - target), formed
+                            in-kernel.  sse_clipped is the same on images clipped to [0, 1].  Both None without a
+                            target.
+    `means2d` [S*V, P, 3] is upstream's gradient holder: it takes no part in the forward and receives the gradient
+    with respect to the projected means.  When no gradient reaches `depth` the backward is the colour-only one
+    (ps_raster_backward without a target, ps_raster_backward_loss with one)."""
 
     @staticmethod
-    def backward(ctx, d_color, _d_radii):
-        means, cov, opac, sh = ctx.saved_tensors
-        st: RasterOutputState = ctx.st
-        st.verify()
-        desc, cams = st.desc, ctx.cams
-        dev = means.device
-        d_color = d_color.contiguous()
-        if d_color.dtype != torch.float32:
-            d_color = d_color.float()
-        sz = _lib.sizes(desc)
-        scratch = torch.empty(sz.backward_bytes, dtype=torch.uint8, device=dev)
-        d_means = torch.empty_like(means)
-        d_cov = torch.empty_like(cov)
-        d_opac = torch.empty_like(opac)
-        d_sh = torch.empty_like(sh)
-        VT = desc.n_scenes * desc.views_per_scene
-        d_m2d = (torch.empty((VT, desc.n_gaussians, 3), dtype=torch.float32, device=dev)
-                 if ctx.want_m2d else None)
-        inputs = _lib.RasterInputs(
-            means.data_ptr(), cov.data_ptr(), opac.data_ptr(), sh.data_ptr(),
-            cams["viewmatrix"].data_ptr(), cams["projmatrix"].data_ptr(), cams["campos"].data_ptr(),
-            cams["tanfov"].data_ptr(), cams["background"].data_ptr(),
-            cams["scene_scale"].data_ptr() if cams.get("scene_scale") is not None else None)
-        grads = _lib.RasterGrads(d_means.data_ptr(), d_cov.data_ptr(), d_opac.data_ptr(),
-                                 d_sh.data_ptr(), d_m2d.data_ptr() if d_m2d is not None else None)
-        state = st.raw_state()
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev)
-            rc = _lib.lib.ps_raster_backward(ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state),
-                                             ctypes.c_void_p(d_color.data_ptr()),
-                                             ctypes.c_void_p(scratch.data_ptr()), scratch.numel(),
-                                             ctypes.byref(grads), ctypes.c_void_p(stream.cuda_stream))
-        _lib.check(rc, "ps_raster_backward")
-        return (d_means, d_cov, d_opac, d_sh, d_m2d) + (None,) * 13
-
-
-def rasterize_gaussians(
-    means: Tensor,            # [S, P, 3]
-    covariances: Tensor,      # [S, P, 6] (triu) or [S, P, 3, 3]
-    opacities: Tensor,        # [S, P]
-    colors: Tensor,           # SH [S, P, M, 3] / [S, P, 3, M], or precomputed RGB [S, P, 3]
-    *,
-    viewmatrix: Tensor,       # [S*V, 16] or [S*V, 4, 4], column-major flattening (see header)
-    projmatrix: Tensor,       # same
-    campos: Tensor,           # [S*V, 3]
-    tanfov: Tensor,           # [S*V, 2]
-    background: Tensor,       # [S*V, 3]
-    image_shape: tuple[int, int],
-    views_per_scene: int,
-    sh_degree: int,
-    use_sh: bool = True,
-    sh_layout: int = PS_SH_M3,
-    scene_scale: Optional[Tensor] = None,   # [S*V]
-    sort_impl: int = 0,
-    state_out: Optional[list] = None,
-    means2d: Optional[Tensor] = None,       # [S*V, P, 3] gradient holder (upstream's means2D)
-    sh_basis=None,                          # "3dgs" / "e3nn"; None = the module default (set_sh_basis)
-) -> tuple[Tensor, Tensor]:
-    """Batched differentiable rasterization: S scenes x V views in one set of launches.
-    Returns (color [S*V, 3, H, W], radii [S*V, P] int32)."""
-    means, covariances, opacities, colors, cams, S, V, P, M, cov_layout, H, W = _prepare(
-        means, covariances, opacities, colors, viewmatrix, projmatrix, campos, tanfov, background, image_shape,
-        views_per_scene, use_sh, sh_layout, scene_scale)
-    VT = S * V
-    if means2d is not None and tuple(means2d.shape) != (VT, P, 3):
-        raise ValueError(f"means2d must be [S*V, P, 3], got {tuple(means2d.shape)}")
-    return _RasterizeFn.apply(means, covariances, opacities, colors, means2d, cams, S, V, P, M,
-                              int(sh_degree), sh_layout, cov_layout, int(H), int(W), int(sort_impl),
-                              state_out, _SH_BASIS if sh_basis is None else convention_id(sh_basis))
-
-
-class _RasterizeMseFn(torch.autograd.Function):
-    """Rasterize + squared error against a target in one pass (SURVEY.md 8 row f-4).  Differentiable output:
-    sse [S*V] = sum over the view's pixels and channels of (C - target)^2; its gradient g [S*V] reaches the
-    composite backward as the per-view scale 2 g of (C - target), formed in-kernel."""
-
-    @staticmethod
-    def forward(ctx, means, cov, opac, sh, target, cams, S, V, P, M, deg, sh_layout, cov_layout, H, W, sort_impl,
-                state_out, sh_basis, want_color):
-        backward_follows = any(ctx.needs_input_grad[:4])
-        color, radii, st, sums = _forward_native(means, cov, opac, sh, cams, S, V, P, M, deg, sh_layout, cov_layout,
-                                                 H, W, sort_impl, True, sh_basis, backward_follows,
-                                                 loss_target=target, want_color=want_color)
-        ctx.save_for_backward(means, cov, opac, sh, target)
-        ctx.cams, ctx.st = cams, st
-        if state_out is not None:
-            state_out.append(st)
-        totals = sums.sum(dim=-1)                                    # [S*V, 2]
-        sse, sse_clipped = totals[:, 0].contiguous(), totals[:, 1].contiguous()
-        if color is None:
-            color = torch.empty(0, device=means.device)
-        ctx.mark_non_differentiable(sse_clipped, color, radii)
-        return sse, sse_clipped, color, radii
-
-    @staticmethod
-    def backward(ctx, d_sse, _d_clip, _d_color, _d_radii):
-        means, cov, opac, sh, target = ctx.saved_tensors
-        st: RasterOutputState = ctx.st
-        st.verify()
-        desc, cams = st.desc, ctx.cams
-        dev = means.device
-        scale = (2.0 * d_sse).to(torch.float32).contiguous()
-        sz = _lib.sizes(desc)
-        scratch = torch.empty(sz.backward_bytes, dtype=torch.uint8, device=dev)
-        d_means, d_cov = torch.empty_like(means), torch.empty_like(cov)
-        d_opac, d_sh = torch.empty_like(opac), torch.empty_like(sh)
-        inputs = _lib.RasterInputs(
-            means.data_ptr(), cov.data_ptr(), opac.data_ptr(), sh.data_ptr(),
-            cams["viewmatrix"].data_ptr(), cams["projmatrix"].data_ptr(), cams["campos"].data_ptr(),
-            cams["tanfov"].data_ptr(), cams["background"].data_ptr(),
-            cams["scene_scale"].data_ptr() if cams.get("scene_scale") is not None else None)
-        grads = _lib.RasterGrads(d_means.data_ptr(), d_cov.data_ptr(), d_opac.data_ptr(), d_sh.data_ptr(), None)
-        state = st.raw_state()
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev)
-            rc = _lib.lib.ps_raster_backward_loss(ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state),
-                                                  ctypes.c_void_p(target.data_ptr()), ctypes.c_void_p(scale.data_ptr()),
-                                                  ctypes.c_void_p(scratch.data_ptr()), scratch.numel(),
-                                                  ctypes.byref(grads), ctypes.c_void_p(stream.cuda_stream))
-        _lib.check(rc, "ps_raster_backward_loss")
-        return (d_means, d_cov, d_opac, d_sh) + (None,) * 15
-
-
-class _RasterizeDepthFn(torch.autograd.Function):
-    """_RasterizeFn (target None) or _RasterizeMseFn (target given) with the depth channel composited in the same
-    pass.  Outputs (color, depth [S*V, H, W], radii, sse, sse_clipped); sse / sse_clipped are empty without a
-    target, and with one the colour is detached (as in _RasterizeMseFn).  When no gradient reaches `depth` the
-    backward is the colour-only one (ps_raster_backward / ps_raster_backward_loss)."""
-
-    @staticmethod
-    def forward(ctx, means, cov, opac, sh, target, cams, S, V, P, M, deg, sh_layout, cov_layout, H, W, sort_impl,
-                state_out, sh_basis, depth_mode, want_color):
+    def forward(ctx, means, cov, opac, sh, means2d, target, cams, cfg: _Config, state_out):
         ctx.set_materialize_grads(False)
-        backward_follows = any(ctx.needs_input_grad[:4])
-        out = _forward_native(means, cov, opac, sh, cams, S, V, P, M, deg, sh_layout, cov_layout, H, W, sort_impl,
-                              True, sh_basis, backward_follows, loss_target=target,
-                              want_color=want_color or target is None, depth_mode=depth_mode)
-        color, radii, st = out[:3]
-        depth = st.depth_image().clone()
+        backward_follows = any(ctx.needs_input_grad[:5])
+        color, radii, st, sums = _forward(means, cov, opac, sh, cams, cfg, backward_follows, target)
         ctx.save_for_backward(means, cov, opac, sh, target)
         ctx.cams, ctx.st = cams, st
         if state_out is not None:
             state_out.append(st)
-        if target is None:
-            sse = sse_clipped = torch.empty(0, device=means.device)
-        else:
-            totals = out[3].sum(dim=-1)                              # [S*V, 2]
+        depth = st.depth_image().clone() if cfg.depth_mode else None
+        sse = sse_clipped = None
+        if target is not None:
+            totals = sums.sum(dim=-1)                                # [S*V, 2]
             sse, sse_clipped = totals[:, 0].contiguous(), totals[:, 1].contiguous()
             if color is None:
                 color = torch.empty(0, device=means.device)
-            ctx.mark_non_differentiable(color)
-        ctx.mark_non_differentiable(radii, sse_clipped)
+            ctx.mark_non_differentiable(color, sse_clipped)
+        ctx.mark_non_differentiable(radii)
         return color, depth, radii, sse, sse_clipped
 
     @staticmethod
@@ -467,92 +329,52 @@ class _RasterizeDepthFn(torch.autograd.Function):
         means, cov, opac, sh, target = ctx.saved_tensors
         st: RasterOutputState = ctx.st
         st.verify()
-        desc, cams = st.desc, ctx.cams
+        desc = st.desc
         dev = means.device
         VT = desc.n_scenes * desc.views_per_scene
-        f32 = lambda t: t.to(torch.float32).contiguous()
         if target is None:
+            # no dL/dC when only the depth reached the loss
             d_color = (torch.zeros((VT, 3, desc.height, desc.width), dtype=torch.float32, device=dev)
-                       if d_color is None else f32(d_color))
+                       if d_color is None else d_color.to(torch.float32).contiguous())
+            scale = None
         else:
-            scale = 2.0 * (torch.zeros(VT, dtype=torch.float32, device=dev) if d_sse is None else f32(d_sse))
-        sz = _lib.sizes(desc)
-        scratch = torch.empty(sz.backward_bytes, dtype=torch.uint8, device=dev)
+            scale = (torch.zeros(VT, dtype=torch.float32, device=dev) if d_sse is None
+                     else (2.0 * d_sse).to(torch.float32).contiguous())
+        scratch = torch.empty(_lib.sizes(desc).backward_bytes, dtype=torch.uint8, device=dev)
         d_means, d_cov = torch.empty_like(means), torch.empty_like(cov)
         d_opac, d_sh = torch.empty_like(opac), torch.empty_like(sh)
-        inputs = _raster_inputs(means, cov, opac, sh, cams)
-        grads = _lib.RasterGrads(d_means.data_ptr(), d_cov.data_ptr(), d_opac.data_ptr(), d_sh.data_ptr(), None)
+        d_m2d = (torch.empty((VT, desc.n_gaussians, 3), dtype=torch.float32, device=dev)
+                 if ctx.needs_input_grad[4] else None)
+        inputs = _raster_inputs(means, cov, opac, sh, ctx.cams)
+        grads = _lib.RasterGrads(d_means.data_ptr(), d_cov.data_ptr(), d_opac.data_ptr(), d_sh.data_ptr(),
+                                 d_m2d.data_ptr() if d_m2d is not None else None)
         state = st.raw_state()
-        p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
-        L = _lib.lib
-        with torch.cuda.device(dev):
-            stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            sc = (ctypes.c_void_p(scratch.data_ptr()), scratch.numel(), ctypes.byref(grads), stream)
-            if d_depth is not None:
-                d_depth = f32(d_depth)
-                rc = L.ps_raster_backward_depth(ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state),
-                                                p(d_color if target is None else None), p(target),
-                                                p(scale if target is not None else None), p(d_depth), *sc)
-                what = "ps_raster_backward_depth"
-            elif target is None:
-                rc = L.ps_raster_backward(ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state),
-                                          p(d_color), *sc)
-                what = "ps_raster_backward"
-            else:
-                rc = L.ps_raster_backward_loss(ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state),
-                                               p(target), p(scale), *sc)
-                what = "ps_raster_backward_loss"
-        _lib.check(rc, what)
-        return (d_means, d_cov, d_opac, d_sh) + (None,) * 16
+        if d_depth is not None:
+            d_depth = d_depth.to(torch.float32).contiguous()
+            fn = _lib.lib.ps_raster_backward_depth
+            args = (_ptr(d_color if target is None else None), _ptr(target), _ptr(scale), _ptr(d_depth))
+        elif target is None:
+            fn, args = _lib.lib.ps_raster_backward, (_ptr(d_color),)
+        else:
+            fn, args = _lib.lib.ps_raster_backward_loss, (_ptr(target), _ptr(scale))
+        stream = torch.cuda.current_stream(dev)
+        rc = _lib.on_device(dev, fn, ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state), *args,
+                            _ptr(scratch), scratch.numel(), ctypes.byref(grads), ctypes.c_void_p(stream.cuda_stream))
+        _lib.check(rc, fn.__name__)
+        return d_means, d_cov, d_opac, d_sh, d_m2d, None, None, None, None
 
 
-def _near_far(near_far: Optional[Tensor], depth_mode: int, VT: int) -> Optional[Tensor]:
-    if depth_mode == 0:
-        raise ValueError(f"depth_mode must be one of {[k for k in _lib.DEPTH_MODES if k]}")
-    if near_far is None:
-        if depth_mode in (3, 4):
-            raise ValueError("depth modes relative_disparity and log need near_far [S*V, 2]")
-        return None
-    return _req(near_far, "near_far", (VT, 2))
-
-
-def rasterize_gaussians_with_depth(
-        means: Tensor, covariances: Tensor, opacities: Tensor, colors: Tensor, *, viewmatrix: Tensor,
-        projmatrix: Tensor, campos: Tensor, tanfov: Tensor, background: Tensor, image_shape: tuple[int, int],
-        views_per_scene: int, sh_degree: int, depth_mode: str, near_far: Optional[Tensor] = None,
-        use_sh: bool = True, sh_layout: int = PS_SH_M3, scene_scale: Optional[Tensor] = None, sort_impl: int = 0,
-        state_out: Optional[list] = None, sh_basis=None, target: Optional[Tensor] = None, want_color: bool = True):
-    """rasterize_gaussians with a depth channel composited in the same pass: the Gaussians' camera-space depth in
-    world units (view-space z / scene_scale), as `depth_mode` "depth" | "disparity" | "relative_disparity" | "log"
-    (the values render_depth_cuda composites), blended with the colour's alphas over a zero background.
-    `near_far` [S*V, 2] (world units) is needed by the last two modes.
-    Returns (color [S*V, 3, H, W], depth [S*V, H, W], radii), both images differentiable.  With `target`
-    [S*V, 3, H, W] the loss epilogue of rasterize_gaussians_mse runs too and the result is (sse [S*V]
-    differentiable, sse_clipped, color detached (empty when want_color=False), depth differentiable, radii)."""
-    means, covariances, opacities, colors, cams, S, V, P, M, cov_layout, H, W = _prepare(
-        means, covariances, opacities, colors, viewmatrix, projmatrix, campos, tanfov, background, image_shape,
-        views_per_scene, use_sh, sh_layout, scene_scale)
-    mode = _lib.DEPTH_MODES.get(depth_mode, 0)
-    cams["near_far"] = _near_far(near_far, mode, S * V)
-    if target is not None:
-        target = _req(target, "target", (S * V, 3, H, W))
-    color, depth, radii, sse, sse_clipped = _RasterizeDepthFn.apply(
-        means, covariances, opacities, colors, target, cams, S, V, P, M, int(sh_degree), sh_layout, cov_layout,
-        H, W, int(sort_impl), state_out, _SH_BASIS if sh_basis is None else convention_id(sh_basis), mode,
-        bool(want_color))
-    if target is None:
-        return color, depth, radii
-    return sse, sse_clipped, color, depth, radii
-
-
-def _prepare(means, covariances, opacities, colors, viewmatrix, projmatrix, campos, tanfov, background, image_shape,
-             views_per_scene, use_sh, sh_layout, scene_scale):
-    """Argument checks shared by rasterize_gaussians and rasterize_gaussians_mse."""
+def _rasterize(means, covariances, opacities, colors, *, viewmatrix, projmatrix, campos, tanfov, background,
+               image_shape, views_per_scene, sh_degree, use_sh=True, sh_layout=PS_SH_M3, scene_scale=None,
+               sort_impl=0, state_out=None, sh_basis=None, target=None, depth_mode=None, near_far=None,
+               want_color=True, means2d=None):
+    """Argument checks of every rasterizer entry point, then one _Rasterize: returns its (color, depth, radii, sse,
+    sse_clipped).  `depth_mode` is a key of _lib.DEPTH_MODES (None: no depth channel)."""
     if means.dim() != 3 or means.shape[-1] != 3:
         raise ValueError(f"means must be [S, P, 3], got {tuple(means.shape)}")
     S, P, _ = means.shape
     V = int(views_per_scene)
-    H, W = image_shape
+    H, W = map(int, image_shape)
     means = _req(means, "means", (S, P, 3))
     if covariances.dim() == 4:
         cov_layout = PS_COV_3X3
@@ -579,7 +401,52 @@ def _prepare(means, covariances, opacities, colors, viewmatrix, projmatrix, camp
         background=_req(background, "background", (VT, 3)),
         scene_scale=None if scene_scale is None else _req(scene_scale, "scene_scale", (VT,)),
     )
-    return means, covariances, opacities, colors, cams, S, V, P, M, cov_layout, int(H), int(W)
+    if depth_mode not in _lib.DEPTH_MODES:
+        raise ValueError(f"depth_mode must be one of {[k for k in _lib.DEPTH_MODES if k]}")
+    mode = _lib.DEPTH_MODES[depth_mode]
+    if near_far is not None:
+        cams["near_far"] = _req(near_far, "near_far", (VT, 2))
+    elif mode in (3, 4):
+        raise ValueError("depth modes relative_disparity and log need near_far [S*V, 2]")
+    if target is not None:
+        target = _req(target, "target", (VT, 3, H, W))
+    if means2d is not None and tuple(means2d.shape) != (VT, P, 3):
+        raise ValueError(f"means2d must be [S*V, P, 3], got {tuple(means2d.shape)}")
+    cfg = _Config(S, V, P, M, int(sh_degree), sh_layout, cov_layout, H, W, int(sort_impl),
+                  _SH_BASIS if sh_basis is None else convention_id(sh_basis), mode, bool(want_color) or target is None)
+    return _Rasterize.apply(means, covariances, opacities, colors, means2d, target, cams, cfg, state_out)
+
+
+def rasterize_gaussians(
+    means: Tensor,            # [S, P, 3]
+    covariances: Tensor,      # [S, P, 6] (triu) or [S, P, 3, 3]
+    opacities: Tensor,        # [S, P]
+    colors: Tensor,           # SH [S, P, M, 3] / [S, P, 3, M], or precomputed RGB [S, P, 3]
+    *,
+    viewmatrix: Tensor,       # [S*V, 16] or [S*V, 4, 4], column-major flattening (see header)
+    projmatrix: Tensor,       # same
+    campos: Tensor,           # [S*V, 3]
+    tanfov: Tensor,           # [S*V, 2]
+    background: Tensor,       # [S*V, 3]
+    image_shape: tuple[int, int],
+    views_per_scene: int,
+    sh_degree: int,
+    use_sh: bool = True,
+    sh_layout: int = PS_SH_M3,
+    scene_scale: Optional[Tensor] = None,   # [S*V]
+    sort_impl: int = 0,
+    state_out: Optional[list] = None,
+    means2d: Optional[Tensor] = None,       # [S*V, P, 3] gradient holder (upstream's means2D)
+    sh_basis=None,                          # "3dgs" / "e3nn"; None = the module default (set_sh_basis)
+) -> tuple[Tensor, Tensor]:
+    """Batched differentiable rasterization: S scenes x V views in one set of launches.
+    Returns (color [S*V, 3, H, W], radii [S*V, P] int32)."""
+    color, _, radii, _, _ = _rasterize(
+        means, covariances, opacities, colors, viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos,
+        tanfov=tanfov, background=background, image_shape=image_shape, views_per_scene=views_per_scene,
+        sh_degree=sh_degree, use_sh=use_sh, sh_layout=sh_layout, scene_scale=scene_scale, sort_impl=sort_impl,
+        state_out=state_out, sh_basis=sh_basis, means2d=means2d)
+    return color, radii
 
 
 def rasterize_gaussians_mse(means: Tensor, covariances: Tensor, opacities: Tensor, colors: Tensor, target: Tensor, *,
@@ -589,13 +456,38 @@ def rasterize_gaussians_mse(means: Tensor, covariances: Tensor, opacities: Tenso
                             state_out: Optional[list] = None, sh_basis=None, want_color: bool = True):
     """rasterize_gaussians + the loss epilogue: returns (sse [S*V] differentiable, sse_clipped [S*V], color
     [S*V, 3, H, W] detached (empty when want_color=False), radii).  `target` is [S*V, 3, H, W]."""
-    means, covariances, opacities, colors, cams, S, V, P, M, cov_layout, H, W = _prepare(
-        means, covariances, opacities, colors, viewmatrix, projmatrix, campos, tanfov, background, image_shape,
-        views_per_scene, use_sh, sh_layout, scene_scale)
-    target = _req(target, "target", (S * V, 3, H, W))
-    return _RasterizeMseFn.apply(means, covariances, opacities, colors, target, cams, S, V, P, M, int(sh_degree),
-                                 sh_layout, cov_layout, H, W, int(sort_impl), state_out,
-                                 _SH_BASIS if sh_basis is None else convention_id(sh_basis), bool(want_color))
+    color, _, radii, sse, sse_clipped = _rasterize(
+        means, covariances, opacities, colors, viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos,
+        tanfov=tanfov, background=background, image_shape=image_shape, views_per_scene=views_per_scene,
+        sh_degree=sh_degree, use_sh=use_sh, sh_layout=sh_layout, scene_scale=scene_scale, sort_impl=sort_impl,
+        state_out=state_out, sh_basis=sh_basis, target=target, want_color=want_color)
+    return sse, sse_clipped, color, radii
+
+
+def rasterize_gaussians_with_depth(
+        means: Tensor, covariances: Tensor, opacities: Tensor, colors: Tensor, *, viewmatrix: Tensor,
+        projmatrix: Tensor, campos: Tensor, tanfov: Tensor, background: Tensor, image_shape: tuple[int, int],
+        views_per_scene: int, sh_degree: int, depth_mode: str, near_far: Optional[Tensor] = None,
+        use_sh: bool = True, sh_layout: int = PS_SH_M3, scene_scale: Optional[Tensor] = None, sort_impl: int = 0,
+        state_out: Optional[list] = None, sh_basis=None, target: Optional[Tensor] = None, want_color: bool = True):
+    """rasterize_gaussians with a depth channel composited in the same pass: the Gaussians' camera-space depth in
+    world units (view-space z / scene_scale), as `depth_mode` "depth" | "disparity" | "relative_disparity" | "log"
+    (the values render_depth_cuda composites), blended with the colour's alphas over a zero background.
+    `near_far` [S*V, 2] (world units) is needed by the last two modes.
+    Returns (color [S*V, 3, H, W], depth [S*V, H, W], radii), both images differentiable.  With `target`
+    [S*V, 3, H, W] the loss epilogue of rasterize_gaussians_mse runs too and the result is (sse [S*V]
+    differentiable, sse_clipped, color detached (empty when want_color=False), depth differentiable, radii)."""
+    if depth_mode is None:
+        raise ValueError("rasterize_gaussians_with_depth needs a depth_mode")
+    color, depth, radii, sse, sse_clipped = _rasterize(
+        means, covariances, opacities, colors, viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos,
+        tanfov=tanfov, background=background, image_shape=image_shape, views_per_scene=views_per_scene,
+        sh_degree=sh_degree, use_sh=use_sh, sh_layout=sh_layout, scene_scale=scene_scale, sort_impl=sort_impl,
+        state_out=state_out, sh_basis=sh_basis, target=target, depth_mode=depth_mode, near_far=near_far,
+        want_color=want_color)
+    if target is None:
+        return color, depth, radii
+    return sse, sse_clipped, color, depth, radii
 
 
 # ------------------------------------------------------------------ drop-in extension surface
