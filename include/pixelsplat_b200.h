@@ -183,10 +183,21 @@ PS_API int ps_timing_read(float *ms);
  *                         1 = always keep the forward's per-block hit lists for the backward (binning_bytes grows).
  * Takes effect for forwards issued afterwards (a backward uses the split and the hit lists its forward used only if
  * the options are unchanged in between).  Also read once from PIXELSPLAT_B200_COMPOSITE / PIXELSPLAT_B200_SEGMENTS /
- * PIXELSPLAT_B200_HIT_LISTS. */
+ * PIXELSPLAT_B200_HIT_LISTS.
+ *   "deterministic"       0 = off (default), 1 = fixed-order composite backward and loss epilogue: the same inputs, call
+ *                         shape, options and GPU give the same bits on every run (no float atomics on the rasterizer
+ *                         path).  Takes effect for calls issued afterwards (sizes queried, forwards and backwards).
+ *                         The legacy compositor has no fixed-order form: with the option on its forward and backward
+ *                         return PS_ERR_UNSUPPORTED before anything is enqueued.  Workspace with the option on, where
+ *                         A(x) rounds x up to a multiple of 256, C = instance_capacity, T = S*V*tiles (16x16 tiles):
+ *                           backward_bytes = A(8 S V P) + A(16 S V P) + A(16 S V P)           (as with the option off)
+ *                                          + A(8 * 8C) + A(16 * 8C) + A(16 * 8C)  the composite's per-(tile block, list
+ *                                                                                 position) gradient records;
+ *                           image_bytes    = (the size with the option off) + A(8 * 8T)  per-warp-task loss partials.
+ *                         geom_bytes, binning_bytes and the ps_raster_layout offsets do not change. */
 PS_API int ps_set_option(const char *name, int value);
 /* The value of an option above as it is in force (the environment included): composite_impl 1 | 2,
- * composite_segments 0 | 1 | 2 | 4, composite_hit_lists 0 | 1 | 2. */
+ * composite_segments 0 | 1 | 2 | 4, composite_hit_lists 0 | 1 | 2, deterministic 0 | 1. */
 PS_API int ps_get_option(const char *name, int *value);
 
 /* Workspace sizes / layout for a descriptor. */

@@ -163,13 +163,19 @@ int launch_preprocess(const Dims &d, const Inputs &in, const Geom &g, cudaStream
 int launch_sh_color(const Dims &d, const Inputs &in, const Geom &g, cudaStream_t st);
 int launch_binning(const Dims &d, const Geom &g, unsigned long long *keys,
                    unsigned long long *keys_alt, int sort_impl, int segment_hint, cudaStream_t st);
+// Deterministic mode (ps_set_option "deterministic"): the forward's loss epilogue goes through loss_partials
+// ([S*V*tiles*8] float2 per-task (sse, sse_clipped), image state) and a fixed-order finish; the backward stores into
+// `records` (the per-(tile block, list position) gradients, 8 x instance_capacity entries of each array, backward
+// scratch) and gathers them into vg in a fixed order.  Null = the default float-atomic path.
 int launch_composite_forward(const Dims &d, const Inputs &in, const Geom &g,
                              const unsigned long long *keys, const ImageState &img,
-                             float *out_color, const LossEpilogue &loss, const HitLists &hl, cudaStream_t st);
+                             float *out_color, const LossEpilogue &loss, const HitLists &hl, float *loss_partials,
+                             cudaStream_t st);
 int launch_composite_backward(const Dims &d, const Inputs &in, const Geom &g,
                               const unsigned long long *keys, const ImageState &img,
                               const float *d_color, const float *d_depth, const ViewGrads &vg,
-                              const LossEpilogue &loss, const HitLists &hl, cudaStream_t st);
+                              const ViewGrads *records, const LossEpilogue &loss, const HitLists &hl,
+                              cudaStream_t st);
 // legacy CTA-per-tile compositor (round 1), kept selectable for A/B measurements
 int launch_composite_forward_v1(const Dims &d, const Inputs &in, const Geom &g,
                                 const unsigned long long *keys, const ImageState &img,

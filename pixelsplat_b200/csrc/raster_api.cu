@@ -75,9 +75,16 @@ static int side_ready(SideCtx *&ctx) {
 
 static size_t align_up(size_t x) { return (x + 255) & ~(size_t)255; }
 
+// Deterministic mode (ps_set_option "deterministic"): fixed-order composite backward and loss epilogue.  Read once
+// per call, by make_layout.
+static int g_deterministic = 0;
+
 struct Layout {
     ps_raster_layout off;
     ps_raster_sizes sizes;
+    bool det;                    // deterministic mode: the two arrays below exist
+    size_t loss_partials;        // image: f32x2 [S*V*tiles*8] per-task (sse, sse_clipped) of the loss epilogue
+    size_t records;              // backward scratch: the composite's block records (d_mean2d, d_conic, d_color)
 };
 
 static int validate(const ps_raster_desc *d) {
@@ -176,9 +183,17 @@ static Layout make_layout(const ps_raster_desc *d) {
         L.off.depth_image = take(px * 4);
         L.off.run_depth = take(px * 4 * (kMaxSegments - 1));
     }
+    L.det = g_deterministic != 0;
+    L.loss_partials = L.det ? take(vt * 8 * 8) : 0;
     L.sizes.image_bytes = o;
-    // backward scratch: d_mean2d (8) + d_conic (16) + d_color (16) per (view, Gaussian)
+    // backward scratch: d_mean2d (8) + d_conic (16) + d_color (16) per (view, Gaussian); deterministic mode: the
+    // same per (tile block, list position), 8 x instance_capacity of them
     L.sizes.backward_bytes = align_up(vp * 8) + align_up(vp * 16) + align_up(vp * 16);
+    L.records = L.sizes.backward_bytes;
+    if (L.det) {
+        const size_t nr = (size_t)m.capacity * 8;
+        L.sizes.backward_bytes += align_up(nr * 8) + align_up(nr * 16) + align_up(nr * 16);
+    }
     return L;
 }
 
@@ -214,8 +229,11 @@ static ImageState make_image(const Layout &L, void *image) {
     return im;
 }
 
+// `backward`: the image state needs no room for the loss partials (a forward issued before the option was set
+// followed by a backward issued after it is fine).
 static int check_common(const ps_raster_desc *desc, const ps_raster_inputs *in, const ps_raster_state *state,
-                        const Layout &L) {
+                        const Layout &L, bool backward) {
+    const size_t image_bytes = backward && L.det ? L.loss_partials : L.sizes.image_bytes;
     if (!in || !state) { set_error("inputs/state is NULL"); return PS_ERR_INVALID_ARGUMENT; }
     if (!in->means || !in->cov || !in->opacities || !in->sh || !in->viewmatrix || !in->projmatrix ||
         !in->campos || !in->tanfov || !in->background) {
@@ -224,9 +242,9 @@ static int check_common(const ps_raster_desc *desc, const ps_raster_inputs *in, 
     }
     if (!state->geom || !state->binning || !state->image) { set_error("a state buffer is NULL"); return PS_ERR_INVALID_ARGUMENT; }
     if (state->geom_bytes < L.sizes.geom_bytes || state->binning_bytes < L.sizes.binning_bytes ||
-        state->image_bytes < L.sizes.image_bytes) {
+        state->image_bytes < image_bytes) {
         set_error("state buffers too small: need geom %zu binning %zu image %zu, got %zu %zu %zu",
-                  L.sizes.geom_bytes, L.sizes.binning_bytes, L.sizes.image_bytes, state->geom_bytes,
+                  L.sizes.geom_bytes, L.sizes.binning_bytes, image_bytes, state->geom_bytes,
                   state->binning_bytes, state->image_bytes);
         return PS_ERR_INVALID_ARGUMENT;
     }
@@ -240,6 +258,10 @@ static int check_common(const ps_raster_desc *desc, const ps_raster_inputs *in, 
     }
     if (desc->depth_mode && composite_impl() == 1) {
         set_error("the legacy compositor (composite_impl = 1) has no depth channel");
+        return PS_ERR_UNSUPPORTED;
+    }
+    if (L.det && composite_impl() == 1) {
+        set_error("the legacy compositor (composite_impl = 1) has no fixed-order (deterministic) form");
         return PS_ERR_UNSUPPORTED;
     }
     return PS_OK;
@@ -286,6 +308,7 @@ PS_API int ps_set_option(const char *name, int value) {
     if (!strcmp(name, "composite_impl")) rc = set_composite_option(0, value);
     else if (!strcmp(name, "composite_segments")) rc = set_composite_option(1, value);
     else if (!strcmp(name, "composite_hit_lists")) rc = set_composite_option(2, value);
+    else if (!strcmp(name, "deterministic") && (value == 0 || value == 1)) { g_deterministic = value; rc = PS_OK; }
     if (rc) set_error("ps_set_option: unknown option or bad value: %s = %d", name, value);
     return rc;
 }
@@ -296,6 +319,7 @@ PS_API int ps_get_option(const char *name, int *value) {
     if (!strcmp(name, "composite_impl")) which = 0;
     else if (!strcmp(name, "composite_segments")) which = 1;
     else if (!strcmp(name, "composite_hit_lists")) which = 2;
+    else if (!strcmp(name, "deterministic")) { *value = g_deterministic; return PS_OK; }
     if (which < 0) { set_error("ps_get_option: unknown option %s", name); return PS_ERR_INVALID_ARGUMENT; }
     *value = get_composite_option(which);
     return PS_OK;
@@ -325,7 +349,7 @@ static int raster_forward_impl(const ps_raster_desc *desc, const ps_raster_input
     int rc = validate(desc);
     if (rc) return rc;
     const Layout L = make_layout(desc);
-    rc = check_common(desc, in, state, L);
+    rc = check_common(desc, in, state, L, false);
     if (rc) return rc;
     LossEpilogue le{nullptr, nullptr, nullptr};
     if (loss) {
@@ -360,14 +384,16 @@ static int raster_forward_impl(const ps_raster_desc *desc, const ps_raster_input
     PS_CUDA_CHECK(cudaStreamWaitEvent(st, sc->join, 0));   // join
     if (n_instances_host)
         PS_CUDA_CHECK(cudaMemcpyAsync(n_instances_host, g.n_instances, 2 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    if (le.sums)
+    // (deterministic mode: the fixed-order finish writes every slot)
+    float *loss_partials = L.det ? reinterpret_cast<float *>(static_cast<char *>(state->image) + L.loss_partials) : nullptr;
+    if (le.sums && !loss_partials)
         PS_CUDA_CHECK(cudaMemsetAsync(le.sums, 0, sizeof(float) * 2 * kLossSlots * (size_t)d.S * d.V, st));
     HitLists hl{nullptr, nullptr};
     if (d.hit_lists) {
         hl.hits = reinterpret_cast<uint2 *>(static_cast<char *>(state->binning) + L.off.block_hits);
         hl.run_hits = reinterpret_cast<uint32_t *>(static_cast<char *>(state->binning) + L.off.run_hits);
     }
-    if ((rc = launch_composite_forward(d, I, g, keys, img, out_color, le, hl, st))) return rc;
+    if ((rc = launch_composite_forward(d, I, g, keys, img, out_color, le, hl, loss_partials, st))) return rc;
     mark(kMarkCompositeFwd, st);
     if (out_radii)
         PS_CUDA_CHECK(cudaMemcpyAsync(out_radii, g.radii, sizeof(int32_t) * (size_t)d.S * d.V * d.P,
@@ -398,7 +424,7 @@ static int raster_backward_impl(const ps_raster_desc *desc, const ps_raster_inpu
     int rc = validate(desc);
     if (rc) return rc;
     const Layout L = make_layout(desc);
-    rc = check_common(desc, in, state, L);
+    rc = check_common(desc, in, state, L, true);
     if (rc) return rc;
     if ((!d_color && !(target && grad_scale)) || !scratch || !grads) {
         set_error("d_color (or target + grad_scale) / scratch / grads is NULL");
@@ -426,6 +452,11 @@ static int raster_backward_impl(const ps_raster_desc *desc, const ps_raster_inpu
     vg.d_mean2d = reinterpret_cast<float2 *>(sb);
     vg.d_conic = reinterpret_cast<float4 *>(sb + align_up(vp * 8));
     vg.d_color = reinterpret_cast<float4 *>(sb + align_up(vp * 8) + align_up(vp * 16));
+    ViewGrads rec;                      // deterministic mode: the block records, after the per-(view, Gaussian) arrays
+    const size_t nr = (size_t)d.capacity * 8;
+    rec.d_mean2d = reinterpret_cast<float2 *>(sb + L.records);
+    rec.d_conic = reinterpret_cast<float4 *>(sb + L.records + align_up(nr * 8));
+    rec.d_color = reinterpret_cast<float4 *>(sb + L.records + align_up(nr * 8) + align_up(nr * 16));
     SideCtx *sc = nullptr;
     if ((rc = side_ready(sc))) return rc;
     std::lock_guard<std::mutex> enqueue_lock(sc->enqueue);
@@ -442,7 +473,8 @@ static int raster_backward_impl(const ps_raster_desc *desc, const ps_raster_inpu
         hl.hits = reinterpret_cast<uint2 *>(static_cast<char *>(state->binning) + L.off.block_hits);
         hl.run_hits = reinterpret_cast<uint32_t *>(static_cast<char *>(state->binning) + L.off.run_hits);
     }
-    if ((rc = launch_composite_backward(d, I, g, keys, img, d_color, d_depth, vg, le, hl, st))) return rc;
+    if ((rc = launch_composite_backward(d, I, g, keys, img, d_color, d_depth, vg, L.det ? &rec : nullptr, le, hl, st)))
+        return rc;
     mark(kMarkCompositeBwd, st);
     PS_CUDA_CHECK(cudaStreamWaitEvent(st, sc->join, 0));   // join
     if ((rc = launch_preprocess_backward(d, I, g, vg, *grads, st))) return rc;

@@ -48,6 +48,19 @@
 //             The state in front of each run, (T, C), is kept per pixel for the backward.
 //   backward: the forward-order prefix form needs only (T, S = C . dL/dC) in front of a run, which the
 //             forward stored, so the runs are independent warps with no combination step at all.
+//
+// Fixed-order (DET) instantiations, for the "deterministic" option (include/pixelsplat_b200.h): the same kernels
+// with the two float-atomic sums replaced by stores and a fixed-order reduction afterwards.
+//   backward: phase 2 STORES its ten numbers (d_mean2d x2, d_conic x3, d_opacity, d_color x3, depth lane) into the
+//             record of (tile block, list position): index tile_start * 8 + block * count + position, the index space
+//             of the forward's hit lists.  Each record has exactly one writer: a list position lies in exactly one run
+//             (K = 1 / 2 / 4), each (tile, block) is exactly one warp task, and a task queues a position at most once.
+//             k_gather_block_records then sums, per on-screen (view, Gaussian), its records in a fixed order (tiles
+//             row-major within a block, then blocks 0..7) and stores the per-(view, Gaussian) gradients
+//             k_preprocess_bwd reads.
+//   forward : the loss epilogue stores each warp task's (sse, sse_clipped) pair; k_loss_finish sums each view's
+//             tasks in a fixed order into the PS_LOSS_SLOTS slots.
+// Everything else (K, hit lists, cull, the arithmetic that forms the numbers) is the default instantiations'.
 #include <cstdlib>
 
 #include "ps_common.cuh"
@@ -321,8 +334,10 @@ __device__ __forceinline__ uint32_t fwd_run(const Geom &geo, const TaskGeom &t, 
 
 // DEPTH instantiations carry one more accumulator through the same loop (and the fold of the K > 1 runs); they are
 // built for fewer resident CTAs (5, or 4 with runs) so that it does not spill.
-template <int K, bool DEPTH>
-__global__ void __launch_bounds__(kFwdWarps * 32, DEPTH ? (K > 1 ? 4 : 5) : PS_FWD_MIN_CTAS)
+// DET: loss.sums is the per-task partials array [S*V*tiles*8] of (sse, sse_clipped) (see the file header); the colour-
+// only DET instantiations are built for the DEPTH ones' CTA counts so that they do not spill.
+template <int K, bool DEPTH, bool DET>
+__global__ void __launch_bounds__(kFwdWarps * 32, (DEPTH || DET) ? (K > 1 ? 4 : 5) : PS_FWD_MIN_CTAS)
 k_composite_fwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsigned long long *__restrict__ keys,
                  ImageState img, float *__restrict__ out_color, LossEpilogue loss, HitLists hl) {
     __shared__ HitQueue s_q[kFwdWarps];
@@ -419,12 +434,33 @@ k_composite_fwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
             sse_clip += __shfl_xor_sync(0xffffffffu, sse_clip, o);
         }
         if (lane == 0) {
-            const int slot = (int)((blockIdx.x * kTasksPerCta + warp / K) & (kLossSlots - 1));
-            float *dst = loss.sums + ((size_t)t.vid * 2) * kLossSlots + slot;
-            atomicAdd(dst, sse);
-            atomicAdd(dst + kLossSlots, sse_clip);
+            if constexpr (DET) {
+                // this task's own pair; k_loss_finish sums them per view in a fixed order
+                reinterpret_cast<float2 *>(loss.sums)[(long long)blockIdx.x * kTasksPerCta + warp / K] =
+                    make_float2(sse, sse_clip);
+            } else {
+                const int slot = (int)((blockIdx.x * kTasksPerCta + warp / K) & (kLossSlots - 1));
+                float *dst = loss.sums + ((size_t)t.vid * 2) * kLossSlots + slot;
+                atomicAdd(dst, sse);
+                atomicAdd(dst + kLossSlots, sse_clip);
+            }
         }
     }
+}
+
+// Fixed-order finish of the DET loss epilogue: block = view, thread s sums the view's tasks s, s + 64, ... in order.
+__global__ void __launch_bounds__(kLossSlots)
+k_loss_finish(const float2 *__restrict__ partials, int tasks_per_view, float *__restrict__ sums) {
+    const int vid = blockIdx.x, s = threadIdx.x;
+    const float2 *p = partials + (size_t)vid * tasks_per_view;
+    float raw = 0.0f, clipped = 0.0f;
+    for (int i = s; i < tasks_per_view; i += kLossSlots) {
+        const float2 v = p[i];
+        raw += v.x;
+        clipped += v.y;
+    }
+    sums[(size_t)vid * 2 * kLossSlots + s] = raw;
+    sums[((size_t)vid * 2 + 1) * kLossSlots + s] = clipped;
 }
 
 // ================================================================================== backward
@@ -451,9 +487,10 @@ struct BwdPixel {
 
 // Phase 1 + phase 2 for the queue entries [head, head + cnt), head a multiple of kBatch, cnt <= kBatch
 // (warp-uniform; entries up to the next multiple of four exist as zero-opacity padding).
-template <bool FULL, bool DEPTH>
+// DET: vg points at the block records and rbase = tile_start * 8 + block * count (see the file header).
+template <bool FULL, bool DEPTH, bool DET>
 __device__ __forceinline__ void bwd_batch(BwdSmem<DEPTH> &sm, BwdPixel &px, const TaskGeom &t, const ViewGrads &vg,
-                                          uint32_t head, int cnt, float kx, float ky, int lane) {
+                                          uint32_t head, int cnt, float kx, float ky, int lane, size_t rbase) {
     // ---- phase 1: lane = pixel, entries front to back
     const uint32_t base = head & (kQ - 1);
 #pragma unroll
@@ -522,15 +559,24 @@ __device__ __forceinline__ void bwd_batch(BwdSmem<DEPTH> &sm, BwdPixel &px, cons
         const size_t rec = t.gbase + __float_as_uint(b2.w);
         // u excludes the opacity factor: position / conic terms pick it up here, dL/dopacity does not
         const float ox = o * s_x, oy = o * s_y;
-        red_add_v2(vg.d_mean2d + rec, kx * (2.0f * b1.x * ox + b1.y * oy), ky * (2.0f * b1.z * oy + b1.y * ox));
-        red_add_v4(vg.d_conic + rec, -0.5f * o * s_xx, -0.5f * o * s_xy, -0.5f * o * s_yy, s_u);
-        red_add_v4(vg.d_color + rec, s_r, s_g, s_b, DEPTH ? s_d : 0.0f);
+        if constexpr (DET) {
+            // the record of (this block, the hit's list position): its only writer, so a plain store
+            const size_t r = rbase + __float_as_uint(b1.w);
+            vg.d_mean2d[r] = make_float2(kx * (2.0f * b1.x * ox + b1.y * oy), ky * (2.0f * b1.z * oy + b1.y * ox));
+            vg.d_conic[r] = make_float4(-0.5f * o * s_xx, -0.5f * o * s_xy, -0.5f * o * s_yy, s_u);
+            vg.d_color[r] = make_float4(s_r, s_g, s_b, DEPTH ? s_d : 0.0f);
+        } else {
+            red_add_v2(vg.d_mean2d + rec, kx * (2.0f * b1.x * ox + b1.y * oy), ky * (2.0f * b1.z * oy + b1.y * ox));
+            red_add_v4(vg.d_conic + rec, -0.5f * o * s_xx, -0.5f * o * s_xy, -0.5f * o * s_yy, s_u);
+            red_add_v4(vg.d_color + rec, s_r, s_g, s_b, DEPTH ? s_d : 0.0f);
+        }
     }
     __syncwarp();
 }
 
 // DEPTH: dL/dD = d_depth rides along (see bwd_batch); built for 5 resident CTAs so that it does not spill.
-template <int K, bool DEPTH>
+// DET: vg points at the block records (see the file header).
+template <int K, bool DEPTH, bool DET>
 __global__ void __launch_bounds__(kBwdWarps * 32, DEPTH ? 5 : 6)
 k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsigned long long *__restrict__ keys,
                  ImageState img, const float *__restrict__ d_color, const float *__restrict__ d_depth, ViewGrads vg,
@@ -584,6 +630,10 @@ k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
     t.run_len = n;
     const float kx = kLn2 * 0.5f * (float)d.W, ky = kLn2 * 0.5f * (float)d.H;
     (void)bg_all;
+    // DET: this block's records of the tile's list (the hit lists' index space)
+    const size_t rbase = DET ? (size_t)t.start * 8 + (size_t)(((long long)blockIdx.x * kTasksPerCta + warp / K) & 7) *
+                                                         t.count
+                             : 0;
 
     uint32_t head = 0, tail = 0;
     if (hl.hits) {
@@ -619,7 +669,7 @@ k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
             tail += (uint32_t)__popc(m);
             __syncwarp();
             while (tail - head >= (uint32_t)kBatch) {
-                bwd_batch<true, DEPTH>(sm, px, t, vg, head, kBatch, kx, ky, lane);
+                bwd_batch<true, DEPTH, DET>(sm, px, t, vg, head, kBatch, kx, ky, lane, rbase);
                 head += kBatch;
             }
             if (m != 0xffffffffu) break;                                      // the list is ordered by position
@@ -633,14 +683,14 @@ k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
             const uint32_t avail = tail;
             if (c < nchunks) tail += (uint32_t)cull_step(p, geo, t, keys, n, c, tail, lane);
             while (avail - head >= (uint32_t)kBatch) {
-                bwd_batch<true, DEPTH>(sm, px, t, vg, head, kBatch, kx, ky, lane);
+                bwd_batch<true, DEPTH, DET>(sm, px, t, vg, head, kBatch, kx, ky, lane, rbase);
                 head += kBatch;
             }
         }
     }
     if (tail != head) {
         queue_pad(sm.q, tail, lane, DEPTH ? sm.dd : nullptr);
-        bwd_batch<false, DEPTH>(sm, px, t, vg, head, (int)(tail - head), kx, ky, lane);
+        bwd_batch<false, DEPTH, DET>(sm, px, t, vg, head, (int)(tail - head), kx, ky, lane, rbase);
     }
 }
 
@@ -672,40 +722,56 @@ int set_composite_option(int which, int value) {
     return PS_ERR_INVALID_ARGUMENT;
 }
 
-template <int K, bool DEPTH>
+template <int K, bool DEPTH, bool DET>
 static int launch_fwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
                       const ImageState &img, float *out_color, const LossEpilogue &loss, const HitLists &hl,
                       cudaStream_t st) {
     const long long tasks = (long long)d.S * d.V * d.tiles * 8;
     constexpr int per_cta = kFwdWarps / K;
-    k_composite_fwd2<K, DEPTH><<<(unsigned)((tasks + per_cta - 1) / per_cta), kFwdWarps * 32, 0, st>>>(d, g, in.bg, keys, img, out_color, loss, hl);
+    k_composite_fwd2<K, DEPTH, DET><<<(unsigned)((tasks + per_cta - 1) / per_cta), kFwdWarps * 32, 0, st>>>(d, g, in.bg, keys, img, out_color, loss, hl);
     PS_LAUNCH_CHECK("k_composite_fwd2");
     return PS_OK;
 }
 
-template <int K>
+template <int K, bool DET>
 static int launch_fwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
                       const ImageState &img, float *out_color, const LossEpilogue &loss, const HitLists &hl,
                       cudaStream_t st) {
-    return d.depth_mode ? launch_fwd<K, true>(d, in, g, keys, img, out_color, loss, hl, st)
-                        : launch_fwd<K, false>(d, in, g, keys, img, out_color, loss, hl, st);
+    return d.depth_mode ? launch_fwd<K, true, DET>(d, in, g, keys, img, out_color, loss, hl, st)
+                        : launch_fwd<K, false, DET>(d, in, g, keys, img, out_color, loss, hl, st);
+}
+
+template <bool DET>
+static int launch_fwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
+                      const ImageState &img, float *out_color, const LossEpilogue &loss, const HitLists &hl,
+                      cudaStream_t st) {
+    switch (d.segK) {
+        case 4: return launch_fwd<4, DET>(d, in, g, keys, img, out_color, loss, hl, st);
+        case 2: return launch_fwd<2, DET>(d, in, g, keys, img, out_color, loss, hl, st);
+        default: return launch_fwd<1, DET>(d, in, g, keys, img, out_color, loss, hl, st);
+    }
 }
 
 int launch_composite_forward(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
                              const ImageState &img, float *out_color, const LossEpilogue &loss, const HitLists &hl,
-                             cudaStream_t st) {
+                             float *loss_partials, cudaStream_t st) {
     if (composite_impl() == 1) {
         if (loss.target || !out_color) { set_error("the legacy compositor has no loss epilogue"); return PS_ERR_UNSUPPORTED; }
         return launch_composite_forward_v1(d, in, g, keys, img, out_color, st);
     }
-    switch (d.segK) {
-        case 4: return launch_fwd<4>(d, in, g, keys, img, out_color, loss, hl, st);
-        case 2: return launch_fwd<2>(d, in, g, keys, img, out_color, loss, hl, st);
-        default: return launch_fwd<1>(d, in, g, keys, img, out_color, loss, hl, st);
-    }
+    if (!loss.target || !loss_partials) return launch_fwd<false>(d, in, g, keys, img, out_color, loss, hl, st);
+    // fixed-order loss epilogue: per-task partials, then k_loss_finish writes every slot of loss.sums
+    LossEpilogue le = loss;
+    le.sums = loss_partials;
+    int rc = launch_fwd<true>(d, in, g, keys, img, out_color, le, hl, st);
+    if (rc) return rc;
+    k_loss_finish<<<(unsigned)(d.S * d.V), kLossSlots, 0, st>>>(reinterpret_cast<const float2 *>(loss_partials),
+                                                                d.tiles * 8, loss.sums);
+    PS_LAUNCH_CHECK("k_loss_finish");
+    return PS_OK;
 }
 
-template <int K, bool DEPTH>
+template <int K, bool DEPTH, bool DET>
 static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
                       const ImageState &img, const float *d_color, const float *d_depth, const ViewGrads &vg,
                       const LossEpilogue &loss, const HitLists &hl, cudaStream_t st) {
@@ -714,34 +780,114 @@ static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const unsi
     const size_t smem = sizeof(BwdSmem<DEPTH>) * kBwdWarps;
     static unsigned long long attr_devices = 0;
     if (first_use_on_device(attr_devices)) {
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_composite_bwd2<K, DEPTH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PS_CUDA_CHECK(cudaFuncSetAttribute(k_composite_bwd2<K, DEPTH, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
-    k_composite_bwd2<K, DEPTH><<<(unsigned)((tasks + per_cta - 1) / per_cta), kBwdWarps * 32, smem, st>>>(
+    k_composite_bwd2<K, DEPTH, DET><<<(unsigned)((tasks + per_cta - 1) / per_cta), kBwdWarps * 32, smem, st>>>(
         d, g, in.bg, keys, img, d_color, d_depth, vg, loss, hl);
     PS_LAUNCH_CHECK("k_composite_bwd2");
     return PS_OK;
 }
 
-template <int K>
+template <int K, bool DET>
 static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
                       const ImageState &img, const float *d_color, const float *d_depth, const ViewGrads &vg,
                       const LossEpilogue &loss, const HitLists &hl, cudaStream_t st) {
-    return d_depth ? launch_bwd<K, true>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st)
-                   : launch_bwd<K, false>(d, in, g, keys, img, d_color, nullptr, vg, loss, hl, st);
+    return d_depth ? launch_bwd<K, true, DET>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st)
+                   : launch_bwd<K, false, DET>(d, in, g, keys, img, d_color, nullptr, vg, loss, hl, st);
+}
+
+template <bool DET>
+static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
+                      const ImageState &img, const float *d_color, const float *d_depth, const ViewGrads &vg,
+                      const LossEpilogue &loss, const HitLists &hl, cudaStream_t st) {
+    switch (d.segK) {
+        case 4: return launch_bwd<4, DET>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
+        case 2: return launch_bwd<2, DET>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
+        default: return launch_bwd<1, DET>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
+    }
+}
+
+// Fixed-order gather of the DET backward's block records: 8 lanes per on-screen (view, Gaussian) pair, lane b = block b.
+// For each tile of the pair's rectangle, row-major, the pair's position in the tile's sorted segment is found by a
+// binary search for the exact key the scatter wrote (float_bits(depth) << 32 | Gaussian; every tile of the rectangle
+// holds exactly one instance of the pair), and lane b adds block b's record of that position.  The 8 lanes' sums are
+// then added in block order 0..7 and STORED into the per-(view, Gaussian) scratch (zero-filled, so pairs that are not
+// listed read zero there).  Every sum has a fixed order: tiles row-major within a block, blocks 0..7.
+constexpr int kGatherThreads = 128;
+
+__global__ void __launch_bounds__(kGatherThreads)
+k_gather_block_records(Dims d, Geom geo, const unsigned long long *__restrict__ keys, ViewGrads rec, ViewGrads vg) {
+    if (*geo.n_instances > d.capacity) return;
+    const long long i = ((long long)blockIdx.x * kGatherThreads + threadIdx.x) >> 3;
+    const int lane = threadIdx.x & 31, b = lane & 7;
+    if (((long long)blockIdx.x * kGatherThreads + (threadIdx.x & ~31)) >> 3 >= geo.n_instances[2]) return;   // warp
+    const bool live = i < geo.n_instances[2];
+    uint32_t vgi = 0;
+    float2 m = make_float2(0.0f, 0.0f);
+    float4 c = make_float4(0.0f, 0.0f, 0.0f, 0.0f), col = c;
+    if (live) {
+        vgi = geo.vis_pairs[i];
+        const uint32_t vid = vgi / (uint32_t)d.P, gid = vgi - vid * (uint32_t)d.P;
+        const ushort4 r = geo.rect[vgi];
+        const unsigned long long key = ((unsigned long long)__float_as_uint(geo.depth[vgi]) << 32) | gid;
+        const uint32_t *__restrict__ t_start = geo.tile_start + (size_t)vid * d.tiles;
+        const uint32_t *__restrict__ t_count = geo.tile_count + (size_t)vid * d.tiles;
+        for (uint32_t ty = r.y; ty < r.w; ++ty)
+            for (uint32_t tx = r.x; tx < r.z; ++tx) {
+                const uint32_t tile = ty * (uint32_t)d.gx + tx;
+                const uint32_t start = t_start[tile], count = t_count[tile];
+                const unsigned long long *__restrict__ seg = keys + start;
+                uint32_t lo = 0, hi = count;       // lower bound of key in the tile's sorted segment
+                while (lo < hi) {
+                    const uint32_t mid = (lo + hi) >> 1;
+                    if (seg[mid] < key) lo = mid + 1; else hi = mid;
+                }
+                if (lo == count || seg[lo] != key) continue;     // (not reached: the scatter wrote it)
+                const size_t q = (size_t)start * 8 + (size_t)b * count + lo;
+                const float2 a = rec.d_mean2d[q];
+                const float4 e = rec.d_conic[q], f = rec.d_color[q];
+                m.x += a.x; m.y += a.y;
+                c.x += e.x; c.y += e.y; c.z += e.z; c.w += e.w;
+                col.x += f.x; col.y += f.y; col.z += f.z; col.w += f.w;
+            }
+    }
+    // blocks 0..7, in order, into lane 0 of the group
+    const int g0 = lane & ~7;
+    float2 sm = make_float2(0.0f, 0.0f);
+    float4 sc = make_float4(0.0f, 0.0f, 0.0f, 0.0f), scol = sc;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const int src = g0 + k;
+        sm.x += __shfl_sync(0xffffffffu, m.x, src); sm.y += __shfl_sync(0xffffffffu, m.y, src);
+        sc.x += __shfl_sync(0xffffffffu, c.x, src); sc.y += __shfl_sync(0xffffffffu, c.y, src);
+        sc.z += __shfl_sync(0xffffffffu, c.z, src); sc.w += __shfl_sync(0xffffffffu, c.w, src);
+        scol.x += __shfl_sync(0xffffffffu, col.x, src); scol.y += __shfl_sync(0xffffffffu, col.y, src);
+        scol.z += __shfl_sync(0xffffffffu, col.z, src); scol.w += __shfl_sync(0xffffffffu, col.w, src);
+    }
+    if (live && b == 0) {
+        vg.d_mean2d[vgi] = sm;
+        vg.d_conic[vgi] = sc;
+        vg.d_color[vgi] = scol;
+    }
 }
 
 int launch_composite_backward(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
                               const ImageState &img, const float *d_color, const float *d_depth, const ViewGrads &vg,
-                              const LossEpilogue &loss, const HitLists &hl, cudaStream_t st) {
+                              const ViewGrads *records, const LossEpilogue &loss, const HitLists &hl,
+                              cudaStream_t st) {
     if (composite_impl() == 1) {
         if (!d_color) { set_error("the legacy compositor has no loss epilogue"); return PS_ERR_UNSUPPORTED; }
         return launch_composite_backward_v1(d, in, g, keys, img, d_color, vg, st);
     }
-    switch (d.segK) {
-        case 4: return launch_bwd<4>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
-        case 2: return launch_bwd<2>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
-        default: return launch_bwd<1>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
-    }
+    if (!records) return launch_bwd<false>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
+    int rc = launch_bwd<true>(d, in, g, keys, img, d_color, d_depth, *records, loss, hl, st);
+    if (rc) return rc;
+    // the pair count lives on the device: launch for the worst case, surplus threads exit at once
+    const long long lanes = (long long)d.S * d.V * d.P * 8;
+    k_gather_block_records<<<(unsigned)((lanes + kGatherThreads - 1) / kGatherThreads), kGatherThreads, 0, st>>>(
+        d, g, keys, *records, vg);
+    PS_LAUNCH_CHECK("k_gather_block_records");
+    return PS_OK;
 }
 
 // Runs per task for a batch of `tasks` warp tasks: enough warps to fill the machine (132 SMs x ~24 resident

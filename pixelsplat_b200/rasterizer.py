@@ -11,6 +11,7 @@ from __future__ import annotations
 import ctypes
 import os
 import threading
+import warnings
 import weakref
 from typing import NamedTuple, Optional
 
@@ -199,6 +200,27 @@ class RasterOutputState:
         return self.image[off:off + 4 * n].view(torch.float32).reshape(-1, d.height, d.width)
 
 
+def _sync_deterministic() -> None:
+    """Carries torch.use_deterministic_algorithms into the library's "deterministic" option (fixed-order composite
+    backward and loss epilogue; include/pixelsplat_b200.h), setting it only when it differs.  Called before every
+    forward and backward enqueues.  The legacy compositor (composite_impl = 1) has no fixed-order form; under the
+    flag it is treated as torch treats an op without a deterministic implementation: RuntimeError, or with
+    warn_only=True a warning and today's path."""
+    want = 1 if torch.are_deterministic_algorithms_enabled() else 0
+    if want and _lib.get_option("composite_impl") == 1:
+        msg = ("pixelsplat_b200 rasterizer with the legacy compositor (composite_impl = 1) does not have a "
+               "deterministic implementation, but you set 'torch.use_deterministic_algorithms(True)'. You can turn "
+               "off determinism just for this operation, or you can use the 'warn_only=True' option, if that's "
+               "acceptable for your application. Select the warp-task compositor (composite_impl = 2, the default) "
+               "for deterministic rasterizer gradients.")
+        if not torch.is_deterministic_algorithms_warn_only_enabled():
+            raise RuntimeError(msg)
+        warnings.warn(msg)
+        want = 0
+    if _lib.get_option("deterministic") != want:
+        _lib.set_option("deterministic", want)
+
+
 class _Config(NamedTuple):
     """The non-tensor settings of one rasterizer call: the ps_raster_desc fields the caller chooses, and whether
     the colour image is written."""
@@ -243,6 +265,7 @@ def _forward(means, cov, opac, sh, cams, cfg: _Config, backward_follows: bool, t
         if capacity is None:
             capacity = max(4096, 3 * S * V * P)
         stream = torch.cuda.current_stream(dev)
+        _sync_deterministic()               # before the sizes: the mode changes the image state
         while True:
             desc = _lib.RasterDesc(S, V, P, cfg.M, cfg.degree, cfg.sh_layout, cfg.cov_layout, H, W, cfg.sort_impl,
                                    min(_segment_hint.get(key, 0), 1 << 30), capacity, cfg.sh_basis, cfg.depth_mode)
@@ -340,6 +363,7 @@ class _Rasterize(torch.autograd.Function):
         else:
             scale = (torch.zeros(VT, dtype=torch.float32, device=dev) if d_sse is None
                      else (2.0 * d_sse).to(torch.float32).contiguous())
+        _sync_deterministic()               # before the sizes: the mode changes the backward scratch
         scratch = torch.empty(_lib.sizes(desc).backward_bytes, dtype=torch.uint8, device=dev)
         d_means, d_cov = torch.empty_like(means), torch.empty_like(cov)
         d_opac, d_sh = torch.empty_like(opac), torch.empty_like(sh)
