@@ -335,6 +335,29 @@ PS_API int ps_epipolar_attention_backward(const ps_epipolar_desc *desc, const ps
                                           const float *dmass, const float *d_row, float *dq_feat,
                                           float *dq_pe, float *dbias, float *dfeatures, void *stream);
 
+/* Fixed-order form of the backward above: dq_feat, dq_pe and dbias are computed by the same code, and dfeatures is
+ * summed without float atomics, so the same inputs, desc and GPU give the same bits on every run.  dfeatures is
+ * fully written (no zero-fill needed).  Each (query, other view, sample) slot t = (n (v-1) + ov) S + s stores its
+ * sample gradient, bilinear weights and cell key; a stable radix sort of the slots by cell, a per-cell sum in
+ * ascending slot id and a per-texel sum of its four cells in a fixed order then form dfeatures.  No host
+ * synchronisation (graph-capturable).  Workspace, where A(x) rounds x up to a multiple of 256,
+ * T = b v R (v-1) S slots and Cn = b v (grid_h+1) (grid_w+1) cells:
+ *   A(512 T)                  per-slot sample gradients [T, 128] f32
+ * + A(16 T)                   per-slot bilinear weights [T, 4] f32
+ * + 4 A(4 T)                  cell keys and slot ids, two of each (radix ping-pong)
+ * + A(1024 ceil(T / 4096))    radix histograms [256, chunks of 4096 slots] u32
+ * + A(4 (Cn + 1))             cell_start u32
+ * + A(2048 Cn)                per-cell tap sums [Cn, 4, 128] f32.
+ * Both functions return what ps_epipolar_attention_forward's descriptor check returns, and PS_ERR_INVALID_ARGUMENT
+ * for a NULL pointer or a short workspace, before anything is enqueued; PS_ERR_UNSUPPORTED when T or Cn does not
+ * fit 31 bits. */
+PS_API int ps_epipolar_attention_backward_workspace_bytes(const ps_epipolar_desc *desc, size_t *out);
+PS_API int ps_epipolar_attention_backward_deterministic(const ps_epipolar_desc *desc, const ps_epipolar_inputs *in,
+                                                        const float *lse, const float *dz, const float *de,
+                                                        const float *dmass, const float *d_row, float *dq_feat,
+                                                        float *dq_pe, float *dbias, float *dfeatures /* fully written */,
+                                                        void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- dense per-image self-attention (wgmma, TF32 operands, FP32 accumulate) -----------------------
  * Replaces the z = None branch of /root/reference/src/model/transformer/attention.py:54-70 as used by
  * ImageSelfAttention (/root/reference/src/model/encoder/epipolar/image_self_attention.py:57-79):

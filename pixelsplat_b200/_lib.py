@@ -101,7 +101,8 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_self_attention_forward", "ps_gaussian_adapter_forward", "ps_gaussian_adapter_backward",
            "ps_sh_rotation_matrices", "ps_set_option", "ps_raster_forward_loss", "ps_raster_backward_loss",
            "ps_self_attention_forward_stats", "ps_self_attention_backward", "ps_get_option",
-           "ps_raster_backward_depth", "ps_ssim_workspace_bytes", "ps_ssim_forward", "ps_ssim_backward")
+           "ps_raster_backward_depth", "ps_ssim_workspace_bytes", "ps_ssim_forward", "ps_ssim_backward",
+           "ps_epipolar_attention_backward_workspace_bytes", "ps_epipolar_attention_backward_deterministic")
 
 
 class NativeLibraryMissing(ImportError):
@@ -147,6 +148,11 @@ def _load() -> ctypes.CDLL:
     lib.ps_epipolar_attention_forward.restype = ctypes.c_int
     lib.ps_epipolar_attention_backward.argtypes = [P(EpipolarDesc), P(EpipolarInputs)] + [ctypes.c_void_p] * 10
     lib.ps_epipolar_attention_backward.restype = ctypes.c_int
+    lib.ps_epipolar_attention_backward_workspace_bytes.argtypes = [P(EpipolarDesc), P(ctypes.c_size_t)]
+    lib.ps_epipolar_attention_backward_workspace_bytes.restype = ctypes.c_int
+    lib.ps_epipolar_attention_backward_deterministic.argtypes = [P(EpipolarDesc), P(EpipolarInputs)] + \
+        [ctypes.c_void_p] * 10 + [ctypes.c_size_t, ctypes.c_void_p]
+    lib.ps_epipolar_attention_backward_deterministic.restype = ctypes.c_int
     lib.ps_self_attention_forward.argtypes = [ctypes.c_int32] * 4 + [ctypes.c_void_p, ctypes.c_float, ctypes.c_void_p,
                                                                       ctypes.c_int32, ctypes.c_void_p]
     lib.ps_self_attention_forward.restype = ctypes.c_int
@@ -209,6 +215,14 @@ def get_option(name: str) -> int:
     v = ctypes.c_int()
     check(lib.ps_get_option(name.encode(), ctypes.byref(v)), "ps_get_option")
     return v.value
+
+
+def epipolar_backward_workspace_bytes(desc: EpipolarDesc) -> int:
+    """Workspace of ps_epipolar_attention_backward_deterministic for `desc` (no device needed)."""
+    out = ctypes.c_size_t()
+    check(lib.ps_epipolar_attention_backward_workspace_bytes(ctypes.byref(desc), ctypes.byref(out)),
+          "ps_epipolar_attention_backward_workspace_bytes")
+    return out.value
 
 
 def sizes(desc: RasterDesc) -> RasterSizes:

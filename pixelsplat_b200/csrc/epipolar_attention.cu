@@ -335,18 +335,33 @@ k_epi_attn_fwd(EpiParams P, int n_queries, float *__restrict__ z_out, float *__r
     }
 }
 
+// Slot records of the fixed-order d(feature map) (ps_epipolar_attention_backward_deterministic).  Slot
+// t = (n * OV + ov) * S + s is one (query, other view, sample); its record holds the sample's gradient vector
+// d f_s [128], its four bilinear tap weights and its cell key
+//   m (h+1)(w+1) + (by+1)(w+1) + (bx+1),   m = b V + o_view,  (by, bx) the cell's top-left tap (make_taps),
+// for cells that touch an in-bounds texel (by in [-1, h-1], bx in [-1, w-1]); every other slot (invalid ray,
+// cell off the map) gets the sentinel key n_cells and no record.
+struct EpiDetRecords {
+    float *df;            // [T, 128]
+    float4 *w;            // [T]
+    unsigned *key;        // [T]
+    unsigned n_cells;     // B V (h+1) (w+1)
+};
+
 // Backward of k_epi_attn_fwd.  Inputs: the forward inputs, lse, the output cotangents (dz, de,
 // dmass) and D_h = dz_h.z_h + de_h.e_h + dmass_h.mass_h (flash-attention's row term, formed
 // outside by one elementwise pass).  Outputs: dqt, dpq, dbias, and d(feature map) accumulated with
 // 16-byte vector atomics (the map gradient is L2-resident; consecutive samples that fall in the
 // same bilinear cell are merged in registers first, which removes most of the atomics on short
 // epipolar segments).  With lse known every sample is independent, so sub-chunks need no rescaling here.
-template <int HEADS, int SUB>
-__global__ void __launch_bounds__(kEpiWarps * 32, 4)
+// DET: instead of the atomics, every slot's record goes to `det` (dfeat is not touched); the sort, per-cell sums
+// and per-texel finish below add them up in a fixed order.
+template <int HEADS, int SUB, bool DET = false>
+__global__ void __launch_bounds__(kEpiWarps * 32, DET ? 3 : 4)   // DET: 168 registers, no spills
 k_epi_attn_bwd(EpiParams P, int n_queries, const float *__restrict__ lse, const float *__restrict__ dz,
                const float *__restrict__ de, const float *__restrict__ dmass, const float *__restrict__ Drow,
                float *__restrict__ dqt_out, float *__restrict__ dpq_out, float *__restrict__ dbias_out,
-               float *__restrict__ dfeat) {
+               float *__restrict__ dfeat, EpiDetRecords det) {
     __shared__ EpiWarpSmem sm_all[kEpiWarps];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     EpiWarpSmem &sm = sm_all[warp];
@@ -386,6 +401,7 @@ k_epi_attn_bwd(EpiParams P, int n_queries, const float *__restrict__ lse, const 
         // ---- PE halves of the score and of d a, and the bilinear taps, lane = sample
         Taps my_taps;
         int my_cell = -0x7ffffffe;
+        unsigned my_key = det.n_cells;                    // DET only: the sentinel unless the cell touches the map
         {
             float pe[kMaxPE];
             const bool has_sample = lane < P.S;
@@ -397,9 +413,20 @@ k_epi_attn_bwd(EpiParams P, int n_queries, const float *__restrict__ lse, const 
                 const int bx = (int)fminf(fmaxf(floorf(ix), -2.0f), (float)P.w + 1.0f);
                 const int by = (int)fminf(fmaxf(floorf(iy), -2.0f), (float)P.h + 1.0f);
                 my_cell = by * (P.w + 4) + bx;            // the bilinear cell (backward merges samples that share it)
+                if constexpr (DET) {
+                    if (bx >= -1 && bx < P.w && by >= -1 && by < P.h)
+                        my_key = (unsigned)(((b * P.V + o_view) * (P.h + 1) + by + 1) * (P.w + 1) + bx + 1);
+                }
             } else {
 #pragma unroll
                 for (int k = 0; k < 4; ++k) { my_taps.off[k] = -1; my_taps.w[k] = 0.0f; }
+            }
+            if constexpr (DET) {
+                if (has_sample) {
+                    const size_t t = ((size_t)n * P.OV + ov) * P.S + lane;
+                    det.key[t] = my_key;
+                    if (my_key != det.n_cells) det.w[t] = make_float4(my_taps.w[0], my_taps.w[1], my_taps.w[2], my_taps.w[3]);
+                }
             }
             positional_encoding(has_sample ? P.rd[ray * P.S + lane] : 0.0f, P.npe, pe);
 #pragma unroll
@@ -495,7 +522,13 @@ k_epi_attn_bwd(EpiParams P, int n_queries, const float *__restrict__ lse, const 
                         df[c] += aw[hd] * gz[hd][c] + dw[hd] * qt[hd][c];
                     }
                 }
-                if (s < P.S && ok) {
+                if constexpr (DET) {
+                    if (s < P.S && ok) {
+                        if (__shfl_sync(0xffffffffu, my_key, s) != det.n_cells)
+                            *reinterpret_cast<float4 *>(det.df + (((size_t)n * P.OV + ov) * P.S + s) * kEpiC + 4 * lane) =
+                                make_float4(df[0], df[1], df[2], df[3]);
+                    }
+                } else if (s < P.S && ok) {
                     Taps t;
 #pragma unroll
                     for (int k = 0; k < 4; ++k) {
@@ -519,7 +552,7 @@ k_epi_attn_bwd(EpiParams P, int n_queries, const float *__restrict__ lse, const 
             }
             __syncwarp();
         }
-        flush();
+        if constexpr (!DET) flush();
         if (dbias_out && lane == 0) {
 #pragma unroll
             for (int hd = 0; hd < HEADS; ++hd) dbias_out[((size_t)n * HEADS + hd) * P.OV + ov] = dbias_acc[hd];
@@ -571,9 +604,251 @@ static int launch_epi(bool backward, const EpiParams &P, int n, float *z, float 
         else k_epi_attn_fwd<HEADS, kEpiSubFwd><<<blocks, kEpiWarps * 32, 0, st>>>(P, n, z, e, mass, lse_out);
         PS_LAUNCH_CHECK("k_epi_attn_fwd");
     } else {
-        k_epi_attn_bwd<HEADS, kEpiSubBwd><<<blocks, kEpiWarps * 32, 0, st>>>(P, n, lse, dz, de, dmass, Drow, dqt, dpq, dbias, dfeat);
+        k_epi_attn_bwd<HEADS, kEpiSubBwd><<<blocks, kEpiWarps * 32, 0, st>>>(P, n, lse, dz, de, dmass, Drow, dqt, dpq, dbias, dfeat,
+                                                                             EpiDetRecords{});
         PS_LAUNCH_CHECK("k_epi_attn_bwd");
     }
+    return PS_OK;
+}
+
+// ---- fixed-order d(feature map) -------------------------------------------------------------------------------
+// A stable LSD radix sort of the slot ids by cell key (8-bit digits, reduce-then-scan), then one warp per cell sums
+// its slots' weighted records in ascending slot id, then one warp per texel adds its four cells' tap sums in a fixed
+// order.  Every sum runs in an order fixed by the inputs, so the result is the same bits on every run.
+constexpr int kSortThreads = 256, kSortTiles = 16, kSortChunk = kSortThreads * kSortTiles;   // slots per chunk
+constexpr int kScanThreads = 1024;
+
+// hist[d * chunks + c] = number of slots of chunk c whose digit is d.
+__global__ void __launch_bounds__(kSortThreads)
+k_epi_radix_hist(const unsigned *__restrict__ keys, int T, int shift, int chunks, unsigned *__restrict__ hist) {
+    __shared__ unsigned h[256];
+    h[threadIdx.x] = 0;
+    __syncthreads();
+    const int base = blockIdx.x * kSortChunk;
+    for (int i = threadIdx.x; i < kSortChunk; i += kSortThreads)
+        if (base + i < T) atomicAdd(&h[(keys[base + i] >> shift) & 255u], 1u);   // integer counts: order-free
+    __syncthreads();
+    hist[(size_t)threadIdx.x * chunks + blockIdx.x] = h[threadIdx.x];
+}
+
+// Exclusive scan of the [256, chunks] histogram in place (digit-major: digit d of chunk c starts after every
+// smaller digit and after digit d of every earlier chunk).  One block; each thread scans a contiguous run.
+__global__ void __launch_bounds__(kScanThreads)
+k_epi_radix_scan(unsigned *__restrict__ hist, int m) {
+    __shared__ unsigned warp_tot[kScanThreads / 32];
+    const int per = (m + kScanThreads - 1) / kScanThreads;
+    const int beg = min(m, (int)threadIdx.x * per), end = min(m, beg + per);
+    unsigned sum = 0;
+    for (int i = beg; i < end; ++i) sum += hist[i];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned incl = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned y = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += y;
+    }
+    if (lane == 31) warp_tot[warp] = incl;
+    __syncthreads();
+    if (warp == 0) {
+        unsigned t = warp_tot[lane], ti = t;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned y = __shfl_up_sync(0xffffffffu, ti, o);
+            if (lane >= o) ti += y;
+        }
+        warp_tot[lane] = ti - t;
+    }
+    __syncthreads();
+    unsigned run = warp_tot[warp] + incl - sum;
+    for (int i = beg; i < end; ++i) {
+        const unsigned c = hist[i];
+        hist[i] = run;
+        run += c;
+    }
+}
+
+// Stable scatter of one chunk: tiles of 256 slots in order; inside a tile, a slot's position among equal digits is
+// (earlier chunks and tiles) + (earlier warps) + (earlier lanes, from match.any).  ids_in NULL = the identity.
+__global__ void __launch_bounds__(kSortThreads)
+k_epi_radix_scatter(const unsigned *__restrict__ keys_in, const unsigned *__restrict__ ids_in, int T, int shift,
+                    int chunks, const unsigned *__restrict__ offsets, unsigned *__restrict__ keys_out,
+                    unsigned *__restrict__ ids_out) {
+    constexpr int kWarps = kSortThreads / 32;
+    __shared__ unsigned wcnt[kWarps][256];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned run = offsets[(size_t)threadIdx.x * chunks + blockIdx.x];   // thread d keeps digit d's cursor
+    const unsigned lt = (1u << lane) - 1u;
+    for (int tile = 0; tile < kSortTiles; ++tile) {
+        const int idx = blockIdx.x * kSortChunk + tile * kSortThreads + threadIdx.x;
+#pragma unroll
+        for (int j = 0; j < kWarps; ++j) wcnt[j][threadIdx.x] = 0;
+        __syncthreads();
+        const bool valid = idx < T;
+        const unsigned key = valid ? keys_in[idx] : 0u;
+        const unsigned id = valid ? (ids_in ? ids_in[idx] : (unsigned)idx) : 0u;
+        const unsigned d = valid ? (key >> shift) & 255u : 256u;
+        const unsigned peers = __match_any_sync(0xffffffffu, d);
+        const unsigned rank = __popc(peers & lt);
+        if (valid && rank == 0) wcnt[warp][d] = __popc(peers);
+        __syncthreads();
+        {
+            unsigned acc = run;
+#pragma unroll
+            for (int j = 0; j < kWarps; ++j) {
+                const unsigned c = wcnt[j][threadIdx.x];
+                wcnt[j][threadIdx.x] = acc;
+                acc += c;
+            }
+            run = acc;
+        }
+        __syncthreads();
+        if (valid) {
+            const unsigned pos = wcnt[warp][d] + rank;
+            keys_out[pos] = key;
+            ids_out[pos] = id;
+        }
+        __syncthreads();
+    }
+}
+
+// cell_start[c] = first sorted position whose key is >= c, for c in [0, n_cells]; cell_start[n_cells] = the number
+// of slots with a record.  Position i fills the cells in (key[i-1], key[i]].
+__global__ void k_epi_cell_bounds(const unsigned *__restrict__ keys, int T, unsigned n_cells,
+                                  unsigned *__restrict__ cell_start) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > T) return;
+    const long long hi = i < T ? (long long)keys[i] : (long long)n_cells;
+    const long long lo = i > 0 ? (long long)keys[i - 1] : -1;
+    for (long long c = lo + 1; c <= hi; ++c) cell_start[c] = (unsigned)i;
+}
+
+// One warp per cell, lane = 4 channels: cell_sum[c][k] = sum over the cell's slots, in ascending slot id, of
+// w_k * d f.  An empty cell writes zeros.
+constexpr int kCellWarps = 8;
+__global__ void __launch_bounds__(kCellWarps * 32)
+k_epi_cell_sums(const float *__restrict__ df, const float4 *__restrict__ w, const unsigned *__restrict__ ids,
+                const unsigned *__restrict__ cell_start, unsigned n_cells, float *__restrict__ cell_sum) {
+    const int lane = threadIdx.x & 31;
+    const unsigned c = blockIdx.x * kCellWarps + (threadIdx.x >> 5);
+    if (c >= n_cells) return;
+    const unsigned beg = cell_start[c], end = cell_start[c + 1];
+    float acc[4][4] = {};
+#pragma unroll 4
+    for (unsigned j = beg; j < end; ++j) {
+        const unsigned t = ids[j];
+        const float4 wk = w[t];
+        const float4 g = ldg4(df + (size_t)t * kEpiC + 4 * lane);
+        const float wv[4] = {wk.x, wk.y, wk.z, wk.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            acc[k][0] += wv[k] * g.x; acc[k][1] += wv[k] * g.y;
+            acc[k][2] += wv[k] * g.z; acc[k][3] += wv[k] * g.w;
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+        *reinterpret_cast<float4 *>(cell_sum + ((size_t)c * 4 + k) * kEpiC + 4 * lane) =
+            make_float4(acc[k][0], acc[k][1], acc[k][2], acc[k][3]);
+}
+
+// One warp per texel (y, x) of map m, lane = 4 channels: the four cells whose taps land on it, in a fixed order --
+// (y-1, x-1) tap 3, (y-1, x) tap 2, (y, x-1) tap 1, (y, x) tap 0.  Writes every texel.
+__global__ void __launch_bounds__(kCellWarps * 32)
+k_epi_texel_finish(const float *__restrict__ cell_sum, int n_texels, int h, int w, float *__restrict__ dfeat) {
+    const int lane = threadIdx.x & 31;
+    const int q = blockIdx.x * kCellWarps + (threadIdx.x >> 5);
+    if (q >= n_texels) return;
+    const int x = q % w, y = (q / w) % h, m = q / (w * h);
+    const size_t c0 = ((size_t)m * (h + 1) + y) * (w + 1) + x;          // cell (y-1, x-1)
+    const float *base = cell_sum + 4 * lane;
+    const float4 a = ldg4(base + (c0 * 4 + 3) * kEpiC);
+    const float4 b = ldg4(base + ((c0 + 1) * 4 + 2) * kEpiC);
+    const float4 c = ldg4(base + ((c0 + w + 1) * 4 + 1) * kEpiC);
+    const float4 d = ldg4(base + ((c0 + w + 2) * 4 + 0) * kEpiC);
+    *reinterpret_cast<float4 *>(dfeat + (size_t)q * kEpiC + 4 * lane) =
+        make_float4(((a.x + b.x) + c.x) + d.x, ((a.y + b.y) + c.y) + d.y, ((a.z + b.z) + c.z) + d.z,
+                    ((a.w + b.w) + c.w) + d.w);
+}
+
+// Workspace of the deterministic backward (A(x) = x rounded up to 256; the header states the same formula).
+struct EpiDetLayout {
+    long long T;                  // slots
+    unsigned n_cells;
+    int chunks, passes;
+    size_t df, w, key[2], id[2], hist, cell_start, cell_sum, total;
+};
+
+static size_t align256(size_t x) { return (x + 255) / 256 * 256; }
+
+static int epi_det_layout(const ps_epipolar_desc *d, EpiDetLayout *L) {
+    const long long rays = (long long)d->batch * d->views * d->grid_h * d->grid_w;
+    const long long T = rays * (d->views - 1) * d->samples;
+    const long long cells = (long long)d->batch * d->views * (d->grid_h + 1) * (d->grid_w + 1);
+    if (rays > 0x7fffffffLL || T > 0x7fffffffLL || cells >= 0x7fffffffLL) {
+        set_error("ps_epipolar_attention_backward_deterministic: b*v*R*(v-1)*S slots and b*v*(h+1)*(w+1) cells must fit 31 bits");
+        return PS_ERR_UNSUPPORTED;
+    }
+    L->T = T;
+    L->n_cells = (unsigned)cells;
+    L->chunks = (int)((T + kSortChunk - 1) / kSortChunk);
+    const int bits = 32 - __builtin_clz(L->n_cells);          // the sentinel key n_cells needs this many bits
+    L->passes = (bits + 7) / 8;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off += align256(bytes); return o; };
+    L->df = take(512 * (size_t)T);
+    L->w = take(16 * (size_t)T);
+    L->key[0] = take(4 * (size_t)T);
+    L->key[1] = take(4 * (size_t)T);
+    L->id[0] = take(4 * (size_t)T);
+    L->id[1] = take(4 * (size_t)T);
+    L->hist = take(4 * 256 * (size_t)L->chunks);
+    L->cell_start = take(4 * ((size_t)cells + 1));
+    L->cell_sum = take(2048 * (size_t)cells);
+    L->total = off;
+    return PS_OK;
+}
+
+template <int HEADS>
+static int launch_epi_bwd_det(const EpiParams &P, int n, const EpiDetLayout &L, char *ws, const float *lse,
+                              const float *dz, const float *de, const float *dmass, const float *Drow, float *dqt,
+                              float *dpq, float *dbias, float *dfeat, cudaStream_t st) {
+    EpiDetRecords rec;
+    rec.df = reinterpret_cast<float *>(ws + L.df);
+    rec.w = reinterpret_cast<float4 *>(ws + L.w);
+    rec.key = reinterpret_cast<unsigned *>(ws + L.key[0]);
+    rec.n_cells = L.n_cells;
+    k_epi_attn_bwd<HEADS, kEpiSubBwd, true><<<(n + kEpiWarps - 1) / kEpiWarps, kEpiWarps * 32, 0, st>>>(
+        P, n, lse, dz, de, dmass, Drow, dqt, dpq, dbias, nullptr, rec);
+    PS_LAUNCH_CHECK("k_epi_attn_bwd<DET>");
+
+    const int T = (int)L.T;
+    unsigned *hist = reinterpret_cast<unsigned *>(ws + L.hist);
+    int cur = 0;                                                   // ping-pong buffer holding the current order
+    for (int pass = 0; pass < L.passes; ++pass) {
+        const unsigned *keys_in = reinterpret_cast<const unsigned *>(ws + L.key[cur]);
+        const unsigned *ids_in = pass == 0 ? nullptr : reinterpret_cast<const unsigned *>(ws + L.id[cur]);
+        k_epi_radix_hist<<<L.chunks, kSortThreads, 0, st>>>(keys_in, T, 8 * pass, L.chunks, hist);
+        PS_LAUNCH_CHECK("k_epi_radix_hist");
+        k_epi_radix_scan<<<1, kScanThreads, 0, st>>>(hist, 256 * L.chunks);
+        PS_LAUNCH_CHECK("k_epi_radix_scan");
+        k_epi_radix_scatter<<<L.chunks, kSortThreads, 0, st>>>(
+            keys_in, ids_in, T, 8 * pass, L.chunks, hist, reinterpret_cast<unsigned *>(ws + L.key[cur ^ 1]),
+            reinterpret_cast<unsigned *>(ws + L.id[cur ^ 1]));
+        PS_LAUNCH_CHECK("k_epi_radix_scatter");
+        cur ^= 1;
+    }
+    unsigned *cell_start = reinterpret_cast<unsigned *>(ws + L.cell_start);
+    k_epi_cell_bounds<<<(T + 1 + 255) / 256, 256, 0, st>>>(reinterpret_cast<const unsigned *>(ws + L.key[cur]), T,
+                                                          L.n_cells, cell_start);
+    PS_LAUNCH_CHECK("k_epi_cell_bounds");
+    float *cell_sum = reinterpret_cast<float *>(ws + L.cell_sum);
+    k_epi_cell_sums<<<(L.n_cells + kCellWarps - 1) / kCellWarps, kCellWarps * 32, 0, st>>>(
+        rec.df, rec.w, reinterpret_cast<const unsigned *>(ws + L.id[cur]), cell_start, L.n_cells, cell_sum);
+    PS_LAUNCH_CHECK("k_epi_cell_sums");
+    const int texels = P.B * P.V * P.h * P.w;
+    k_epi_texel_finish<<<(texels + kCellWarps - 1) / kCellWarps, kCellWarps * 32, 0, st>>>(cell_sum, texels, P.h, P.w,
+                                                                                            dfeat);
+    PS_LAUNCH_CHECK("k_epi_texel_finish");
     return PS_OK;
 }
 
@@ -644,5 +919,45 @@ extern "C" PS_API int ps_epipolar_attention_backward(const ps_epipolar_desc *d, 
         case 2: return launch_epi<2>(true, P, n, 0, 0, 0, 0, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
         case 3: return launch_epi<3>(true, P, n, 0, 0, 0, 0, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
         default: return launch_epi<4>(true, P, n, 0, 0, 0, 0, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
+    }
+}
+
+extern "C" PS_API int ps_epipolar_attention_backward_workspace_bytes(const ps_epipolar_desc *d, size_t *out) {
+    int rc = epi_check(d);
+    if (rc) return rc;
+    if (!out) { set_error("ps_epipolar_attention_backward_workspace_bytes: out is NULL"); return PS_ERR_INVALID_ARGUMENT; }
+    EpiDetLayout L;
+    if ((rc = epi_det_layout(d, &L))) return rc;
+    *out = L.total;
+    return PS_OK;
+}
+
+extern "C" PS_API int ps_epipolar_attention_backward_deterministic(
+        const ps_epipolar_desc *d, const ps_epipolar_inputs *in, const float *lse, const float *dz, const float *de,
+        const float *dmass, const float *d_row, float *dq_feat, float *dq_pe, float *dbias, float *dfeatures,
+        void *workspace, size_t workspace_bytes, void *stream) {
+    int rc = epi_check(d);
+    if (rc) return rc;
+    if (!in || !in->features || !in->segments || !in->valid || !in->rel_disparity || !in->q_feat || !lse ||
+        !dz || (d->pe_dim > 0 && (!in->q_pe || !de || !dq_pe)) || !d_row || !dq_feat || !dfeatures || !workspace) {
+        set_error("ps_epipolar_attention_backward_deterministic: a required pointer is NULL");
+        return PS_ERR_INVALID_ARGUMENT;
+    }
+    EpiDetLayout L;
+    if ((rc = epi_det_layout(d, &L))) return rc;
+    if (workspace_bytes < L.total) {
+        set_error("ps_epipolar_attention_backward_deterministic: workspace of %zu bytes, %zu needed", workspace_bytes,
+                  L.total);
+        return PS_ERR_INVALID_ARGUMENT;
+    }
+    const EpiParams P = epi_params(d, in);
+    const int n = d->batch * d->views * d->grid_h * d->grid_w;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    char *ws = static_cast<char *>(workspace);
+    switch (d->heads) {
+        case 1: return launch_epi_bwd_det<1>(P, n, L, ws, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
+        case 2: return launch_epi_bwd_det<2>(P, n, L, ws, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
+        case 3: return launch_epi_bwd_det<3>(P, n, L, ws, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
+        default: return launch_epi_bwd_det<4>(P, n, L, ws, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
     }
 }

@@ -148,12 +148,22 @@ class _EpipolarAttentionFn(torch.autograd.Function):
         dqt = torch.empty_like(qt)
         dpq = torch.empty_like(pq)
         dbias = torch.empty_like(bias) if ctx.has_bias else None
-        dfeat = torch.zeros_like(feat_cl)
         stream = torch.cuda.current_stream(dev)
-        rc = _lib.on_device(dev, _lib.lib.ps_epipolar_attention_backward,
-            ctypes.byref(desc), ctypes.byref(inputs), _p(lse), _p(dz), _p(de), _p(dmass) if use_mass else None,
-            _p(d_row), _p(dqt), _p(dpq), _p(dbias), _p(dfeat), ctypes.c_void_p(stream.cuda_stream))
-        _lib.check(rc, "ps_epipolar_attention_backward")
+        args = (ctypes.byref(desc), ctypes.byref(inputs), _p(lse), _p(dz), _p(de), _p(dmass) if use_mass else None,
+                _p(d_row), _p(dqt), _p(dpq), _p(dbias))
+        if torch.are_deterministic_algorithms_enabled():
+            # fixed-order d(feature map): slot records sorted by bilinear cell, summed per cell, then per texel;
+            # every texel is written, so dfeat needs no zero-fill
+            ws = torch.empty(_lib.epipolar_backward_workspace_bytes(desc), dtype=torch.uint8, device=dev)
+            dfeat = torch.empty_like(feat_cl)
+            rc = _lib.on_device(dev, _lib.lib.ps_epipolar_attention_backward_deterministic, *args, _p(dfeat),
+                                _p(ws), ws.numel(), ctypes.c_void_p(stream.cuda_stream))
+            _lib.check(rc, "ps_epipolar_attention_backward_deterministic")
+        else:
+            dfeat = torch.zeros_like(feat_cl)
+            rc = _lib.on_device(dev, _lib.lib.ps_epipolar_attention_backward, *args, _p(dfeat),
+                                ctypes.c_void_p(stream.cuda_stream))
+            _lib.check(rc, "ps_epipolar_attention_backward")
         return dqt, dpq, dbias, dfeat, None, None
 
 

@@ -49,7 +49,13 @@ def main():
                     help="add LossDepth (re10k_depth_loss: weight 0.25, sigma 12, second derivative) on the fused depth")
     ap.add_argument("--two-pass-depth", action="store_true",
                     help="with --depth-loss: render the depth as a second pass (render_depth) instead (A/B)")
+    ap.add_argument("--deterministic", action="store_true",
+                    help="torch.use_deterministic_algorithms(True): fixed-order encoder and rasterizer gradients")
     args = ap.parse_args()
+    if args.deterministic:                         # cuBLAS needs its workspace setting before its first call
+        import os
+        os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
+        torch.use_deterministic_algorithms(True)
     from pixelsplat_b200 import parallel, synthetic
     from pixelsplat_b200.decoder import DecoderSplattingCUDA, DecoderSplattingCUDACfg
     from pixelsplat_b200.encoder import EpipolarTransformer, EpipolarTransformerCfg, ImageSelfAttentionCfg
@@ -180,6 +186,7 @@ def main():
             "allreduce": ("after backward, torch.cat buckets (round-1 path)" if reducer is None else
                           f"{len(reducer.buckets)} flat buckets of <= {args.bucket_mb} MB, issued from backward hooks "
                           "(overlapped); phase 'allreduce' is the exposed tail only"),
+            "deterministic": args.deterministic,
             "peak_gib": torch.cuda.max_memory_allocated() / 2 ** 30, "loss": float(loss),
             "n_gpus": world, "data": "synthetic", "dtype": "f32"}))
     if world > 1:
