@@ -128,6 +128,8 @@ class _EpipolarAttentionFn(torch.autograd.Function):
         ctx.save_for_backward(qt, pq, bias_c if bias_c is not None else torch.empty(0, device=dev), feat_cl,
                               z, e, mass, lse)
         ctx.geometry, ctx.desc, ctx.has_bias = geometry, desc, bias_c is not None
+        # an output no loss reaches gets None, not a zero tensor: an unused mass then costs nothing in the backward
+        ctx.set_materialize_grads(False)
         return z, e, mass
 
     @staticmethod
@@ -135,8 +137,9 @@ class _EpipolarAttentionFn(torch.autograd.Function):
         qt, pq, bias, feat_cl, z, e, mass, lse = ctx.saved_tensors
         g, desc = ctx.geometry, ctx.desc
         dev = feat_cl.device
-        dz, de = dz.contiguous().float(), de.contiguous().float()
-        use_mass = ctx.has_bias and dmass is not None
+        dz = torch.zeros_like(z) if dz is None else dz.contiguous().float()
+        de = torch.zeros_like(e) if de is None else de.contiguous().float()
+        use_mass = dmass is not None          # with or without a bias: mass depends on qt, pq and the features
         d_row = (dz * z).sum(-1) + (de * e).sum(-1)
         if use_mass:
             dmass = dmass.contiguous().float()
