@@ -133,9 +133,9 @@ typedef struct ps_raster_layout {
     size_t tile_start;    /* u32  [S*V*tiles] exclusive scan, global instance offsets          */
     size_t tile_cursor;   /* u32  scratch                                                      */
     size_t n_instances;   /* i64  [4] instances needed (may exceed capacity), longest segment,
-                                     #visible (view,Gaussian) pairs, #Gaussians visible in any view */
+                                     #visible (view,Gaussian) pairs, unused (0)                     */
     size_t vis_pairs;     /* u32  [S*V*P] compact list of on-screen (view,Gaussian) flat indices  */
-    size_t vis_any;       /* u32  [S*P]   compact list of (scene,Gaussian) visible in >= 1 view    */
+    size_t vis_any;       /* u32  [S*P]   unused (no longer written; the offset is kept)            */
     /* binning */
     size_t keys;          /* u64  [capacity]  per tile sorted (float_bits(depth)<<32 | gaussian) */
     size_t keys_alt;      /* u64  [capacity]  scratch                                          */
@@ -171,7 +171,7 @@ PS_API const char *ps_last_error(void); /* thread-local, valid until the next fa
 /* Instrumentation used by bench.py: number of kernels this library has launched so far, and
  * optional per-stage CUDA-event timing (on the launching stream) of the most recent
  * forward + backward pair: ms[7] = preprocess, count-scan + scatter, sort, composite forward,
- * gradient zero-fill, composite backward, preprocess backward. */
+ * clearing of the on-screen gradient scratch rows, composite backward, preprocess backward. */
 PS_API unsigned long long ps_launch_count(void);
 PS_API void ps_timing_enable(int on);
 PS_API int ps_timing_read(float *ms);
@@ -236,6 +236,8 @@ PS_API int ps_raster_forward(const ps_raster_desc *desc, const ps_raster_inputs 
  * Backward: composite backward (warp-reduced, one atomic per (tile, Gaussian)) ->
  * per-Gaussian cov2D / projection / SH backward summed over the V views of a scene.
  * Replaces _C.rasterize_gaussians_backward.  `scratch` has ps_raster_sizes.backward_bytes.
+ * Every element of every gradient in `grads` is written (zeros where no gradient flows), so they need no
+ * initialisation; `scratch` needs none either.
  */
 PS_API int ps_raster_backward(const ps_raster_desc *desc, const ps_raster_inputs *in,
                        const ps_raster_state *state, const float *d_color /* [S*V,3,H,W] */,

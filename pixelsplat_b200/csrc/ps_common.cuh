@@ -22,9 +22,8 @@ struct Geom {
     uint32_t *tile_count;
     uint32_t *tile_start;
     uint32_t *tile_cursor;
-    long long *n_instances;   // [0] instances, [1] longest segment, [2] #vis_pairs, [3] #vis_any
+    long long *n_instances;   // [0] instances, [1] longest segment, [2] #vis_pairs, [3] unused (0)
     uint32_t *vis_pairs;      // compact list of (view, Gaussian) flat indices that are on screen
-    uint32_t *vis_any;        // compact list of (scene, Gaussian) flat indices visible in >= 1 view
     float4 *cull;             // xy + half-extents of the alpha >= 1/255 box (compositor's cull record)
 };
 
@@ -191,6 +190,8 @@ int composite_segments(long long tasks);
 bool composite_hit_lists(long long capacity);      // keep the forward's hit lists for the backward?
 int launch_preprocess_backward(const Dims &d, const Inputs &in, const Geom &g, const ViewGrads &vg,
                                const ps_raster_grads &out, cudaStream_t st);
-int launch_gradient_fill(const Dims &d, const ps_raster_grads &out, cudaStream_t st);
+// Clears the gradient scratch rows of the on-screen (view, Gaussian) pairs: the only rows the composite backward
+// writes and the preprocess backward reads.
+int launch_clear_pair_grads(const Dims &d, const Geom &g, const ViewGrads &vg, cudaStream_t st);
 
 }  // namespace ps

@@ -47,11 +47,11 @@ void mark(int id, cudaStream_t st) {
     cudaEventRecord(g_events[id], st);
 }
 
-// Side stream for work that is independent of the critical path (gradient zero-fill overlapping
-// the composite backward).  Fork/join with events, which also captures cleanly into CUDA graphs.
+// Side stream for work that is independent of the critical path (SH -> RGB overlapping the binning
+// in the forward).  Fork/join with events, which also captures cleanly into CUDA graphs.
 // The library's side stream and its fork / join events, one set per device ordinal (created on first
 // use on that device; a host process may drive several GPUs).
-// The fork / join event pair is shared by every call on a device, so the enqueue of one forward (or backward)
+// The fork / join event pair is shared by every call on a device, so the enqueue of one forward
 // -- record fork, side-stream work, record join, wait join -- must not interleave with another host thread's on
 // the same device: each entry point holds the device's mutex while it enqueues (host-side only; ~tens of us).
 struct SideCtx {
@@ -157,9 +157,9 @@ static Layout make_layout(const ps_raster_desc *d) {
     L.off.tile_count = take(vt * 4);
     L.off.tile_start = take(vt * 4);
     L.off.tile_cursor = take(vt * 4);
-    L.off.n_instances = take(32);   // [0] instances, [1] longest segment, [2] #visible pairs, [3] #visible Gaussians
+    L.off.n_instances = take(32);   // [0] instances, [1] longest segment, [2] #visible pairs, [3] unused
     L.off.vis_pairs = take(vp * 4);
-    L.off.vis_any = take((size_t)m.S * m.P * 4);
+    L.off.vis_any = take((size_t)m.S * m.P * 4);   // unused; kept so that the ABI layout does not change
     L.off.cull = take(vp * 16);
     L.sizes.geom_bytes = o;
     o = 0;
@@ -212,7 +212,6 @@ static Geom make_geom(const Layout &L, void *geom) {
     g.tile_cursor = reinterpret_cast<uint32_t *>(b + L.off.tile_cursor);
     g.n_instances = reinterpret_cast<long long *>(b + L.off.n_instances);
     g.vis_pairs = reinterpret_cast<uint32_t *>(b + L.off.vis_pairs);
-    g.vis_any = reinterpret_cast<uint32_t *>(b + L.off.vis_any);
     g.cull = reinterpret_cast<float4 *>(b + L.off.cull);
     return g;
 }
@@ -457,16 +456,10 @@ static int raster_backward_impl(const ps_raster_desc *desc, const ps_raster_inpu
     rec.d_mean2d = reinterpret_cast<float2 *>(sb + L.records);
     rec.d_conic = reinterpret_cast<float4 *>(sb + L.records + align_up(nr * 8));
     rec.d_color = reinterpret_cast<float4 *>(sb + L.records + align_up(nr * 8) + align_up(nr * 16));
-    SideCtx *sc = nullptr;
-    if ((rc = side_ready(sc))) return rc;
-    std::lock_guard<std::mutex> enqueue_lock(sc->enqueue);
     mark(kMarkBwdStart, st);
-    // fork: zero the output gradients on the side stream while the composite backward runs
-    PS_CUDA_CHECK(cudaEventRecord(sc->fork, st));
-    PS_CUDA_CHECK(cudaStreamWaitEvent(sc->side, sc->fork, 0));
-    if ((rc = launch_gradient_fill(d, *grads, sc->side))) return rc;
-    PS_CUDA_CHECK(cudaEventRecord(sc->join, sc->side));
-    PS_CUDA_CHECK(cudaMemsetAsync(scratch, 0, L.sizes.backward_bytes, st));
+    if ((rc = launch_clear_pair_grads(d, g, vg, st))) return rc;
+    // deterministic mode: the gather reads a record for every list position, whether or not a block stored one
+    if (L.det) PS_CUDA_CHECK(cudaMemsetAsync(sb + L.records, 0, L.sizes.backward_bytes - L.records, st));
     mark(kMarkBwdZero, st);
     HitLists hl{nullptr, nullptr};
     if (d.hit_lists) {
@@ -476,7 +469,6 @@ static int raster_backward_impl(const ps_raster_desc *desc, const ps_raster_inpu
     if ((rc = launch_composite_backward(d, I, g, keys, img, d_color, d_depth, vg, L.det ? &rec : nullptr, le, hl, st)))
         return rc;
     mark(kMarkCompositeBwd, st);
-    PS_CUDA_CHECK(cudaStreamWaitEvent(st, sc->join, 0));   // join
     if ((rc = launch_preprocess_backward(d, I, g, vg, *grads, st))) return rc;
     mark(kMarkPreprocessBwd, st);
     return PS_OK;

@@ -811,8 +811,8 @@ static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const unsi
 // For each tile of the pair's rectangle, row-major, the pair's position in the tile's sorted segment is found by a
 // binary search for the exact key the scatter wrote (float_bits(depth) << 32 | Gaussian; every tile of the rectangle
 // holds exactly one instance of the pair), and lane b adds block b's record of that position.  The 8 lanes' sums are
-// then added in block order 0..7 and STORED into the per-(view, Gaussian) scratch (zero-filled, so pairs that are not
-// listed read zero there).  Every sum has a fixed order: tiles row-major within a block, blocks 0..7.
+// then added in block order 0..7 and STORED into the per-(view, Gaussian) scratch (every listed pair's row, the rows
+// the preprocess backward reads).  Every sum has a fixed order: tiles row-major within a block, blocks 0..7.
 constexpr int kGatherThreads = 128;
 
 __global__ void __launch_bounds__(kGatherThreads)

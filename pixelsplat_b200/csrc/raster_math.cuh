@@ -229,10 +229,12 @@ __device__ __forceinline__ void gather_rows(const float *__restrict__ base, unsi
 
 // Asynchronous form of gather_rows: every element is one cp.async (LDGSTS, 4 bytes -- rows start on 4-byte
 // boundaries only), so the whole warp's 32 x sh_n floats are in flight at once instead of one L2 / HBM round
-// trip per batch of four rows, and the caller can do unrelated work before gather_rows_wait().
+// trip per batch of four rows, and the caller can do unrelated work before gather_rows_wait().  Only the rows of
+// the lanes set in `rows` are fetched; the others are left as they are.
 __device__ __forceinline__ void gather_rows_async(const float *__restrict__ base, unsigned long long row_of_lane,
-                                                  int rows_valid, int sh_n, float *wrows, int row_stride, int lane) {
-    for (int r = 0; r < rows_valid; ++r) {
+                                                  unsigned rows, int sh_n, float *wrows, int row_stride, int lane) {
+    for (unsigned m = rows; m != 0u; m &= m - 1u) {
+        const int r = __ffs(m) - 1;
         const unsigned long long rs = __shfl_sync(0xffffffffu, row_of_lane, r);
         const float *src = base + rs * (unsigned long long)sh_n;
         float *dst = wrows + r * row_stride;
@@ -249,13 +251,16 @@ __device__ __forceinline__ void gather_rows_wait() {
     __syncwarp();
 }
 
-// The inverse: write the warp's staged rows back to their scattered global rows.
-__device__ __forceinline__ void scatter_rows(float *__restrict__ base, unsigned long long row_of_lane,
-                                             int rows_valid, int sh_n, const float *wrows, int row_stride, int lane) {
-    for (int r = 0; r < rows_valid; ++r) {
-        const unsigned long long rs = __shfl_sync(0xffffffffu, row_of_lane, r);
-        float *__restrict__ dst = base + rs * (unsigned long long)sh_n;
-        for (int c = lane; c < sh_n; c += 32) dst[c] = wrows[r * row_stride + c];
+// The inverse for consecutive rows: the warp's first `rows` staged rows go to dst[0 .. rows * sh_n) as one
+// contiguous, coalesced block (element e of it is column e % sh_n of staged row e / sh_n).
+__device__ __forceinline__ void store_rows(float *__restrict__ dst, int rows, int sh_n, const float *wrows,
+                                           int row_stride, int lane) {
+    const int dr = 32 / sh_n, dc = 32 - dr * sh_n;
+    int r = lane / sh_n, c = lane - r * sh_n;
+    for (int e = lane; e < rows * sh_n; e += 32) {
+        dst[e] = wrows[r * row_stride + c];
+        r += dr; c += dc;
+        if (c >= sh_n) { c -= sh_n; ++r; }
     }
 }
 

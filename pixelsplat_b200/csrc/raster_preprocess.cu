@@ -58,7 +58,6 @@ k_preprocess(Dims d, Inputs in, Geom geo, int use_smem_hist) {
 #pragma unroll
         for (int i = 0; i < 6; ++i) cov_raw[i] = tmp[i];
     }
-    bool any_vis = false;
 
     for (int v = 0; v < d.V; ++v) {
         const int vid = scene * d.V + v;
@@ -136,10 +135,8 @@ k_preprocess(Dims d, Inputs in, Geom geo, int use_smem_hist) {
                 }
             }
         }
-        any_vis |= vis;
         warp_append(vis, (uint32_t)vg, geo.vis_pairs, geo.n_instances + 2, lane);
     }
-    warp_append(any_vis, (uint32_t)sg, geo.vis_any, geo.n_instances + 3, lane);
     if (use_smem_hist) {
         __syncthreads();
         uint32_t *dst = geo.tile_count + (size_t)scene * d.V * d.tiles;
@@ -171,7 +168,7 @@ k_sh_color(Dims d, Inputs in, Geom geo, int row_stride) {
     const int sh_n = 3 * d.M;
     float *wrows = s_rows + (size_t)warp * 32 * row_stride;
     // all 32 rows in flight at once (cp.async), the direction set-up below runs under their latency
-    gather_rows_async(in.sh, (unsigned long long)sg, (int)min((long long)32, n - i0), sh_n, wrows, row_stride, lane);
+    gather_rows_async(in.sh, (unsigned long long)sg, __ballot_sync(0xffffffffu, live), sh_n, wrows, row_stride, lane);
     const float sc = in.scale ? in.scale[vid] : 1.0f;
     const float m0 = in.means[3 * sg + 0], m1 = in.means[3 * sg + 1], m2 = in.means[3 * sg + 2];
     const float px = in.scale ? m0 * sc : m0, py = in.scale ? m1 * sc : m1, pz = in.scale ? m2 * sc : m2;

@@ -14,41 +14,59 @@ namespace ps {
 
 constexpr int kPreBwdThreads = 128;
 
-// One thread per Gaussian that is on screen in at least one view (the compact list built by the
-// forward pass), so warps are dense; Gaussians that are not listed receive zero gradients from
-// launch_gradient_fill (plain memsets, issued on a side stream so that they overlap the
-// compute-bound composite backward).  SH rows are staged per warp in shared memory: coefficients
-// come in with coalesced row-wise loads, dL/dSH goes out the same way.
+// Each warp owns 32 consecutive (scene, Gaussian) indices of S*P and writes every element of their rows of every
+// output gradient, which the caller may hand over uninitialised: a Gaussian that is on screen in no view gets zeros,
+// and so does every Gaussian when the binning overflowed its capacity (the composite backward then did not run).  A
+// warp none of whose Gaussians is on screen only stores zeros.  On screen in view v means radii > 0, the rows
+// k_clear_pair_grads cleared and the composite backward accumulated into.  SH rows are staged per warp in shared
+// memory: the coefficients of the on-screen lanes come in with cp.async, dL/dSH of all 32 rows goes out as one
+// contiguous block.
 // DEPTH: the depth value's chain to the means is added (a depth gradient was given); built for 4 resident CTAs so
 // that it does not spill.
 template <bool DEPTH>
 __global__ void __launch_bounds__(kPreBwdThreads, DEPTH ? 4 : 5)
 k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, ps_raster_grads out, int row_stride) {
     extern __shared__ float s_dsh[];   // [warps][32][row_stride] coefficients (V == 1: reused for the gradient)
-    if (*geo.n_instances > d.capacity) return;
-    const long long n = geo.n_instances[3];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const long long i0 = ((long long)blockIdx.x * kPreBwdThreads) + warp * 32;
-    if (i0 >= n) return;
-    const long long li = i0 + lane;
-    const bool live = li < n;
-    const uint32_t sgi = live ? geo.vis_any[li] : 0u;
+    const long long sp = (long long)d.S * d.P;
+    const long long sg0 = ((long long)blockIdx.x * kPreBwdThreads) + warp * 32;
+    if (sg0 >= sp) return;
+    const int rows = (int)min((long long)32, sp - sg0);
+    const bool live = lane < rows;
+    const uint32_t sgi = (uint32_t)(live ? sg0 + lane : sg0);
     const uint32_t scene = sgi / (uint32_t)d.P, g = sgi - scene * (uint32_t)d.P;
     const size_t sg = sgi;
     const int cov_n = d.cov_layout == PS_COV_TRIU6 ? 6 : 9;
     const int sh_n = d.M > 0 ? 3 * d.M : 3;
     const int M = d.M, layout = d.sh_layout;
+
+    bool any = false;
+    if (live && *geo.n_instances <= d.capacity)
+        for (int v = 0; v < d.V; ++v) any |= geo.radii[(size_t)((int)scene * d.V + v) * d.P + g] > 0;
+    const unsigned vis_lanes = __ballot_sync(0xffffffffu, any);
+    if (vis_lanes == 0u) {
+        for (int e = lane; e < rows * 3; e += 32) out.d_means[3 * sg0 + e] = 0.0f;
+        for (int e = lane; e < rows * cov_n; e += 32) out.d_cov[cov_n * sg0 + e] = 0.0f;
+        if (lane < rows) out.d_opacities[sg0 + lane] = 0.0f;
+        for (int e = lane; e < rows * sh_n; e += 32) out.d_sh[sh_n * sg0 + e] = 0.0f;
+        if (out.d_means2d && live)
+            for (int v = 0; v < d.V; ++v) {
+                float *m2 = out.d_means2d + 3 * ((size_t)((int)scene * d.V + v) * d.P + g);
+                m2[0] = 0.0f; m2[1] = 0.0f; m2[2] = 0.0f;
+            }
+        return;
+    }
+
     float *wrows = s_dsh + (size_t)warp * 32 * row_stride;
     float *row = wrows + lane * row_stride;
     const bool in_place = M > 0 && d.V == 1;     // read each coefficient, then overwrite its slot with the gradient
     float *grow = in_place ? row : row + (size_t)kPreBwdThreads * row_stride;   // separate gradient rows when V > 1
 
-    const int rows_valid = (int)min((long long)32, n - i0);
     // the SH rows stream into shared memory while the geometry part below runs; waited for at first use
-    if (M > 0) gather_rows_async(in.sh, (unsigned long long)sg, rows_valid, sh_n, wrows, row_stride, lane);
+    if (M > 0) gather_rows_async(in.sh, (unsigned long long)sg, vis_lanes, sh_n, wrows, row_stride, lane);
 
     float mx0 = 0.0f, my0 = 0.0f, mz0 = 0.0f;
-    if (live) { mx0 = in.means[3 * sg + 0]; my0 = in.means[3 * sg + 1]; mz0 = in.means[3 * sg + 2]; }
+    if (any) { mx0 = in.means[3 * sg + 0]; my0 = in.means[3 * sg + 1]; mz0 = in.means[3 * sg + 2]; }
     const float *covp = in.cov + sg * cov_n;
 
     float dmx = 0.0f, dmy = 0.0f, dmz = 0.0f, dop = 0.0f;
@@ -59,11 +77,11 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, ps_raster_grads out
     for (int v = 0; v < d.V; ++v) {
         const int vid = (int)scene * d.V + v;
         const size_t vg = (size_t)vid * d.P + g;
-        const bool vis = live && geo.radii[vg] > 0;
-        if (live && out.d_means2d && vis) {
+        const bool vis = any && geo.radii[vg] > 0;
+        if (live && out.d_means2d) {
             float *m2 = out.d_means2d + 3 * vg;
-            const float2 t = vgr.d_mean2d[vg];
-            m2[0] = t.x; m2[1] = t.y;
+            const float2 t = vis ? vgr.d_mean2d[vg] : make_float2(0.0f, 0.0f);
+            m2[0] = t.x; m2[1] = t.y; m2[2] = 0.0f;
         }
         // (no `continue` for the views this Gaussian is not on screen in: the warp must stay convergent for the
         //  shared-memory hand-over of the SH rows below)
@@ -199,7 +217,8 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, ps_raster_grads out
             for (int i = 0; i < 6; ++i) dc[i] = dcov[i];
         } else {
             dc[0] = dcov[0]; dc[1] = dcov[1]; dc[2] = dcov[2];
-            dc[4] = dcov[3]; dc[5] = dcov[4]; dc[8] = dcov[5];      // lower triangle stays zero (pre-filled)
+            dc[3] = 0.0f; dc[4] = dcov[3]; dc[5] = dcov[4];
+            dc[6] = 0.0f; dc[7] = 0.0f; dc[8] = dcov[5];      // the lower triangle receives no gradient
         }
         if (M == 0) {
             float *dsh = out.d_sh + sg * 3;
@@ -207,23 +226,34 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, ps_raster_grads out
         }
     }
     if (M > 0) {
-        // every listed Gaussian is visible in >= 1 view, so its gradient row was written above
+        if (!sh_written)                   // on screen in no view: the row was neither fetched nor written
+            for (int c = 0; c < sh_n; ++c) grow[c] = 0.0f;
         __syncwarp();
         const float *gsrc = in_place ? wrows : wrows + (size_t)kPreBwdThreads * row_stride;
-        scatter_rows(out.d_sh, (unsigned long long)sg, rows_valid, sh_n, gsrc, row_stride, lane);
+        store_rows(out.d_sh + (size_t)sg0 * sh_n, rows, sh_n, gsrc, row_stride, lane);
     }
 }
 
-// Zero gradients for everything the dense kernel does not write (Gaussians that are on screen in
-// no view, the lower covariance triangle, optional screen-space gradients).  Pure memsets.
-int launch_gradient_fill(const Dims &d, const ps_raster_grads &out, cudaStream_t st) {
-    const size_t sp = (size_t)d.S * d.P;
-    PS_CUDA_CHECK(cudaMemsetAsync(out.d_means, 0, sp * 3 * sizeof(float), st));
-    PS_CUDA_CHECK(cudaMemsetAsync(out.d_cov, 0, sp * (d.cov_layout == PS_COV_TRIU6 ? 6 : 9) * sizeof(float), st));
-    PS_CUDA_CHECK(cudaMemsetAsync(out.d_opacities, 0, sp * sizeof(float), st));
-    PS_CUDA_CHECK(cudaMemsetAsync(out.d_sh, 0, sp * (d.M > 0 ? 3 * d.M : 3) * sizeof(float), st));
-    if (out.d_means2d)
-        PS_CUDA_CHECK(cudaMemsetAsync(out.d_means2d, 0, (size_t)d.S * d.V * d.P * 3 * sizeof(float), st));
+// Clears the per-(view, Gaussian) gradient scratch rows of the on-screen pairs (the compact list k_preprocess built):
+// those, and only those, are accumulated into by the composite backward (its tile lists hold exactly the listed
+// pairs), stored by the fixed-order gather, and read by k_preprocess_bwd (radii > 0 implies listed).  Every other row
+// of the scratch is left as it is.  One thread per list entry; the count lives on the device, so the grid is sized
+// for the worst case and surplus threads exit at once.
+constexpr int kClearThreads = 256;
+
+__global__ void __launch_bounds__(kClearThreads) k_clear_pair_grads(Geom geo, ViewGrads vg) {
+    const long long i = (long long)blockIdx.x * kClearThreads + threadIdx.x;
+    if (i >= geo.n_instances[2]) return;
+    const uint32_t p = geo.vis_pairs[i];
+    vg.d_mean2d[p] = make_float2(0.0f, 0.0f);
+    vg.d_conic[p] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    vg.d_color[p] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+}
+
+int launch_clear_pair_grads(const Dims &d, const Geom &g, const ViewGrads &vg, cudaStream_t st) {
+    const long long pairs = (long long)d.S * d.V * d.P;
+    k_clear_pair_grads<<<(unsigned)((pairs + kClearThreads - 1) / kClearThreads), kClearThreads, 0, st>>>(g, vg);
+    PS_LAUNCH_CHECK("k_clear_pair_grads");
     return PS_OK;
 }
 
@@ -236,7 +266,7 @@ int launch_preprocess_backward(const Dims &d, const Inputs &in, const Geom &g, c
         PS_CUDA_CHECK(cudaFuncSetAttribute(k_preprocess_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
         PS_CUDA_CHECK(cudaFuncSetAttribute(k_preprocess_bwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
     }
-    const long long sp = (long long)d.S * d.P;               // worst case; surplus warps exit at once
+    const long long sp = (long long)d.S * d.P;
     const unsigned blocks = (unsigned)((sp + kPreBwdThreads - 1) / kPreBwdThreads);
     if (d.depth_mode)
         k_preprocess_bwd<true><<<blocks, kPreBwdThreads, smem, st>>>(d, in, g, vg, out, row_stride);
