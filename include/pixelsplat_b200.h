@@ -157,13 +157,41 @@ typedef struct ps_raster_layout {
     size_t run_depth;     /* image: f32 [S*V*3*H*W] depth in front of list runs 1..3 (next to run_state)        */
 } ps_raster_layout;
 
+/* Camera gradients of a rasterizer backward (ps_raster_grads.camera).  The function differentiated is the one whose
+ * Gaussian gradients the backward returns, with viewmatrix, projmatrix, campos and tanfov as independent inputs:
+ * upstream's straight-through min(0.99, .) and hard skip masks, no gradient through radii, tile rectangles or the
+ * sort, and the +-1.3 tan(fov) clamp (it removes d/dt.x (d/dt.y) and passes nothing through its limit), so tanfov
+ * receives a gradient only through the focal lengths W / (2 tanfov) of the projection Jacobian.  Entries the forward
+ * never reads -- viewmatrix [3] [7] [11] [15], projmatrix [2] [6] [10] [14] -- get exactly 0, and so does campos with
+ * colours instead of SH.  With a depth gradient the depth value's chain to the viewmatrix is included;
+ * scene_scale and near_far are not differentiated.  After a binning overflow every entry is 0.
+ * Each output may be NULL (not written); the others are written in full, so they need no initialisation.  No float
+ * atomics: in deterministic mode the camera gradients are the same bits on every run.
+ * `workspace` (16-byte aligned, no initialisation) has ps_raster_camera_workspace_bytes: the preprocess backward
+ * stores one partial sum per (warp of 32 Gaussians, view) there and a finish kernel adds them in a fixed order. */
+typedef struct ps_raster_camera_grads {
+    float *d_viewmatrix; /* [S*V, 16] column-major like viewmatrix                              */
+    float *d_projmatrix; /* [S*V, 16]                                                           */
+    float *d_campos;     /* [S*V, 3]                                                            */
+    float *d_tanfov;     /* [S*V, 2]                                                            */
+    void *workspace;
+    size_t workspace_bytes;
+} ps_raster_camera_grads;
+
 typedef struct ps_raster_grads {
     float *d_means;     /* [S, P, 3]                                                           */
     float *d_cov;       /* same layout as cov                                                  */
     float *d_opacities; /* [S, P]                                                              */
     float *d_sh;        /* same layout as sh (or [S, P, 3] for colours)                        */
     float *d_means2d;   /* [S*V, P, 3] or NULL: upstream's screen-space gradient (x, y, 0)     */
+    /* appended with camera gradients (struct grows at the end only) */
+    const ps_raster_camera_grads *camera; /* NULL: no camera gradients (the backward is unchanged)  */
 } ps_raster_grads;
+
+/* Workspace of ps_raster_grads.camera for a descriptor, closed form (no device needed):
+ *   S * V * ((P - 1) / 32 + 2) * 128 bytes  (one 32-float row per warp overlapping a scene, per view).
+ * No other size query changes when camera gradients are requested. */
+PS_API int ps_raster_camera_workspace_bytes(const ps_raster_desc *desc, size_t *out);
 
 PS_API int ps_version(void);
 PS_API const char *ps_last_error(void); /* thread-local, valid until the next failing call */
@@ -217,6 +245,19 @@ PS_API int ps_camera_setup(int32_t n_views, const float *extrinsics, const float
                            const float *near_plane, const float *far_plane, int32_t scale_invariant,
                            float *viewmatrix, float *projmatrix, float *campos, float *tanfov,
                            float *scene_scale, void *stream);
+
+/*
+ * Reverse mode of ps_camera_setup, one thread per view (float64 inside): the gradients of the four camera arrays
+ * (each may be NULL = zero) are carried back through campos, view @ proj, the 4x4 inverse, the projection matrix,
+ * tan / acos of the field of view and the 3x3 inverse of the intrinsics, and the scale-invariant rescale of the
+ * translation, to d_extrinsics [n,4,4] and d_intrinsics [n,3,3] (both written in full).  near / far and
+ * scene_scale are not differentiated.  Bad arguments return PS_ERR_INVALID_ARGUMENT before anything is enqueued;
+ * the call does not synchronise the host (graph-capturable).
+ */
+PS_API int ps_camera_setup_backward(int32_t n_views, const float *extrinsics, const float *intrinsics,
+                                    const float *near_plane, const float *far_plane, int32_t scale_invariant,
+                                    const float *d_viewmatrix, const float *d_projmatrix, const float *d_campos,
+                                    const float *d_tanfov, float *d_extrinsics, float *d_intrinsics, void *stream);
 
 /*
  * Forward: preprocess -> per-tile count/scan -> scatter -> per-tile radix sort -> composite.

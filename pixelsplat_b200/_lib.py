@@ -89,9 +89,14 @@ class RasterLoss(ctypes.Structure):
 LOSS_SLOTS = 64
 
 
+class RasterCameraGrads(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in ("d_viewmatrix", "d_projmatrix", "d_campos", "d_tanfov", "workspace")] + \
+        [("workspace_bytes", ctypes.c_size_t)]
+
+
 class RasterGrads(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in (
-        "d_means", "d_cov", "d_opacities", "d_sh", "d_means2d")]
+        "d_means", "d_cov", "d_opacities", "d_sh", "d_means2d")] + [("camera", ctypes.POINTER(RasterCameraGrads))]
 
 
 EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_layout_query",
@@ -102,7 +107,8 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_sh_rotation_matrices", "ps_set_option", "ps_raster_forward_loss", "ps_raster_backward_loss",
            "ps_self_attention_forward_stats", "ps_self_attention_backward", "ps_get_option",
            "ps_raster_backward_depth", "ps_ssim_workspace_bytes", "ps_ssim_forward", "ps_ssim_backward",
-           "ps_epipolar_attention_backward_workspace_bytes", "ps_epipolar_attention_backward_deterministic")
+           "ps_epipolar_attention_backward_workspace_bytes", "ps_epipolar_attention_backward_deterministic",
+           "ps_raster_camera_workspace_bytes", "ps_camera_setup_backward")
 
 
 class NativeLibraryMissing(ImportError):
@@ -137,6 +143,11 @@ def _load() -> ctypes.CDLL:
     lib.ps_camera_setup.argtypes = [ctypes.c_int32] + [ctypes.c_void_p] * 4 + [ctypes.c_int32] + \
         [ctypes.c_void_p] * 6
     lib.ps_camera_setup.restype = ctypes.c_int
+    lib.ps_camera_setup_backward.argtypes = [ctypes.c_int32] + [ctypes.c_void_p] * 4 + [ctypes.c_int32] + \
+        [ctypes.c_void_p] * 7
+    lib.ps_camera_setup_backward.restype = ctypes.c_int
+    lib.ps_raster_camera_workspace_bytes.argtypes = [P(RasterDesc), P(ctypes.c_size_t)]
+    lib.ps_raster_camera_workspace_bytes.restype = ctypes.c_int
     lib.ps_launch_count.restype = ctypes.c_ulonglong
     lib.ps_timing_enable.argtypes = [ctypes.c_int]
     lib.ps_timing_enable.restype = None
@@ -229,6 +240,13 @@ def sizes(desc: RasterDesc) -> RasterSizes:
     out = RasterSizes()
     check(lib.ps_raster_sizes_query(ctypes.byref(desc), ctypes.byref(out)), "ps_raster_sizes_query")
     return out
+
+
+def camera_workspace_bytes(desc: RasterDesc) -> int:
+    out = ctypes.c_size_t()
+    check(lib.ps_raster_camera_workspace_bytes(ctypes.byref(desc), ctypes.byref(out)),
+          "ps_raster_camera_workspace_bytes")
+    return out.value
 
 
 def layout(desc: RasterDesc) -> RasterLayout:

@@ -67,6 +67,16 @@ struct Inputs {
     const float *near_far;    // [S*V, 2] world units (depth modes 3, 4)
 };
 
+// The Gaussian-side outputs of ps_raster_grads, as the preprocess backward receives them.
+struct GaussGrads {
+    float *d_means, *d_cov, *d_opacities, *d_sh, *d_means2d;
+};
+
+// Camera gradients (ps_raster_camera_grads): 29 used entries per partial row, rows of 32 floats, at most
+// (P - 1) / 32 + 2 warps of 32 consecutive (scene, Gaussian) indices overlap one scene's P Gaussians.
+constexpr int kCamEntries = 29, kCamRowFloats = 32;
+__host__ __device__ __forceinline__ int cam_rows_per_view(int P) { return (P - 1) / 32 + 2; }
+
 // Per-(view,Gaussian) gradient scratch written by the composite backward.
 struct ViewGrads {
     float2 *d_mean2d;  // NDC-scaled like upstream (x * 0.5 W, y * 0.5 H)
@@ -188,8 +198,9 @@ int set_composite_option(int which, int value);   // 0: impl (1 | 2), 1: segment
 int get_composite_option(int which);              // the value in force (environment included)
 int composite_segments(long long tasks);
 bool composite_hit_lists(long long capacity);      // keep the forward's hit lists for the backward?
+// With grads.camera set, the camera-gradient instantiation runs and a finish kernel writes the camera gradients.
 int launch_preprocess_backward(const Dims &d, const Inputs &in, const Geom &g, const ViewGrads &vg,
-                               const ps_raster_grads &out, cudaStream_t st);
+                               const ps_raster_grads &grads, cudaStream_t st);
 // Clears the gradient scratch rows of the on-screen (view, Gaussian) pairs: the only rows the composite backward
 // writes and the preprocess backward reads.
 int launch_clear_pair_grads(const Dims &d, const Geom &g, const ViewGrads &vg, cudaStream_t st);

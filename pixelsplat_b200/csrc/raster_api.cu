@@ -197,6 +197,11 @@ static Layout make_layout(const ps_raster_desc *d) {
     return L;
 }
 
+// ps_raster_camera_workspace_bytes: one partial row per (warp overlapping a scene, view)
+static size_t camera_workspace_bytes(const ps_raster_desc *d) {
+    return (size_t)d->n_scenes * d->views_per_scene * cam_rows_per_view(d->n_gaussians) * kCamRowFloats * sizeof(float);
+}
+
 static Geom make_geom(const Layout &L, void *geom) {
     char *b = static_cast<char *>(geom);
     Geom g;
@@ -340,6 +345,14 @@ PS_API int ps_raster_layout_query(const ps_raster_desc *desc, ps_raster_layout *
     return PS_OK;
 }
 
+PS_API int ps_raster_camera_workspace_bytes(const ps_raster_desc *desc, size_t *out) {
+    int rc = validate(desc);
+    if (rc) return rc;
+    if (!out) { set_error("out is NULL"); return PS_ERR_INVALID_ARGUMENT; }
+    *out = camera_workspace_bytes(desc);
+    return PS_OK;
+}
+
 }  // extern "C"
 
 static int raster_forward_impl(const ps_raster_desc *desc, const ps_raster_inputs *in, const ps_raster_state *state,
@@ -437,6 +450,14 @@ static int raster_backward_impl(const ps_raster_desc *desc, const ps_raster_inpu
     if (scratch_bytes < L.sizes.backward_bytes || ((uintptr_t)scratch & 15)) {
         set_error("backward scratch too small or misaligned: need %zu, got %zu", L.sizes.backward_bytes, scratch_bytes);
         return PS_ERR_INVALID_ARGUMENT;
+    }
+    if (const ps_raster_camera_grads *cg = grads->camera) {
+        const size_t need = camera_workspace_bytes(desc);
+        if (!cg->workspace || cg->workspace_bytes < need || ((uintptr_t)cg->workspace & 15)) {
+            set_error("camera-gradient workspace NULL, too small or misaligned: need %zu, got %zu", need,
+                      cg->workspace_bytes);
+            return PS_ERR_INVALID_ARGUMENT;
+        }
     }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     Dims d = make_dims(desc);

@@ -14,6 +14,16 @@ namespace ps {
 
 constexpr int kPreBwdThreads = 128;
 
+// Camera-gradient partial row of (scene s, view v) stored by the warp that owns indices sg0.. of S*P: rows of one
+// view are indexed by the warp's position among the warps overlapping the scene, kCamRowFloats floats each:
+//   [0..11]  d viewmatrix [0 1 2 | 4 5 6 | 8 9 10 | 12 13 14]
+//   [12..23] d projmatrix [0 1 3 | 4 5 7 | 8 9 11 | 12 13 15]
+//   [24..26] d campos, [27..28] d tanfov, [29..31] unused
+__device__ __forceinline__ float *cam_row(float *ws, const Dims &d, int s, int v, long long sg0) {
+    const long long w = sg0 / 32 - ((long long)s * d.P) / 32;
+    return ws + ((size_t)(s * d.V + v) * cam_rows_per_view(d.P) + (size_t)w) * kCamRowFloats;
+}
+
 // Each warp owns 32 consecutive (scene, Gaussian) indices of S*P and writes every element of their rows of every
 // output gradient, which the caller may hand over uninitialised: a Gaussian that is on screen in no view gets zeros,
 // and so does every Gaussian when the binning overflowed its capacity (the composite backward then did not run).  A
@@ -23,9 +33,13 @@ constexpr int kPreBwdThreads = 128;
 // contiguous block.
 // DEPTH: the depth value's chain to the means is added (a depth gradient was given); built for 4 resident CTAs so
 // that it does not spill.
-template <bool DEPTH>
-__global__ void __launch_bounds__(kPreBwdThreads, DEPTH ? 4 : 5)
-k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, ps_raster_grads out, int row_stride) {
+// CAM: camera gradients are requested.  Each lane also forms its Gaussian's contribution to the kCamEntries camera
+// entries of every view it is on screen in; the warp sums them per (scene, view) in a fixed shuffle order and
+// stores one partial row per (warp, view) into `cam_ws` (layout: cam_row), zeros included, which k_camera_finish
+// sums.  Built for 2 resident CTAs: the 29 partial sums are live beside the colour chain.
+template <bool DEPTH, bool CAM>
+__global__ void __launch_bounds__(kPreBwdThreads, CAM ? 2 : (DEPTH ? 4 : 5))
+k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int row_stride, float *cam_ws) {
     extern __shared__ float s_dsh[];   // [warps][32][row_stride] coefficients (V == 1: reused for the gradient)
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const long long sp = (long long)d.S * d.P;
@@ -54,6 +68,11 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, ps_raster_grads out
                 float *m2 = out.d_means2d + 3 * ((size_t)((int)scene * d.V + v) * d.P + g);
                 m2[0] = 0.0f; m2[1] = 0.0f; m2[2] = 0.0f;
             }
+        if (CAM) {
+            const int s_lo = (int)(sg0 / d.P), s_hi = (int)((sg0 + rows - 1) / d.P);
+            for (int s = s_lo; s <= s_hi; ++s)
+                for (int v = 0; v < d.V; ++v) cam_row(cam_ws, d, s, v, sg0)[lane] = 0.0f;
+        }
         return;
     }
 
@@ -87,6 +106,11 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, ps_raster_grads out
         //  shared-memory hand-over of the SH rows below)
         float gx = 0.0f, gy = 0.0f, gz = 0.0f;
         float4 gcol = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        float cam[CAM ? kCamEntries : 1];   // this Gaussian's share of the view's camera gradient (cam_row order)
+        if (CAM) {
+#pragma unroll
+            for (int k = 0; k < kCamEntries; ++k) cam[k] = 0.0f;
+        }
         const float sc = in.scale ? in.scale[vid] : 1.0f;
         const float px = mx0 * sc, py = my0 * sc, pz = mz0 * sc;
         if (vis) {
@@ -153,6 +177,28 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, ps_raster_grads out
         gx += (pm[0] * m_w - pm[3] * mul1) * g2.x + (pm[1] * m_w - pm[3] * mul2) * g2.y;
         gy += (pm[4] * m_w - pm[7] * mul1) * g2.x + (pm[5] * m_w - pm[7] * mul2) * g2.y;
         gz += (pm[8] * m_w - pm[11] * mul1) * g2.x + (pm[9] * m_w - pm[11] * mul2) * g2.y;
+        if (CAM) {
+            // viewmatrix: t = W p + (vm[12], vm[13], vm[14]) and M = J W (W[i][j] = vm[4j+i]);
+            // projmatrix: h = pm p (p.w = 1), screen xy from (hx, hy) / (hw + 1e-7);
+            // tanfov: only through the focal lengths in J (f = size / (2 tanfov); the clamp limit passes nothing)
+            const float j00 = focal_x * tz, j02 = -focal_x * cv.ctx * tz2;
+            const float j11 = focal_y * tz, j12 = -focal_y * cv.cty * tz2;
+            const float p[3] = {px, py, pz};
+            const float dhx = g2.x * m_w, dhy = g2.y * m_w, dhw = -(mul1 * g2.x + mul2 * g2.y);
+#pragma unroll
+            for (int j = 0; j < 3; ++j) {
+                cam[3 * j + 0] = dM0[j] * j00 + dL_dtx * p[j];
+                cam[3 * j + 1] = dM1[j] * j11 + dL_dty * p[j];
+                cam[3 * j + 2] = dM0[j] * j02 + dM1[j] * j12 + dL_dtz * p[j];
+                cam[12 + 3 * j + 0] = dhx * p[j];
+                cam[12 + 3 * j + 1] = dhy * p[j];
+                cam[12 + 3 * j + 2] = dhw * p[j];
+            }
+            cam[9] = dL_dtx; cam[10] = dL_dty; cam[11] = dL_dtz;
+            cam[21] = dhx; cam[22] = dhy; cam[23] = dhw;
+            cam[27] = (dJ00 * tz - dJ02 * cv.ctx * tz2) * (-focal_x / tanfovx);
+            cam[28] = (dJ11 * tz - dJ12 * cv.cty * tz2) * (-focal_y / tanfovy);
+        }
         }   // vis (geometry part)
 
         if (M > 0 && !sh_ready) {          // warp-uniform; the rows have had the geometry math to arrive
@@ -195,6 +241,16 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, ps_raster_grads out
             gx += ((len2 - ddx * ddx) * dLdx - ddy * ddx * dLdy - ddz * ddx * dLdz) * inv3;
             gy += (-ddx * ddy * dLdx + (len2 - ddy * ddy) * dLdy - ddz * ddy * dLdz) * inv3;
             gz += (-ddx * ddz * dLdx - ddy * ddz * dLdy + (len2 - ddz * ddz) * dLdz) * inv3;
+            if (CAM) {
+                // the direction is p - campos.  Rounded intrinsics: plain products shared with the lines above
+                // would change how those are contracted, and the Gaussian gradients must keep their bits.
+                const float xx = __fmul_rn(ddx, ddx), yy = __fmul_rn(ddy, ddy), zz = __fmul_rn(ddz, ddz);
+                const float xy = __fmul_rn(ddx, ddy), xz = __fmul_rn(ddx, ddz), yz = __fmul_rn(ddy, ddz);
+                const float ex = __fadd_rn(__fadd_rn(__fmul_rn(__fsub_rn(len2, xx), dLdx), -__fmul_rn(xy, dLdy)), -__fmul_rn(xz, dLdz));
+                const float ey = __fadd_rn(__fadd_rn(-__fmul_rn(xy, dLdx), __fmul_rn(__fsub_rn(len2, yy), dLdy)), -__fmul_rn(yz, dLdz));
+                const float ez = __fadd_rn(__fadd_rn(-__fmul_rn(xz, dLdx), -__fmul_rn(yz, dLdy)), __fmul_rn(__fsub_rn(len2, zz), dLdz));
+                cam[24] = -__fmul_rn(ex, inv3); cam[25] = -__fmul_rn(ey, inv3); cam[26] = -__fmul_rn(ez, inv3);
+            }
         } else if (vis) {
             dcol[0] += gcol.x; dcol[1] += gcol.y; dcol[2] += gcol.z;
         }
@@ -205,6 +261,30 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, ps_raster_grads out
             const float *__restrict__ vm = in.view + 16 * vid;
             const float dz = vgr.d_color[vg].w * depth_value_grad(d.depth_mode, geo.depth[vg], in.scale, in.near_far, vid);
             dmx += dz * vm[2]; dmy += dz * vm[6]; dmz += dz * vm[10];
+            if (CAM) {   // z = (vm[2], vm[6], vm[10]) . mean + vm[14] / sc
+                cam[2] += dz * mx0; cam[5] += dz * my0; cam[8] += dz * mz0; cam[11] += dz / sc;
+            }
+        }
+        if (CAM) {
+            // per (scene, view) sums over the warp's lanes in a fixed butterfly order; a warp whose Gaussians span
+            // two scenes (P not a multiple of 32) stores one row for each
+            const int s_lo = (int)(sg0 / d.P), s_hi = (int)((sg0 + rows - 1) / d.P);
+            for (int s = s_lo; s <= s_hi; ++s) {
+                const bool mine = (int)scene == s;
+                float sum[kCamEntries];
+#pragma unroll
+                for (int k = 0; k < kCamEntries; ++k) {
+                    float x = mine ? cam[k] : 0.0f;
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+                    sum[k] = x;
+                }
+                if (lane == 0) {
+                    float *r = cam_row(cam_ws, d, s, v, sg0);
+#pragma unroll
+                    for (int k = 0; k < kCamEntries; ++k) r[k] = sum[k];
+                }
+            }
         }
     }
 
@@ -257,22 +337,70 @@ int launch_clear_pair_grads(const Dims &d, const Geom &g, const ViewGrads &vg, c
     return PS_OK;
 }
 
+// One CTA per flat view: sums the view's partial rows in ascending warp order -- 8 strided running sums, then a
+// fixed tree over the 8 -- and writes all 16 / 16 / 3 / 2 entries of the four camera gradients (the entries the
+// forward never reads get 0).  No atomics: the same rows give the same bits.
+constexpr int kCamFinishThreads = 8 * kCamRowFloats;
+
+__global__ void __launch_bounds__(kCamFinishThreads) k_camera_finish(Dims d, const float *__restrict__ ws,
+                                                                     ps_raster_camera_grads cg) {
+    __shared__ float part[8][kCamRowFloats];
+    const int vid = blockIdx.x, s = vid / d.V;
+    const int k = threadIdx.x % kCamRowFloats, grp = threadIdx.x / kCamRowFloats;
+    const long long w_lo = ((long long)s * d.P) / 32, w_hi = ((long long)(s + 1) * d.P - 1) / 32;
+    const int nrows = (int)(w_hi - w_lo + 1);
+    const float *rows = ws + (size_t)vid * cam_rows_per_view(d.P) * kCamRowFloats;
+    float acc = 0.0f;
+    for (int r = grp; r < nrows; r += 8) acc += rows[(size_t)r * kCamRowFloats + k];
+    part[grp][k] = acc;
+    __syncthreads();
+#pragma unroll
+    for (int stride = 4; stride > 0; stride >>= 1) {
+        if (grp < stride) part[grp][k] += part[grp + stride][k];
+        __syncthreads();
+    }
+    const int t = threadIdx.x;
+    if (t < 16) {
+        const int j = t / 4, i = t % 4;
+        if (cg.d_viewmatrix) cg.d_viewmatrix[16 * vid + t] = i == 3 ? 0.0f : part[0][3 * j + i];
+        if (cg.d_projmatrix) cg.d_projmatrix[16 * vid + t] = i == 2 ? 0.0f : part[0][12 + 3 * j + (i == 3 ? 2 : i)];
+    }
+    if (t < 3 && cg.d_campos) cg.d_campos[3 * vid + t] = part[0][24 + t];
+    if (t < 2 && cg.d_tanfov) cg.d_tanfov[2 * vid + t] = part[0][27 + t];
+}
+
+template <bool DEPTH, bool CAM>
+static int launch_preprocess_bwd_kernel(unsigned blocks, size_t smem, const Dims &d, const Inputs &in, const Geom &g,
+                                        const ViewGrads &vg, const GaussGrads &out, int row_stride, float *cam_ws,
+                                        cudaStream_t st) {
+    static unsigned long long attr_devices = 0;
+    if (first_use_on_device(attr_devices))
+        PS_CUDA_CHECK(cudaFuncSetAttribute(k_preprocess_bwd<DEPTH, CAM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           96 * 1024));
+    k_preprocess_bwd<DEPTH, CAM><<<blocks, kPreBwdThreads, smem, st>>>(d, in, g, vg, out, row_stride, cam_ws);
+    PS_LAUNCH_CHECK("k_preprocess_bwd");
+    return PS_OK;
+}
+
 int launch_preprocess_backward(const Dims &d, const Inputs &in, const Geom &g, const ViewGrads &vg,
-                               const ps_raster_grads &out, cudaStream_t st) {
+                               const ps_raster_grads &grads, cudaStream_t st) {
     const int row_stride = d.M > 0 ? ((3 * d.M) | 1) : 1;   // odd word count: conflict-free per-lane rows
     const size_t smem = d.M > 0 ? sizeof(float) * kPreBwdThreads * row_stride * (d.V == 1 ? 1 : 2) : 0;
-    static unsigned long long attr_devices = 0;
-    if (first_use_on_device(attr_devices)) {
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_preprocess_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_preprocess_bwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-    }
     const long long sp = (long long)d.S * d.P;
     const unsigned blocks = (unsigned)((sp + kPreBwdThreads - 1) / kPreBwdThreads);
+    const GaussGrads out{grads.d_means, grads.d_cov, grads.d_opacities, grads.d_sh, grads.d_means2d};
+    const ps_raster_camera_grads *cg = grads.camera;
+    float *ws = cg ? static_cast<float *>(cg->workspace) : nullptr;
+    int rc;
     if (d.depth_mode)
-        k_preprocess_bwd<true><<<blocks, kPreBwdThreads, smem, st>>>(d, in, g, vg, out, row_stride);
+        rc = cg ? launch_preprocess_bwd_kernel<true, true>(blocks, smem, d, in, g, vg, out, row_stride, ws, st)
+                : launch_preprocess_bwd_kernel<true, false>(blocks, smem, d, in, g, vg, out, row_stride, ws, st);
     else
-        k_preprocess_bwd<false><<<blocks, kPreBwdThreads, smem, st>>>(d, in, g, vg, out, row_stride);
-    PS_LAUNCH_CHECK("k_preprocess_bwd");
+        rc = cg ? launch_preprocess_bwd_kernel<false, true>(blocks, smem, d, in, g, vg, out, row_stride, ws, st)
+                : launch_preprocess_bwd_kernel<false, false>(blocks, smem, d, in, g, vg, out, row_stride, ws, st);
+    if (rc || !cg) return rc;
+    k_camera_finish<<<(unsigned)(d.S * d.V), kCamFinishThreads, 0, st>>>(d, ws, *cg);
+    PS_LAUNCH_CHECK("k_camera_finish");
     return PS_OK;
 }
 

@@ -41,26 +41,57 @@ def get_projection_matrix(near: Tensor, far: Tensor, fov_x: Tensor, fov_y: Tenso
     return out
 
 
+class _CameraSetup(torch.autograd.Function):
+    """ps_camera_setup forward, ps_camera_setup_backward backward: (extrinsics, intrinsics) -> (viewmatrix,
+    projmatrix, campos, tanfov, scene_scale).  near, far and scene_scale are not differentiated."""
+
+    @staticmethod
+    def forward(ctx, extrinsics, intrinsics, near, far, scale_invariant: bool):
+        n = extrinsics.shape[0]
+        dev = extrinsics.device
+        f = lambda t: t.to(torch.float32).contiguous()
+        e, k, nr, fr = f(extrinsics), f(intrinsics), f(near), f(far)
+        view = torch.empty((n, 16), dtype=torch.float32, device=dev)
+        proj = torch.empty((n, 16), dtype=torch.float32, device=dev)
+        campos = torch.empty((n, 3), dtype=torch.float32, device=dev)
+        tanfov = torch.empty((n, 2), dtype=torch.float32, device=dev)
+        scale = torch.empty((n,), dtype=torch.float32, device=dev)
+        p = lambda t: ctypes.c_void_p(t.data_ptr())
+        stream = torch.cuda.current_stream(dev)
+        rc = _lib.on_device(dev, _lib.lib.ps_camera_setup, n, p(e), p(k), p(nr), p(fr), 1 if scale_invariant else 0,
+                            p(view), p(proj), p(campos), p(tanfov), p(scale), ctypes.c_void_p(stream.cuda_stream))
+        _lib.check(rc, "ps_camera_setup")
+        ctx.set_materialize_grads(False)
+        ctx.mark_non_differentiable(scale)
+        ctx.save_for_backward(e, k, nr, fr)
+        ctx.scale_invariant = scale_invariant
+        ctx.dtypes = (extrinsics.dtype, intrinsics.dtype)
+        return view, proj, campos, tanfov, scale
+
+    @staticmethod
+    def backward(ctx, d_view, d_proj, d_campos, d_tanfov, _d_scale):
+        e, k, nr, fr = ctx.saved_tensors
+        n, dev = e.shape[0], e.device
+        d_e = torch.empty((n, 4, 4), dtype=torch.float32, device=dev)
+        d_k = torch.empty((n, 3, 3), dtype=torch.float32, device=dev)
+        p = lambda t: None if t is None else ctypes.c_void_p(t.data_ptr())
+        keep = [None if t is None else t.to(torch.float32).contiguous() for t in (d_view, d_proj, d_campos, d_tanfov)]
+        stream = torch.cuda.current_stream(dev)
+        rc = _lib.on_device(dev, _lib.lib.ps_camera_setup_backward, n, p(e), p(k), p(nr), p(fr),
+                            1 if ctx.scale_invariant else 0, *[p(t) for t in keep], p(d_e), p(d_k),
+                            ctypes.c_void_p(stream.cuda_stream))
+        _lib.check(rc, "ps_camera_setup_backward")
+        return (d_e.to(ctx.dtypes[0]) if ctx.needs_input_grad[0] else None,
+                d_k.to(ctx.dtypes[1]) if ctx.needs_input_grad[1] else None, None, None, None)
+
+
 def camera_setup(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor,
                  scale_invariant: bool) -> dict[str, Tensor]:
-    """[n,4,4], [n,3,3], [n], [n] -> rasterizer camera arrays, one kernel launch."""
-    n = extrinsics.shape[0]
-    dev = extrinsics.device
+    """[n,4,4], [n,3,3], [n], [n] -> rasterizer camera arrays, one kernel launch.  Differentiable with respect to
+    extrinsics and intrinsics (one more launch in the backward); not with respect to near and far."""
     if not extrinsics.is_cuda:
         raise ValueError("extrinsics must be a CUDA tensor (pixelsplat_b200 has no CPU path)")
-    f = lambda t: t.to(torch.float32).contiguous()
-    e, k, nr, fr = f(extrinsics), f(intrinsics), f(near), f(far)
-    view = torch.empty((n, 16), dtype=torch.float32, device=dev)
-    proj = torch.empty((n, 16), dtype=torch.float32, device=dev)
-    campos = torch.empty((n, 3), dtype=torch.float32, device=dev)
-    tanfov = torch.empty((n, 2), dtype=torch.float32, device=dev)
-    scale = torch.empty((n,), dtype=torch.float32, device=dev)
-    p = lambda t: ctypes.c_void_p(t.data_ptr())
-    stream = torch.cuda.current_stream(dev)
-    rc = _lib.on_device(dev, _lib.lib.ps_camera_setup, n, p(e), p(k), p(nr), p(fr), 1 if scale_invariant else 0, p(view),
-                                  p(proj), p(campos), p(tanfov), p(scale),
-                                  ctypes.c_void_p(stream.cuda_stream))
-    _lib.check(rc, "ps_camera_setup")
+    view, proj, campos, tanfov, scale = _CameraSetup.apply(extrinsics, intrinsics, near, far, bool(scale_invariant))
     return dict(viewmatrix=view, projmatrix=proj, campos=campos, tanfov=tanfov, scene_scale=scale)
 
 

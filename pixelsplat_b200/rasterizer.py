@@ -325,12 +325,17 @@ class _Rasterize(torch.autograd.Function):
                             target.
     `means2d` [S*V, P, 3] is upstream's gradient holder: it takes no part in the forward and receives the gradient
     with respect to the projected means.  When no gradient reaches `depth` the backward is the colour-only one
-    (ps_raster_backward without a target, ps_raster_backward_loss with one)."""
+    (ps_raster_backward without a target, ps_raster_backward_loss with one).
+    The four camera arrays (viewmatrix, projmatrix, campos, tanfov; the same tensors as in `cams`) are inputs of the
+    Function: when one of them requires grad the backward also returns the camera gradients (ps_raster_camera_grads,
+    include/pixelsplat_b200.h); otherwise its launches and bits are those of the Gaussian-only backward.  background,
+    scene_scale and near_far are not differentiated."""
 
     @staticmethod
-    def forward(ctx, means, cov, opac, sh, means2d, target, cams, cfg: _Config, state_out):
+    def forward(ctx, means, cov, opac, sh, means2d, target, viewmatrix, projmatrix, campos, tanfov, cams,
+                cfg: _Config, state_out):
         ctx.set_materialize_grads(False)
-        backward_follows = any(ctx.needs_input_grad[:5])
+        backward_follows = any(ctx.needs_input_grad[:5]) or any(ctx.needs_input_grad[6:10])
         color, radii, st, sums = _forward(means, cov, opac, sh, cams, cfg, backward_follows, target)
         ctx.save_for_backward(means, cov, opac, sh, target)
         ctx.cams, ctx.st = cams, st
@@ -372,6 +377,15 @@ class _Rasterize(torch.autograd.Function):
         inputs = _raster_inputs(means, cov, opac, sh, ctx.cams)
         grads = _lib.RasterGrads(d_means.data_ptr(), d_cov.data_ptr(), d_opac.data_ptr(), d_sh.data_ptr(),
                                  d_m2d.data_ptr() if d_m2d is not None else None)
+        d_cams = [None] * 4                 # viewmatrix, projmatrix, campos, tanfov
+        if any(ctx.needs_input_grad[6:10]):
+            widths = (16, 16, 3, 2)
+            d_cams = [torch.empty((VT, n), dtype=torch.float32, device=dev) if ctx.needs_input_grad[6 + i] else None
+                      for i, n in enumerate(widths)]
+            cam_ws = torch.empty(_lib.camera_workspace_bytes(desc), dtype=torch.uint8, device=dev)
+            cam = _lib.RasterCameraGrads(*[None if t is None else t.data_ptr() for t in d_cams], cam_ws.data_ptr(),
+                                         cam_ws.numel())
+            grads.camera = ctypes.pointer(cam)
         state = st.raw_state()
         if d_depth is not None:
             d_depth = d_depth.to(torch.float32).contiguous()
@@ -385,7 +399,7 @@ class _Rasterize(torch.autograd.Function):
         rc = _lib.on_device(dev, fn, ctypes.byref(desc), ctypes.byref(inputs), ctypes.byref(state), *args,
                             _ptr(scratch), scratch.numel(), ctypes.byref(grads), ctypes.c_void_p(stream.cuda_stream))
         _lib.check(rc, fn.__name__)
-        return d_means, d_cov, d_opac, d_sh, d_m2d, None, None, None, None
+        return (d_means, d_cov, d_opac, d_sh, d_m2d, None, *d_cams, None, None, None)
 
 
 def _rasterize(means, covariances, opacities, colors, *, viewmatrix, projmatrix, campos, tanfov, background,
@@ -438,7 +452,8 @@ def _rasterize(means, covariances, opacities, colors, *, viewmatrix, projmatrix,
         raise ValueError(f"means2d must be [S*V, P, 3], got {tuple(means2d.shape)}")
     cfg = _Config(S, V, P, M, int(sh_degree), sh_layout, cov_layout, H, W, int(sort_impl),
                   _SH_BASIS if sh_basis is None else convention_id(sh_basis), mode, bool(want_color) or target is None)
-    return _Rasterize.apply(means, covariances, opacities, colors, means2d, target, cams, cfg, state_out)
+    return _Rasterize.apply(means, covariances, opacities, colors, means2d, target, cams["viewmatrix"],
+                            cams["projmatrix"], cams["campos"], cams["tanfov"], cams, cfg, state_out)
 
 
 def rasterize_gaussians(
@@ -464,7 +479,9 @@ def rasterize_gaussians(
     sh_basis=None,                          # "3dgs" / "e3nn"; None = the module default (set_sh_basis)
 ) -> tuple[Tensor, Tensor]:
     """Batched differentiable rasterization: S scenes x V views in one set of launches.
-    Returns (color [S*V, 3, H, W], radii [S*V, P] int32)."""
+    Returns (color [S*V, 3, H, W], radii [S*V, P] int32).  Differentiable with respect to the Gaussians and to
+    viewmatrix, projmatrix, campos and tanfov (tanfov only through the focal lengths; see ps_raster_camera_grads);
+    not with respect to background or scene_scale."""
     color, _, radii, _, _ = _rasterize(
         means, covariances, opacities, colors, viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos,
         tanfov=tanfov, background=background, image_shape=image_shape, views_per_scene=views_per_scene,
