@@ -131,14 +131,16 @@ typedef struct ps_raster_layout {
     size_t clamped;       /* u8   bit c set = channel c was clamped to 0                       */
     size_t tile_count;    /* u32  [S*V*tiles]                                                  */
     size_t tile_start;    /* u32  [S*V*tiles] exclusive scan, global instance offsets          */
-    size_t tile_cursor;   /* u32  scratch                                                      */
+    size_t tile_cursor;   /* u32  [S*V*tiles] after the sort: live entries per tile (keys_alt)  */
     size_t n_instances;   /* i64  [4] instances needed (may exceed capacity), longest segment,
                                      #visible (view,Gaussian) pairs, unused (0)                     */
     size_t vis_pairs;     /* u32  [S*V*P] compact list of on-screen (view,Gaussian) flat indices  */
     size_t vis_any;       /* u32  [S*P]   unused (no longer written; the offset is kept)            */
     /* binning */
     size_t keys;          /* u64  [capacity]  per tile sorted (float_bits(depth)<<32 | gaussian) */
-    size_t keys_alt;      /* u64  [capacity]  scratch                                          */
+    size_t keys_alt;      /* u64  [capacity]  sort scratch; after the sort, per tile at tile_start:
+                             u32x2 (position << 8 | 8x4-block mask, gaussian) of the entries whose
+                             cull box meets the tile, in list order (the compositor's live lists) */
     /* image */
     size_t final_T;       /* f32  [S*V*H*W]                                                    */
     size_t n_contrib;     /* u32  [S*V*H*W]                                                    */

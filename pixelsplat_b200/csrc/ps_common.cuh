@@ -133,6 +133,29 @@ __device__ __forceinline__ float2 cull_extent(float a, float c, float o) {
     return make_float2(sqrtf(tau2 * a) * 1.001f + 0.01f, sqrtf(tau2 * c) * 1.001f + 0.01f);
 }
 
+// Per-tile LIVE LISTS (written by the tile sort, walked by the warp-task compositor).  After a (view, tile) segment
+// is sorted, its entries whose cull box meets at least one of the tile's eight 8x4 pixel blocks are compacted, in
+// list order, into uint2 records (position in the tile's list << 8 | block mask, Gaussian id) at the segment's
+// tile_start offset of keys_alt; tile_cursor[segment] holds how many there are.  Block b of a tile covers pixels
+// x0 + (b & 1) * 8 + 0..7, y0 + (b >> 1) * 4 + 0..3.  A segment longer than kLivePosLimit (positions no longer fit
+// in 24 bits) keeps every entry, so that there the position of a record is its index in the live list.
+constexpr uint32_t kLivePosLimit = 1u << 24;
+
+// Bit b set = the cull record's box meets block b of the tile whose top-left pixel is (x0, y0).  The test (and its
+// float arithmetic) is the one the compositor applied per block before the live lists: alpha >= 1/255 somewhere in
+// the block's rectangle [rx0, rx0 + 7] x [ry0, ry0 + 3] is possible only if the box overlaps it.
+__device__ __forceinline__ uint32_t tile_block_mask(const float4 &cr, int x0, int y0) {
+    const float xl = cr.x - cr.z, xh = cr.x + cr.z, yl = cr.y - cr.w, yh = cr.y + cr.w;
+    uint32_t xm = 0, m = 0;
+#pragma unroll
+    for (int bx = 0; bx < 2; ++bx)
+        xm |= ((xh >= (float)(x0 + 8 * bx)) && (xl <= (float)(x0 + 8 * bx + 7))) ? 1u << bx : 0u;
+#pragma unroll
+    for (int by = 0; by < 4; ++by)
+        m |= ((yh >= (float)(y0 + 4 * by)) && (yl <= (float)(y0 + 4 * by + 3))) ? xm << (2 * by) : 0u;
+    return m;
+}
+
 void set_error(const char *fmt, ...);
 
 // Optional per-stage device timing (bench.py's roofline leg): when enabled, the entry points
@@ -170,18 +193,21 @@ bool first_use_on_device(unsigned long long &mask);
 // stage launchers (each returns PS_OK / PS_ERR_*)
 int launch_preprocess(const Dims &d, const Inputs &in, const Geom &g, cudaStream_t st);
 int launch_sh_color(const Dims &d, const Inputs &in, const Geom &g, cudaStream_t st);
+// `scanned` (may be null) is recorded on `st` once the scan has written the instance count and the longest segment.
 int launch_binning(const Dims &d, const Geom &g, unsigned long long *keys,
-                   unsigned long long *keys_alt, int sort_impl, int segment_hint, cudaStream_t st);
+                   unsigned long long *keys_alt, int sort_impl, int segment_hint, cudaEvent_t scanned,
+                   cudaStream_t st);
 // Deterministic mode (ps_set_option "deterministic"): the forward's loss epilogue goes through loss_partials
 // ([S*V*tiles*8] float2 per-task (sse, sse_clipped), image state) and a fixed-order finish; the backward stores into
 // `records` (the per-(tile block, list position) gradients, 8 x instance_capacity entries of each array, backward
 // scratch) and gathers them into vg in a fixed order.  Null = the default float-atomic path.
+// `live`: the tile sort's live lists (keys_alt, see kLivePosLimit); `keys`: the sorted segments.
 int launch_composite_forward(const Dims &d, const Inputs &in, const Geom &g,
-                             const unsigned long long *keys, const ImageState &img,
+                             const unsigned long long *keys, const uint2 *live, const ImageState &img,
                              float *out_color, const LossEpilogue &loss, const HitLists &hl, float *loss_partials,
                              cudaStream_t st);
 int launch_composite_backward(const Dims &d, const Inputs &in, const Geom &g,
-                              const unsigned long long *keys, const ImageState &img,
+                              const unsigned long long *keys, const uint2 *live, const ImageState &img,
                               const float *d_color, const float *d_depth, const ViewGrads &vg,
                               const ViewGrads *records, const LossEpilogue &loss, const HitLists &hl,
                               cudaStream_t st);

@@ -57,6 +57,7 @@ void mark(int id, cudaStream_t st) {
 struct SideCtx {
     cudaStream_t side = nullptr;
     cudaEvent_t fork = nullptr, join = nullptr;
+    cudaEvent_t scanned = nullptr, copied = nullptr;   // the capacity read-back: after the scan, back before return
     std::mutex enqueue;
 };
 static SideCtx g_side_ctx[64];
@@ -70,6 +71,8 @@ static int side_ready(SideCtx *&ctx) {
     PS_CUDA_CHECK(cudaStreamCreateWithFlags(&ctx->side, cudaStreamNonBlocking));
     PS_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->fork, cudaEventDisableTiming));
     PS_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->join, cudaEventDisableTiming));
+    PS_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->scanned, cudaEventDisableTiming));
+    PS_CUDA_CHECK(cudaEventCreateWithFlags(&ctx->copied, cudaEventDisableTiming));
     return PS_OK;
 }
 
@@ -391,11 +394,19 @@ static int raster_forward_impl(const ps_raster_desc *desc, const ps_raster_input
     PS_CUDA_CHECK(cudaStreamWaitEvent(sc->side, sc->fork, 0));
     if ((rc = launch_sh_color(d, I, g, sc->side))) return rc;
     PS_CUDA_CHECK(cudaEventRecord(sc->join, sc->side));
-    if ((rc = launch_binning(d, g, keys, keys_alt, desc->sort_impl, desc->sort_segment_hint, st))) return rc;
+    if ((rc = launch_binning(d, g, keys, keys_alt, desc->sort_impl, desc->sort_segment_hint,
+                             n_instances_host ? sc->scanned : nullptr, st)))
+        return rc;
     mark(kMarkSort, st);
     PS_CUDA_CHECK(cudaStreamWaitEvent(st, sc->join, 0));   // join
-    if (n_instances_host)
-        PS_CUDA_CHECK(cudaMemcpyAsync(n_instances_host, g.n_instances, 2 * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    if (n_instances_host) {
+        // capacity read-back on the side stream, once the scan has the counts: a device-to-host copy between the sort
+        // and the compositor would sit on the critical path (also of every captured graph); joined back below
+        PS_CUDA_CHECK(cudaStreamWaitEvent(sc->side, sc->scanned, 0));
+        PS_CUDA_CHECK(cudaMemcpyAsync(n_instances_host, g.n_instances, 2 * sizeof(int64_t), cudaMemcpyDeviceToHost,
+                                      sc->side));
+        PS_CUDA_CHECK(cudaEventRecord(sc->copied, sc->side));
+    }
     // (deterministic mode: the fixed-order finish writes every slot)
     float *loss_partials = L.det ? reinterpret_cast<float *>(static_cast<char *>(state->image) + L.loss_partials) : nullptr;
     if (le.sums && !loss_partials)
@@ -405,7 +416,10 @@ static int raster_forward_impl(const ps_raster_desc *desc, const ps_raster_input
         hl.hits = reinterpret_cast<uint2 *>(static_cast<char *>(state->binning) + L.off.block_hits);
         hl.run_hits = reinterpret_cast<uint32_t *>(static_cast<char *>(state->binning) + L.off.run_hits);
     }
-    if ((rc = launch_composite_forward(d, I, g, keys, img, out_color, le, hl, loss_partials, st))) return rc;
+    if ((rc = launch_composite_forward(d, I, g, keys, reinterpret_cast<const uint2 *>(keys_alt), img, out_color, le, hl,
+                                       loss_partials, st)))
+        return rc;
+    if (n_instances_host) PS_CUDA_CHECK(cudaStreamWaitEvent(st, sc->copied, 0));   // join the read-back
     mark(kMarkCompositeFwd, st);
     if (out_radii)
         PS_CUDA_CHECK(cudaMemcpyAsync(out_radii, g.radii, sizeof(int32_t) * (size_t)d.S * d.V * d.P,
@@ -465,6 +479,7 @@ static int raster_backward_impl(const ps_raster_desc *desc, const ps_raster_inpu
     const Inputs I = make_inputs(in);
     const Geom g = make_geom(L, state->geom);
     const unsigned long long *keys = reinterpret_cast<const unsigned long long *>(static_cast<char *>(state->binning) + L.off.keys);
+    const uint2 *live = reinterpret_cast<const uint2 *>(static_cast<char *>(state->binning) + L.off.keys_alt);
     const ImageState img = make_image(L, state->image);
     const size_t vp = (size_t)d.S * d.V * d.P;
     char *sb = static_cast<char *>(scratch);
@@ -487,7 +502,8 @@ static int raster_backward_impl(const ps_raster_desc *desc, const ps_raster_inpu
         hl.hits = reinterpret_cast<uint2 *>(static_cast<char *>(state->binning) + L.off.block_hits);
         hl.run_hits = reinterpret_cast<uint32_t *>(static_cast<char *>(state->binning) + L.off.run_hits);
     }
-    if ((rc = launch_composite_backward(d, I, g, keys, img, d_color, d_depth, vg, L.det ? &rec : nullptr, le, hl, st)))
+    if ((rc = launch_composite_backward(d, I, g, keys, live, img, d_color, d_depth, vg, L.det ? &rec : nullptr, le, hl,
+                                        st)))
         return rc;
     mark(kMarkCompositeBwd, st);
     if ((rc = launch_preprocess_backward(d, I, g, vg, *grads, st))) return rc;

@@ -1,5 +1,6 @@
 // Binning: (view, tile) instance counts -> exclusive scan -> scatter of
-// (float_bits(depth) << 32 | gaussian) keys into per-tile segments -> per-tile LSD radix sort.
+// (float_bits(depth) << 32 | gaussian) keys into per-tile segments -> per-tile LSD radix sort -> per-tile live
+// list (the entries whose cull box meets the tile, with their 8x4 block masks; see kLivePosLimit).
 //
 // The sorted order inside a tile (ascending depth bits, ties by ascending Gaussian index) is
 // exactly what upstream obtains from its global stable radix sort of (tile << 32 | depth) keys
@@ -166,9 +167,13 @@ __device__ void bitonic_sort_smem(unsigned long long *s_keys, int n_pad) {
 constexpr int kSortThreads = 512;   // 64 regs x 512 threads: two CTAs per SM
 constexpr int kSortWarps = kSortThreads / 32;
 
+constexpr int kLiveItems = 4;      // entries per thread per round of the live-list compaction
+static_assert(kLiveItems * kSortWarps == 64, "write_live_list scans the (item, warp) counts two per lane");
+
 struct SortSmem {
     uint32_t cnt[kSortWarps * 256];
     uint32_t misc[64];
+    uint32_t live[kLiveItems * kSortWarps];   // per-(item, warp) live counts of a compaction round
 };
 
 // passes [0, num_passes): digit p = ((key >> key_shift) - sub) >> (8 p) & 255 (key_shift = 32 and
@@ -242,17 +247,76 @@ __device__ unsigned long long *radix8_passes(unsigned long long *a, unsigned lon
 
 static size_t sort_smem_bytes(int cap) { return sizeof(SortSmem) + sizeof(unsigned long long) * 2 * (size_t)cap; }
 
+// The live list of segment `seg` (see kLivePosLimit) from its sorted keys `sorted[0, n)` (shared or global memory),
+// written by the whole CTA: rounds of kSortThreads * kLiveItems entries, each thread gathering the cull records of
+// kLiveItems entries at once (one L2 latency per round), then a stable CTA-wide compaction in list order.
+__device__ void write_live_list(const Dims &d, const Geom &geo, const unsigned long long *sorted, int n, int seg,
+                                uint2 *__restrict__ live, SortSmem &sm) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int vid = seg / d.tiles, tile = seg - vid * d.tiles;
+    const int x0 = (tile % d.gx) * kTile, y0 = (tile / d.gx) * kTile;
+    const float4 *__restrict__ cull = geo.cull + (size_t)vid * d.P;
+    const bool keep_all = (uint32_t)n > kLivePosLimit;
+    uint32_t carry = 0;
+    for (int base = 0; base < n; base += kSortThreads * kLiveItems) {
+        uint32_t g[kLiveItems];
+        float4 cr[kLiveItems];
+#pragma unroll
+        for (int k = 0; k < kLiveItems; ++k) {
+            const int i = base + k * kSortThreads + tid;
+            g[k] = i < n ? (uint32_t)sorted[i] : 0u;
+            cr[k] = i < n ? cull[g[k]] : make_float4(0.0f, 0.0f, -3.0e38f, -3.0e38f);
+        }
+        uint32_t mask[kLiveItems], ballot[kLiveItems];
+#pragma unroll
+        for (int k = 0; k < kLiveItems; ++k) {
+            const int i = base + k * kSortThreads + tid;
+            mask[k] = i < n ? tile_block_mask(cr[k], x0, y0) : 0u;
+            ballot[k] = __ballot_sync(0xffffffffu, i < n && (mask[k] != 0u || keep_all));
+            if (lane == 0) sm.live[k * kSortWarps + warp] = (uint32_t)__popc(ballot[k]);
+        }
+        __syncthreads();
+        // exclusive prefix of the 64 (item, warp) counts in list order, two per lane, by every warp at once
+        const uint32_t c0 = sm.live[lane], c1 = sm.live[32 + lane];
+        uint32_t e0 = c0, e1 = c1;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t y0 = __shfl_up_sync(0xffffffffu, e0, o), y1 = __shfl_up_sync(0xffffffffu, e1, o);
+            if (lane >= o) { e0 += y0; e1 += y1; }
+        }
+        const uint32_t half = __shfl_sync(0xffffffffu, e0, 31);
+        const uint32_t total = half + __shfl_sync(0xffffffffu, e1, 31);
+        e0 -= c0;
+        e1 += half - c1;
+        uint32_t off[kLiveItems];      // (item k, this warp) sits at index k * 16 + warp
+        off[0] = carry + __shfl_sync(0xffffffffu, e0, warp);
+        off[1] = carry + __shfl_sync(0xffffffffu, e0, 16 + warp);
+        off[2] = carry + __shfl_sync(0xffffffffu, e1, warp);
+        off[3] = carry + __shfl_sync(0xffffffffu, e1, 16 + warp);
+        carry += total;
+#pragma unroll
+        for (int k = 0; k < kLiveItems; ++k) {
+            const int i = base + k * kSortThreads + tid;
+            if ((ballot[k] >> lane) & 1u)
+                live[off[k] + (uint32_t)__popc(ballot[k] & ((1u << lane) - 1u))] =
+                    make_uint2(((uint32_t)i << 8) | mask[k], g[k]);
+        }
+        __syncthreads();
+    }
+    if (tid == 0) geo.tile_cursor[seg] = carry;
+}
+
 __global__ void __launch_bounds__(kSortThreads)
-k_tile_sort(const uint32_t *__restrict__ tile_start, const uint32_t *__restrict__ tile_count,
-            const long long *__restrict__ n_instances, long long capacity,
-            unsigned long long *__restrict__ keys, unsigned long long *__restrict__ keys_alt, int cap, int id_bits) {
+k_tile_sort(Dims d, Geom geo, unsigned long long *__restrict__ keys, unsigned long long *__restrict__ keys_alt,
+            int cap, int id_bits) {
     extern __shared__ __align__(16) unsigned char s_sort[];
-    if (*n_instances > capacity) return;
+    if (*geo.n_instances > d.capacity) return;
     const int seg = blockIdx.x;
-    const int n = (int)tile_count[seg];
-    if (n < 2) return;
-    const uint32_t s0 = tile_start[seg];
+    const int n = (int)geo.tile_count[seg];
+    const uint32_t s0 = geo.tile_start[seg];
     SortSmem &sm = *reinterpret_cast<SortSmem *>(s_sort);
+    uint2 *live = reinterpret_cast<uint2 *>(keys_alt + s0);   // keys_alt is dead once the segment is sorted
+    if (n < 2) { write_live_list(d, geo, keys + s0, n, seg, live, sm); return; }
     const int tid = threadIdx.x, lane = tid & 31;
     if (n > cap) {   // too long for shared memory: full-key radix through HBM
         unsigned long long *r = radix8_passes(keys + s0, keys_alt + s0, n, sm, 0, 0u, (id_bits + 7) / 8);
@@ -260,6 +324,8 @@ k_tile_sort(const uint32_t *__restrict__ tile_start, const uint32_t *__restrict_
         r = radix8_passes(r, o, n, sm, 32, 0u, 4);
         if (r != keys + s0)
             for (int i = tid; i < n; i += kSortThreads) keys[s0 + i] = r[i];
+        __syncthreads();
+        write_live_list(d, geo, keys + s0, n, seg, live, sm);
         return;
     }
     unsigned long long *A = reinterpret_cast<unsigned long long *>(s_sort + sizeof(SortSmem));
@@ -310,13 +376,26 @@ k_tile_sort(const uint32_t *__restrict__ tile_start, const uint32_t *__restrict_
         bitonic_sort_smem<kSortThreads>(A, n_pad);
     }
     for (int i = tid; i < n; i += kSortThreads) keys[s0 + i] = A[i];
+    write_live_list(d, geo, A, n, seg, live, sm);
+}
+
+// The live lists after the CUB debug sort (one CTA per segment, as in k_tile_sort).
+__global__ void __launch_bounds__(kSortThreads)
+k_live_lists(Dims d, Geom geo, const unsigned long long *__restrict__ keys, unsigned long long *__restrict__ keys_alt) {
+    __shared__ SortSmem sm;
+    if (*geo.n_instances > d.capacity) return;
+    const int seg = blockIdx.x;
+    const uint32_t s0 = geo.tile_start[seg];
+    write_live_list(d, geo, keys + s0, (int)geo.tile_count[seg], seg, reinterpret_cast<uint2 *>(keys_alt + s0), sm);
 }
 
 int launch_binning(const Dims &d, const Geom &g, unsigned long long *keys,
-                   unsigned long long *keys_alt, int sort_impl, int segment_hint, cudaStream_t st) {
+                   unsigned long long *keys_alt, int sort_impl, int segment_hint, cudaEvent_t scanned,
+                   cudaStream_t st) {
     const int n_seg = d.S * d.V * d.tiles;
     k_tile_scan<<<1, kScanThreads, 0, st>>>(n_seg, g.tile_count, g.tile_start, g.tile_cursor, g.n_instances);
     PS_LAUNCH_CHECK("k_tile_scan");
+    if (scanned) PS_CUDA_CHECK(cudaEventRecord(scanned, st));
     const int use_smem = d.tiles <= kScatterMaxSmemTiles;
     static unsigned long long scatter_attr_devices = 0;
     if (first_use_on_device(scatter_attr_devices)) {
@@ -346,6 +425,8 @@ int launch_binning(const Dims &d, const Geom &g, unsigned long long *keys,
             PS_CUDA_CHECK(cudaMemcpyAsync(keys, db.Current(), sizeof(unsigned long long) * (size_t)d.capacity,
                                           cudaMemcpyDeviceToDevice, st));
         PS_CUDA_CHECK(cudaFreeAsync(tmp, st));
+        k_live_lists<<<n_seg, kSortThreads, 0, st>>>(d, g, keys, keys_alt);
+        PS_LAUNCH_CHECK("k_live_lists");
         return PS_OK;
     }
 
@@ -361,8 +442,7 @@ int launch_binning(const Dims &d, const Geom &g, unsigned long long *keys,
         PS_CUDA_CHECK(cudaFuncSetAttribute(k_tile_sort, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)sort_smem_bytes(8192)));
     }
-    k_tile_sort<<<n_seg, kSortThreads, sort_smem_bytes(cap), st>>>(
-        g.tile_start, g.tile_count, g.n_instances, d.capacity, keys, keys_alt, cap, id_bits);
+    k_tile_sort<<<n_seg, kSortThreads, sort_smem_bytes(cap), st>>>(d, g, keys, keys_alt, cap, id_bits);
     PS_LAUNCH_CHECK("k_tile_sort");
     return PS_OK;
 }

@@ -5,12 +5,12 @@
 // (SURVEY.md A.3 / A.5; the call the reference makes at
 // /root/reference/src/model/decoder/cuda_splatting.py:113-124) without changing a per-pixel decision.
 //
-// Front end (shared by both directions): the warp streams the tile's depth-sorted instance list 32
-// entries at a time -- key -> Gaussian id -> 16-byte cull record (screen position + half-extents of the
-// box outside of which alpha < 1/255, written by k_preprocess) -- tests the box against its 8x4
-// rectangle, and only for the hits gathers conic/opacity/colour into a per-warp shared-memory queue.
-// The three dependent loads are software-pipelined across iterations (keys two chunks ahead, cull
-// records one ahead, hit records parked one iteration later), so nothing waits on L2.
+// Front end (shared by both directions): the warp streams the tile's LIVE LIST 32 records at a time (written by
+// the tile sort, ps_common.cuh: the entries whose alpha >= 1/255 box meets the tile, in list order, each with the
+// mask of the 8x4 blocks the box meets), takes a ballot of its block's mask bit, and only for the hits gathers
+// position/conic/opacity/colour into a per-warp shared-memory queue.  The box test happened once per entry in the
+// sort, not once per block here.  The loads are software-pipelined across iterations (records one chunk ahead,
+// hit records parked one iteration later), so nothing waits on L2.
 //
 // Both kernels are bound by instruction issue (ncu: 65-80 % issue-active forward), so the per-hit loop is
 // built to be short:
@@ -109,12 +109,10 @@ __device__ __forceinline__ float hit_power2(const float4 &a0, const float4 &a1, 
     return fmaf(fj, t2, fmaf(fi, t1, a0.x));
 }
 
-// Registers of the cull pipeline (see file header).
+// Registers of the live-list pipeline (see file header).
 struct CullPipe {
-    unsigned long long key_next;   // keys of chunk c + 2
-    float4 cr;                     // cull record of chunk c + 1 (this lane's entry)
-    uint32_t g;                    // its Gaussian id
-    // hit of chunk c waiting to be parked in the queue
+    uint2 rec;                     // live record of chunk c (this lane's entry)
+    // hit of chunk c - 1 waiting to be parked in the queue
     float4 h_co, h_rgb;
     float2 h_xy;
     uint32_t h_g, h_pos, h_slot;
@@ -122,16 +120,21 @@ struct CullPipe {
 };
 
 struct TaskGeom {
-    int vid, pxi, pyi;
+    int vid, pxi, pyi, sub;
     bool inside;
     float fi, fj;                 // block-local pixel offsets of this lane (0..7, 0..3)
-    float rx0, rx1, ry0, ry1;     // the block's pixel rectangle
+    float rx0, ry0;               // the block's origin
     uint32_t start, count;        // the tile's list
-    uint32_t run_begin, run_len;  // this warp's run of it (whole list when segK == 1)
+    uint32_t run_begin, run_len;  // this warp's run of it, in list positions (whole list when segK == 1)
+    const uint2 *live;            // the tile's live list (ps_common.cuh, kLivePosLimit)
+    uint32_t n_live;              // its length
+    uint32_t live_begin;          // index of the run's first live entry; the run takes the live entries from there
+                                  // on whose position is < run_begin + run_len
     size_t gbase, pix, hw;
 };
 
-// Run k of segK over a list of `count` entries: whole 32-entry chunks, the same split in both directions.
+// Run k of segK over a list of `count` entries: whole 32-entry chunks of the FULL list, the same split in both
+// directions (so the fold of the runs, and with it every pixel's bits, does not depend on the live lists).
 __device__ __forceinline__ void run_bounds(uint32_t count, int segK, int k, uint32_t &begin, uint32_t &len) {
     const uint32_t chunks = (count + 31u) >> 5;
     const uint32_t per = (chunks + (uint32_t)segK - 1u) / (uint32_t)segK;
@@ -139,44 +142,64 @@ __device__ __forceinline__ void run_bounds(uint32_t count, int segK, int k, uint
     len = min(count, (uint32_t)(k + 1) * per * 32u) - begin;
 }
 
-__device__ __forceinline__ bool task_setup(const Dims &d, const Geom &geo, long long task, int lane, TaskGeom &t) {
-    const int sub = (int)(task & 7);
+__device__ __forceinline__ bool task_setup(const Dims &d, const Geom &geo, const uint2 *live, long long task, int lane,
+                                           TaskGeom &t) {
+    t.sub = (int)(task & 7);
     const long long seg = task >> 3;
     if (seg >= (long long)d.S * d.V * d.tiles) return false;
     t.vid = (int)(seg / d.tiles);
     const int tile = (int)(seg - (long long)t.vid * d.tiles);
     const int tx = tile % d.gx, ty = tile / d.gx;
-    const int wx0 = tx * kTile + (sub & 1) * 8, wy0 = ty * kTile + (sub >> 1) * 4;
+    const int wx0 = tx * kTile + (t.sub & 1) * 8, wy0 = ty * kTile + (t.sub >> 1) * 4;
     t.pxi = wx0 + (lane & 7);
     t.pyi = wy0 + (lane >> 3);
     t.inside = t.pxi < d.W && t.pyi < d.H;
     t.fi = (float)(lane & 7); t.fj = (float)(lane >> 3);
-    t.rx0 = (float)wx0; t.rx1 = (float)(wx0 + 7); t.ry0 = (float)wy0; t.ry1 = (float)(wy0 + 3);
+    t.rx0 = (float)wx0; t.ry0 = (float)wy0;
     t.start = geo.tile_start[seg];
     t.count = geo.tile_count[seg];
     t.run_begin = 0;
     t.run_len = t.count;
+    t.live = live + t.start;
+    t.n_live = 0;
+    t.live_begin = 0;
     t.gbase = (size_t)t.vid * d.P;
     t.hw = (size_t)d.H * d.W;
     t.pix = (size_t)t.pyi * d.W + t.pxi;
     return true;
 }
 
-// ---- cull pipeline ------------------------------------------------------------------------------
-__device__ __forceinline__ void cull_prologue(CullPipe &p, const Geom &geo, const TaskGeom &t,
-                                              const unsigned long long *__restrict__ keys, uint32_t n, int lane) {
+// Index of the first live entry at list position >= pos (n_live if none): a 32-way search, two or three rounds of
+// coalescing-free but independent loads for the lists seen in practice.
+__device__ __forceinline__ uint32_t live_lower_bound(const TaskGeom &t, uint32_t pos, int lane) {
+    if (t.count > kLivePosLimit) return min(pos, t.n_live);     // every entry kept: index = position
+    uint32_t lo = 0, hi = t.n_live;                             // the answer lies in [lo, hi]
+    while (lo < hi) {
+        const uint32_t step = (hi - lo + 31u) >> 5;
+        const uint32_t i = lo + (uint32_t)lane * step;
+        const bool below = i < hi && (t.live[i].x >> 8) < pos;
+        const uint32_t c = (uint32_t)__popc(__ballot_sync(0xffffffffu, below));
+        if (c == 0) break;
+        lo += (c - 1u) * step + 1u;       // past the last probe below pos; the next probe (if any) is not
+        hi = min(hi, lo - 1u + step);
+    }
+    return lo;
+}
+
+// Positions the run [run_begin, run_begin + run_len) of the task's list on its live list.
+__device__ __forceinline__ void live_run(TaskGeom &t, const Geom &geo, long long task, int lane) {
+    t.n_live = geo.tile_cursor[task >> 3];
+    t.live_begin = t.run_len == 0 ? t.n_live : t.run_begin == 0 ? 0u : live_lower_bound(t, t.run_begin, lane);
+}
+
+// ---- live-list pipeline ---------------------------------------------------------------------------
+__device__ __forceinline__ void cull_prologue(CullPipe &p, const TaskGeom &t, int lane) {
     p.h_pending = false;
     p.h_slot = 0; p.h_g = 0; p.h_pos = 0;
     p.h_xy = make_float2(0.0f, 0.0f);
     p.h_co = p.h_rgb = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-    p.g = 0;
-    p.cr = make_float4(0.0f, 0.0f, -3.0e38f, -3.0e38f);
-    p.key_next = 0;
-    if ((uint32_t)lane < n) {
-        p.g = (uint32_t)keys[t.start + t.run_begin + lane];
-        p.cr = geo.cull[t.gbase + p.g];
-    }
-    if (32u + (uint32_t)lane < n) p.key_next = keys[t.start + t.run_begin + 32u + lane];
+    p.rec = make_uint2(0u, 0u);
+    if (t.live_begin + (uint32_t)lane < t.n_live) p.rec = t.live[t.live_begin + lane];
 }
 
 // Parks the hit found in the previous iteration (its gathers have had a whole iteration to land): forms the
@@ -219,35 +242,32 @@ __device__ __forceinline__ uint32_t queue_pad(HitQueue &q, uint32_t tail, int la
     return padded;
 }
 
-// Tests chunk c (positions 32c .. 32c+31 of the warp's run, n = run length) and advances the pipeline.
-// Returns the number of hits; they become readable in the queue after the NEXT cull_park.
-__device__ __forceinline__ int cull_step(CullPipe &p, const Geom &geo, const TaskGeom &t,
-                                         const unsigned long long *__restrict__ keys, uint32_t n, uint32_t c,
-                                         uint32_t tail, int lane, uint2 *__restrict__ hit_out = nullptr) {
-    const uint32_t pos = c * 32u + (uint32_t)lane;
-    const float4 cr = p.cr;
-    const bool hit = pos < n && (cr.x + cr.z >= t.rx0) && (cr.x - cr.z <= t.rx1) && (cr.y + cr.w >= t.ry0) &&
-                     (cr.y - cr.w <= t.ry1);
+// Takes chunk c of the run's live entries (indices live_begin + 32c ...): the block's mask bit decides, nothing is
+// box-tested here.  Returns the number of hits -- they become readable in the queue after the NEXT cull_park -- or
+// -1 when the chunk lies past the run.
+__device__ __forceinline__ int cull_step(CullPipe &p, const Geom &geo, const TaskGeom &t, uint32_t c, uint32_t tail,
+                                         int lane, uint2 *__restrict__ hit_out = nullptr) {
+    const uint32_t i = t.live_begin + c * 32u + (uint32_t)lane;
+    const uint2 rec = p.rec;
+    const uint32_t pos = t.count > kLivePosLimit ? i : rec.x >> 8;   // position in the TILE's list
+    const bool in_run = i < t.n_live && pos < t.run_begin + t.run_len;
+    if (!__any_sync(0xffffffffu, in_run)) return -1;
+    const bool hit = in_run && ((rec.x >> t.sub) & 1u);
     const uint32_t mask = __ballot_sync(0xffffffffu, hit);
     if (hit) {
         p.h_pending = true;
         const uint32_t idx = tail + (uint32_t)__popc(mask & ((1u << lane) - 1u));
         p.h_slot = idx & (kQ - 1);
-        p.h_g = p.g;
-        p.h_pos = t.run_begin + pos;          // position in the TILE's list (n_contrib semantics)
-        if (hit_out) hit_out[idx] = make_uint2(p.h_pos, p.g);     // the backward walks this list instead of culling
-        p.h_xy = make_float2(cr.x, cr.y);
-        p.h_co = geo.conic_opacity[t.gbase + p.g];
-        p.h_rgb = geo.rgb[t.gbase + p.g];
+        p.h_g = rec.y;
+        p.h_pos = pos;                        // (n_contrib semantics)
+        if (hit_out) hit_out[idx] = make_uint2(pos, rec.y);     // the backward walks this list instead
+        p.h_xy = *reinterpret_cast<const float2 *>(geo.cull + t.gbase + rec.y);
+        p.h_co = geo.conic_opacity[t.gbase + rec.y];
+        p.h_rgb = geo.rgb[t.gbase + rec.y];
     }
-    // advance: cull record of chunk c+1 from the key loaded an iteration ago, key of chunk c+2
-    const uint32_t pos1 = pos + 32u, pos2 = pos + 64u;
-    p.cr = make_float4(0.0f, 0.0f, -3.0e38f, -3.0e38f);
-    if (pos1 < n) {
-        p.g = (uint32_t)p.key_next;
-        p.cr = geo.cull[t.gbase + p.g];
-    }
-    if (pos2 < n) p.key_next = keys[t.start + t.run_begin + pos2];
+    // advance: the live record of chunk c + 1
+    p.rec = make_uint2(0u, 0u);
+    if (i + 32u < t.n_live) p.rec = t.live[i + 32u];
     return __popc(mask);
 }
 
@@ -304,27 +324,27 @@ __device__ __forceinline__ void fwd_blend4(const HitQueue &q, uint32_t base, con
 
 // Front-to-back blend of the warp's run [t.run_begin, t.run_begin + t.run_len) onto the per-lane state px.
 template <bool DEPTH>
-__device__ __forceinline__ uint32_t fwd_run(const Geom &geo, const TaskGeom &t, const unsigned long long *__restrict__ keys,
-                                            HitQueue &q, FwdPixel &px, int lane, uint2 *__restrict__ hit_out = nullptr) {
-    const uint32_t n = t.run_len;
+__device__ __forceinline__ uint32_t fwd_run(const Geom &geo, const TaskGeom &t, HitQueue &q, FwdPixel &px, int lane,
+                                            uint2 *__restrict__ hit_out = nullptr) {
     float T = px.T, Cr = px.Cr, Cg = px.Cg, Cb = px.Cb, D = px.D;
     uint32_t last = px.last;
     bool done = px.done, stopped = px.stopped;
     CullPipe p;
-    cull_prologue(p, geo, t, keys, n, lane);
+    cull_prologue(p, t, lane);
     uint32_t head = 0, tail = 0;
-    const uint32_t nchunks = (n + 31u) >> 5;
-    for (uint32_t c = 0; c <= nchunks; ++c) {          // one extra iteration drains the last parked hits
+    for (uint32_t c = 0;; ++c) {                       // the first chunk past the run drains the last parked hits
         cull_park<false, DEPTH>(p, q, nullptr, t);
         uint32_t avail = tail;                         // parked so far
-        if (c < nchunks) tail += (uint32_t)cull_step(p, geo, t, keys, n, c, tail, lane, hit_out);
+        const int nh = cull_step(p, geo, t, c, tail, lane, hit_out);
+        if (nh >= 0) tail += (uint32_t)nh;
         else avail = queue_pad(q, tail, lane);
         // whole groups of four (their power / exp evaluations are independent, only the transmittance chains)
         while (avail - head >= 4u) {
             fwd_blend4<DEPTH>(q, head & (kQ - 1), t, T, Cr, Cg, Cb, D, last, done, stopped);
             head += 4u;
         }
-        if (__all_sync(0xffffffffu, done)) break;     // (hits beyond this point are behind every pixel's last contributor)
+        // (hits beyond this point are behind every pixel's last contributor)
+        if (nh < 0 || __all_sync(0xffffffffu, done)) break;
         __syncwarp();
     }
     __syncwarp();
@@ -338,38 +358,41 @@ __device__ __forceinline__ uint32_t fwd_run(const Geom &geo, const TaskGeom &t, 
 // only DET instantiations are built for the DEPTH ones' CTA counts so that they do not spill.
 template <int K, bool DEPTH, bool DET>
 __global__ void __launch_bounds__(kFwdWarps * 32, (DEPTH || DET) ? (K > 1 ? 4 : 5) : PS_FWD_MIN_CTAS)
-k_composite_fwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsigned long long *__restrict__ keys,
+k_composite_fwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const uint2 *__restrict__ live,
                  ImageState img, float *__restrict__ out_color, LossEpilogue loss, HitLists hl) {
     __shared__ HitQueue s_q[kFwdWarps];
     __shared__ float4 s_ct[K > 1 ? kFwdWarps : 1][32];      // a run's (Cr, Cg, Cb, T)
     __shared__ float s_d[K > 1 && DEPTH ? kFwdWarps : 1][32];   // its depth
     __shared__ uint32_t s_last[K > 1 ? kFwdWarps : 1][32];   // its last contributor | stopped << 31
+    __shared__ uint32_t s_live_begin[K > 1 ? kFwdWarps : 1];   // where each run starts on the live list
     constexpr int kTasksPerCta = kFwdWarps / K;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int run = warp % K;
     HitQueue &q = s_q[warp];
     TaskGeom t;
-    const bool valid = task_setup(d, geo, (long long)blockIdx.x * kTasksPerCta + warp / K, lane, t);
+    const long long task = (long long)blockIdx.x * kTasksPerCta + warp / K;
+    const bool valid = task_setup(d, geo, live, task, lane, t);
     const bool truncated = *geo.n_instances > d.capacity;
     const uint32_t count = (valid && !truncated) ? t.count : 0u;
     t.count = count;
     t.run_len = count;
     if (K > 1) run_bounds(count, K, run, t.run_begin, t.run_len);
+    if (count) live_run(t, geo, task, lane);
 
     FwdPixel px;
     px.T = 1.0f; px.Cr = px.Cg = px.Cb = 0.0f; px.D = 0.0f;
     px.last = 0; px.stopped = false;
     px.done = !valid || !t.inside;
     if (valid) {
-        const long long task = (long long)blockIdx.x * kTasksPerCta + warp / K;
         uint2 *hit_out = nullptr;
         if (hl.hits)   // this run's slice of the block's region (a run has at most run_len hits)
             hit_out = hl.hits + ((size_t)t.start * 8 + (size_t)(task & 7) * t.count + t.run_begin);
-        const uint32_t nh = fwd_run<DEPTH>(geo, t, keys, q, px, lane, hit_out);
+        const uint32_t nh = fwd_run<DEPTH>(geo, t, q, px, lane, hit_out);
         if (hl.run_hits && lane == 0) hl.run_hits[task * kMaxSegments + run] = nh;
     }
 
     if (K > 1) {
+        if (lane == 0) s_live_begin[warp] = t.live_begin;
         s_ct[warp][lane] = make_float4(px.Cr, px.Cg, px.Cb, px.T);
         if (DEPTH) s_d[warp][lane] = px.D;
         s_last[warp][lane] = px.last | (px.stopped ? 0x80000000u : 0u);
@@ -389,9 +412,10 @@ k_composite_fwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
                 // the pixel saturates inside (or near) run j: replay it with the true transmittance
                 TaskGeom tj = t;
                 run_bounds(count, K, j, tj.run_begin, tj.run_len);
+                tj.live_begin = s_live_begin[warp + j];
                 FwdPixel pj = px;
                 pj.done = px.done || !replay;
-                fwd_run<DEPTH>(geo, tj, keys, q, pj, lane);
+                fwd_run<DEPTH>(geo, tj, q, pj, lane);
                 if (replay) px = pj;
             }
             if (!replay && !px.done) {
@@ -578,7 +602,7 @@ __device__ __forceinline__ void bwd_batch(BwdSmem<DEPTH> &sm, BwdPixel &px, cons
 // DET: vg points at the block records (see the file header).
 template <int K, bool DEPTH, bool DET>
 __global__ void __launch_bounds__(kBwdWarps * 32, DEPTH ? 5 : 6)
-k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsigned long long *__restrict__ keys,
+k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const uint2 *__restrict__ live,
                  ImageState img, const float *__restrict__ d_color, const float *__restrict__ d_depth, ViewGrads vg,
                  LossEpilogue loss, HitLists hl) {
     extern __shared__ __align__(16) unsigned char s_raw[];
@@ -588,7 +612,8 @@ k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
     BwdSmem<DEPTH> &sm = reinterpret_cast<BwdSmem<DEPTH> *>(s_raw)[warp];
     if (*geo.n_instances > d.capacity) return;
     TaskGeom t;
-    if (!task_setup(d, geo, (long long)blockIdx.x * kTasksPerCta + warp / K, lane, t)) return;
+    const long long task = (long long)blockIdx.x * kTasksPerCta + warp / K;
+    if (!task_setup(d, geo, live, task, lane, t)) return;
 
     BwdPixel px;
     px.T = 1.0f; px.S = 0.0f;
@@ -631,14 +656,11 @@ k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
     const float kx = kLn2 * 0.5f * (float)d.W, ky = kLn2 * 0.5f * (float)d.H;
     (void)bg_all;
     // DET: this block's records of the tile's list (the hit lists' index space)
-    const size_t rbase = DET ? (size_t)t.start * 8 + (size_t)(((long long)blockIdx.x * kTasksPerCta + warp / K) & 7) *
-                                                         t.count
-                             : 0;
+    const size_t rbase = DET ? (size_t)t.start * 8 + (size_t)(task & 7) * t.count : 0;
 
     uint32_t head = 0, tail = 0;
     if (hl.hits) {
         // ---- the forward left this run's hit list: no cull, every lane parks a hit
-        const long long task = (long long)blockIdx.x * kTasksPerCta + warp / K;
         const uint2 *__restrict__ hits = hl.hits + ((size_t)t.start * 8 + (size_t)(task & 7) * t.count + t.run_begin);
         const uint32_t nh = n ? hl.run_hits[task * kMaxSegments + run] : 0u;
         uint2 hnext = make_uint2(0u, 0u);
@@ -675,17 +697,20 @@ k_composite_bwd2(Dims d, Geom geo, const float *__restrict__ bg_all, const unsig
             if (m != 0xffffffffu) break;                                      // the list is ordered by position
         }
     } else {
+        // ---- walk the run's live entries in front of nmax
+        live_run(t, geo, task, lane);
         CullPipe p;
-        cull_prologue(p, geo, t, keys, n, lane);
-        const uint32_t nchunks = (n + 31u) >> 5;
-        for (uint32_t c = 0; c <= nchunks; ++c) {
+        cull_prologue(p, t, lane);
+        for (uint32_t c = 0;; ++c) {
             cull_park<true, DEPTH>(p, sm.q, sm.d0, t, sm.dd);
             const uint32_t avail = tail;
-            if (c < nchunks) tail += (uint32_t)cull_step(p, geo, t, keys, n, c, tail, lane);
+            const int nh = cull_step(p, geo, t, c, tail, lane);
+            if (nh >= 0) tail += (uint32_t)nh;
             while (avail - head >= (uint32_t)kBatch) {
                 bwd_batch<true, DEPTH, DET>(sm, px, t, vg, head, kBatch, kx, ky, lane, rbase);
                 head += kBatch;
             }
+            if (nh < 0) break;
         }
     }
     if (tail != head) {
@@ -723,47 +748,47 @@ int set_composite_option(int which, int value) {
 }
 
 template <int K, bool DEPTH, bool DET>
-static int launch_fwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
+static int launch_fwd(const Dims &d, const Inputs &in, const Geom &g, const uint2 *live,
                       const ImageState &img, float *out_color, const LossEpilogue &loss, const HitLists &hl,
                       cudaStream_t st) {
     const long long tasks = (long long)d.S * d.V * d.tiles * 8;
     constexpr int per_cta = kFwdWarps / K;
-    k_composite_fwd2<K, DEPTH, DET><<<(unsigned)((tasks + per_cta - 1) / per_cta), kFwdWarps * 32, 0, st>>>(d, g, in.bg, keys, img, out_color, loss, hl);
+    k_composite_fwd2<K, DEPTH, DET><<<(unsigned)((tasks + per_cta - 1) / per_cta), kFwdWarps * 32, 0, st>>>(d, g, in.bg, live, img, out_color, loss, hl);
     PS_LAUNCH_CHECK("k_composite_fwd2");
     return PS_OK;
 }
 
 template <int K, bool DET>
-static int launch_fwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
+static int launch_fwd(const Dims &d, const Inputs &in, const Geom &g, const uint2 *live,
                       const ImageState &img, float *out_color, const LossEpilogue &loss, const HitLists &hl,
                       cudaStream_t st) {
-    return d.depth_mode ? launch_fwd<K, true, DET>(d, in, g, keys, img, out_color, loss, hl, st)
-                        : launch_fwd<K, false, DET>(d, in, g, keys, img, out_color, loss, hl, st);
+    return d.depth_mode ? launch_fwd<K, true, DET>(d, in, g, live, img, out_color, loss, hl, st)
+                        : launch_fwd<K, false, DET>(d, in, g, live, img, out_color, loss, hl, st);
 }
 
 template <bool DET>
-static int launch_fwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
+static int launch_fwd(const Dims &d, const Inputs &in, const Geom &g, const uint2 *live,
                       const ImageState &img, float *out_color, const LossEpilogue &loss, const HitLists &hl,
                       cudaStream_t st) {
     switch (d.segK) {
-        case 4: return launch_fwd<4, DET>(d, in, g, keys, img, out_color, loss, hl, st);
-        case 2: return launch_fwd<2, DET>(d, in, g, keys, img, out_color, loss, hl, st);
-        default: return launch_fwd<1, DET>(d, in, g, keys, img, out_color, loss, hl, st);
+        case 4: return launch_fwd<4, DET>(d, in, g, live, img, out_color, loss, hl, st);
+        case 2: return launch_fwd<2, DET>(d, in, g, live, img, out_color, loss, hl, st);
+        default: return launch_fwd<1, DET>(d, in, g, live, img, out_color, loss, hl, st);
     }
 }
 
 int launch_composite_forward(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
-                             const ImageState &img, float *out_color, const LossEpilogue &loss, const HitLists &hl,
+                             const uint2 *live, const ImageState &img, float *out_color, const LossEpilogue &loss, const HitLists &hl,
                              float *loss_partials, cudaStream_t st) {
     if (composite_impl() == 1) {
         if (loss.target || !out_color) { set_error("the legacy compositor has no loss epilogue"); return PS_ERR_UNSUPPORTED; }
         return launch_composite_forward_v1(d, in, g, keys, img, out_color, st);
     }
-    if (!loss.target || !loss_partials) return launch_fwd<false>(d, in, g, keys, img, out_color, loss, hl, st);
+    if (!loss.target || !loss_partials) return launch_fwd<false>(d, in, g, live, img, out_color, loss, hl, st);
     // fixed-order loss epilogue: per-task partials, then k_loss_finish writes every slot of loss.sums
     LossEpilogue le = loss;
     le.sums = loss_partials;
-    int rc = launch_fwd<true>(d, in, g, keys, img, out_color, le, hl, st);
+    int rc = launch_fwd<true>(d, in, g, live, img, out_color, le, hl, st);
     if (rc) return rc;
     k_loss_finish<<<(unsigned)(d.S * d.V), kLossSlots, 0, st>>>(reinterpret_cast<const float2 *>(loss_partials),
                                                                 d.tiles * 8, loss.sums);
@@ -772,7 +797,7 @@ int launch_composite_forward(const Dims &d, const Inputs &in, const Geom &g, con
 }
 
 template <int K, bool DEPTH, bool DET>
-static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
+static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const uint2 *live,
                       const ImageState &img, const float *d_color, const float *d_depth, const ViewGrads &vg,
                       const LossEpilogue &loss, const HitLists &hl, cudaStream_t st) {
     const long long tasks = (long long)d.S * d.V * d.tiles * 8;
@@ -783,27 +808,27 @@ static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const unsi
         PS_CUDA_CHECK(cudaFuncSetAttribute(k_composite_bwd2<K, DEPTH, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     }
     k_composite_bwd2<K, DEPTH, DET><<<(unsigned)((tasks + per_cta - 1) / per_cta), kBwdWarps * 32, smem, st>>>(
-        d, g, in.bg, keys, img, d_color, d_depth, vg, loss, hl);
+        d, g, in.bg, live, img, d_color, d_depth, vg, loss, hl);
     PS_LAUNCH_CHECK("k_composite_bwd2");
     return PS_OK;
 }
 
 template <int K, bool DET>
-static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
+static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const uint2 *live,
                       const ImageState &img, const float *d_color, const float *d_depth, const ViewGrads &vg,
                       const LossEpilogue &loss, const HitLists &hl, cudaStream_t st) {
-    return d_depth ? launch_bwd<K, true, DET>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st)
-                   : launch_bwd<K, false, DET>(d, in, g, keys, img, d_color, nullptr, vg, loss, hl, st);
+    return d_depth ? launch_bwd<K, true, DET>(d, in, g, live, img, d_color, d_depth, vg, loss, hl, st)
+                   : launch_bwd<K, false, DET>(d, in, g, live, img, d_color, nullptr, vg, loss, hl, st);
 }
 
 template <bool DET>
-static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
+static int launch_bwd(const Dims &d, const Inputs &in, const Geom &g, const uint2 *live,
                       const ImageState &img, const float *d_color, const float *d_depth, const ViewGrads &vg,
                       const LossEpilogue &loss, const HitLists &hl, cudaStream_t st) {
     switch (d.segK) {
-        case 4: return launch_bwd<4, DET>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
-        case 2: return launch_bwd<2, DET>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
-        default: return launch_bwd<1, DET>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
+        case 4: return launch_bwd<4, DET>(d, in, g, live, img, d_color, d_depth, vg, loss, hl, st);
+        case 2: return launch_bwd<2, DET>(d, in, g, live, img, d_color, d_depth, vg, loss, hl, st);
+        default: return launch_bwd<1, DET>(d, in, g, live, img, d_color, d_depth, vg, loss, hl, st);
     }
 }
 
@@ -872,15 +897,15 @@ k_gather_block_records(Dims d, Geom geo, const unsigned long long *__restrict__ 
 }
 
 int launch_composite_backward(const Dims &d, const Inputs &in, const Geom &g, const unsigned long long *keys,
-                              const ImageState &img, const float *d_color, const float *d_depth, const ViewGrads &vg,
+                              const uint2 *live, const ImageState &img, const float *d_color, const float *d_depth, const ViewGrads &vg,
                               const ViewGrads *records, const LossEpilogue &loss, const HitLists &hl,
                               cudaStream_t st) {
     if (composite_impl() == 1) {
         if (!d_color) { set_error("the legacy compositor has no loss epilogue"); return PS_ERR_UNSUPPORTED; }
         return launch_composite_backward_v1(d, in, g, keys, img, d_color, vg, st);
     }
-    if (!records) return launch_bwd<false>(d, in, g, keys, img, d_color, d_depth, vg, loss, hl, st);
-    int rc = launch_bwd<true>(d, in, g, keys, img, d_color, d_depth, *records, loss, hl, st);
+    if (!records) return launch_bwd<false>(d, in, g, live, img, d_color, d_depth, vg, loss, hl, st);
+    int rc = launch_bwd<true>(d, in, g, live, img, d_color, d_depth, *records, loss, hl, st);
     if (rc) return rc;
     // the pair count lives on the device: launch for the worst case, surplus threads exit at once
     const long long lanes = (long long)d.S * d.V * d.P * 8;
