@@ -170,7 +170,13 @@ typedef struct ps_raster_layout {
  * Each output may be NULL (not written); the others are written in full, so they need no initialisation.  No float
  * atomics: in deterministic mode the camera gradients are the same bits on every run.
  * `workspace` (16-byte aligned, no initialisation) has ps_raster_camera_workspace_bytes: the preprocess backward
- * stores one partial sum per (warp of 32 Gaussians, view) there and a finish kernel adds them in a fixed order. */
+ * stores one partial sum per (warp of 32 Gaussians, view) there and a finish kernel adds them in a fixed order.
+ * Camera-only backward: with `camera` set, d_means, d_cov, d_opacities, d_sh and d_means2d may ALL be NULL.  The call
+ * then writes the camera gradients and nothing else (no Gaussian gradient is formed; the SH rows are read only for
+ * the campos term of on-screen Gaussians).  Its camera gradients are the full backward's (the same per-Gaussian terms
+ * summed in the same order; the compiler may round the campos term differently), and it takes the same scratch and
+ * workspace sizes and the same number of launches.  Some but not all of the four required Gaussian pointers NULL, or all five
+ * NULL without `camera`, is PS_ERR_INVALID_ARGUMENT before anything is enqueued. */
 typedef struct ps_raster_camera_grads {
     float *d_viewmatrix; /* [S*V, 16] column-major like viewmatrix                              */
     float *d_projmatrix; /* [S*V, 16]                                                           */
@@ -180,7 +186,7 @@ typedef struct ps_raster_camera_grads {
     size_t workspace_bytes;
 } ps_raster_camera_grads;
 
-typedef struct ps_raster_grads {
+typedef struct ps_raster_grads {   /* Gaussian outputs all NULL with `camera` set: camera-only backward (above) */
     float *d_means;     /* [S, P, 3]                                                           */
     float *d_cov;       /* same layout as cov                                                  */
     float *d_opacities; /* [S, P]                                                              */

@@ -457,7 +457,13 @@ static int raster_backward_impl(const ps_raster_desc *desc, const ps_raster_inpu
         return PS_ERR_INVALID_ARGUMENT;
     }
     const LossEpilogue le{d_color ? nullptr : target, nullptr, d_color ? nullptr : grad_scale};
-    if (!grads->d_means || !grads->d_cov || !grads->d_opacities || !grads->d_sh) {
+    // camera-only backward: every Gaussian-side output NULL, camera gradients requested
+    const bool camera_only = !grads->d_means && !grads->d_cov && !grads->d_opacities && !grads->d_sh && !grads->d_means2d;
+    if (camera_only && !grads->camera) {
+        set_error("every gradient pointer is NULL and no camera gradients are requested");
+        return PS_ERR_INVALID_ARGUMENT;
+    }
+    if (!camera_only && (!grads->d_means || !grads->d_cov || !grads->d_opacities || !grads->d_sh)) {
         set_error("a required gradient pointer is NULL");
         return PS_ERR_INVALID_ARGUMENT;
     }

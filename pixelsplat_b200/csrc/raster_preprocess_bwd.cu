@@ -24,6 +24,38 @@ __device__ __forceinline__ float *cam_row(float *ws, const Dims &d, int s, int v
     return ws + ((size_t)(s * d.V + v) * cam_rows_per_view(d.P) + (size_t)w) * kCamRowFloats;
 }
 
+// Word kCamEntries of a view's row 0 is k_camera_finish's arrival counter: every producer of a partial row stores all
+// kCamRowFloats words, the unused ones as 0, so the counter starts at 0 on every call.
+__device__ __forceinline__ unsigned *cam_counter(float *ws, const Dims &d, int vid) {
+    return reinterpret_cast<unsigned *>(ws + (size_t)vid * cam_rows_per_view(d.P) * kCamRowFloats) + kCamEntries;
+}
+
+// The warp's partial rows of view v: per scene its lanes belong to, the kCamEntries entries summed over those lanes in
+// a fixed xor-butterfly order, stored by lane 0 (with the unused words as 0).  A warp whose Gaussians span two scenes
+// (P not a multiple of 32) stores one row for each.
+__device__ __forceinline__ void store_cam_partials(const float (&cam)[kCamEntries], float *cam_ws, const Dims &d,
+                                                   int v, long long sg0, int rows, uint32_t scene, int lane) {
+    const int s_lo = (int)(sg0 / d.P), s_hi = (int)((sg0 + rows - 1) / d.P);
+    for (int s = s_lo; s <= s_hi; ++s) {
+        const bool mine = (int)scene == s;
+        float sum[kCamEntries];
+#pragma unroll
+        for (int k = 0; k < kCamEntries; ++k) {
+            float x = mine ? cam[k] : 0.0f;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+            sum[k] = x;
+        }
+        if (lane == 0) {
+            float *r = cam_row(cam_ws, d, s, v, sg0);
+#pragma unroll
+            for (int k = 0; k < kCamEntries; ++k) r[k] = sum[k];
+#pragma unroll
+            for (int k = kCamEntries; k < kCamRowFloats; ++k) r[k] = 0.0f;
+        }
+    }
+}
+
 // Each warp owns 32 consecutive (scene, Gaussian) indices of S*P and writes every element of their rows of every
 // output gradient, which the caller may hand over uninitialised: a Gaussian that is on screen in no view gets zeros,
 // and so does every Gaussian when the binning overflowed its capacity (the composite backward then did not run).  A
@@ -265,27 +297,7 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int
                 cam[2] += dz * mx0; cam[5] += dz * my0; cam[8] += dz * mz0; cam[11] += dz / sc;
             }
         }
-        if (CAM) {
-            // per (scene, view) sums over the warp's lanes in a fixed butterfly order; a warp whose Gaussians span
-            // two scenes (P not a multiple of 32) stores one row for each
-            const int s_lo = (int)(sg0 / d.P), s_hi = (int)((sg0 + rows - 1) / d.P);
-            for (int s = s_lo; s <= s_hi; ++s) {
-                const bool mine = (int)scene == s;
-                float sum[kCamEntries];
-#pragma unroll
-                for (int k = 0; k < kCamEntries; ++k) {
-                    float x = mine ? cam[k] : 0.0f;
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-                    sum[k] = x;
-                }
-                if (lane == 0) {
-                    float *r = cam_row(cam_ws, d, s, v, sg0);
-#pragma unroll
-                    for (int k = 0; k < kCamEntries; ++k) r[k] = sum[k];
-                }
-            }
-        }
+        if constexpr (CAM) store_cam_partials(cam, cam_ws, d, v, sg0, rows, scene, lane);
     }
 
     if (live) {
@@ -337,27 +349,197 @@ int launch_clear_pair_grads(const Dims &d, const Geom &g, const ViewGrads &vg, c
     return PS_OK;
 }
 
-// One CTA per flat view: sums the view's partial rows in ascending warp order -- 8 strided running sums, then a
-// fixed tree over the 8 -- and writes all 16 / 16 / 3 / 2 entries of the four camera gradients (the entries the
-// forward never reads get 0).  No atomics: the same rows give the same bits.
-constexpr int kCamFinishThreads = 8 * kCamRowFloats;
+// Camera-only backward (ps_raster_grads with every Gaussian gradient NULL): the 29 camera entries of k_preprocess_bwd's
+// CAM path, and nothing else.  One thread per (view, Gaussian) pair; a CTA covers kCamBwdThreads consecutive (scene,
+// Gaussian) indices of S*P for ONE view v (blockIdx.x = chunk * V + v: the V CTAs of a chunk run side by side and share
+// its SH rows in L2), so each warp stores exactly the partial rows k_preprocess_bwd<·, true> stores for (its 32
+// indices, v), summed in the same order, and the same k_camera_finish adds them.  It reads the scratch of the on-screen
+// pairs and the means, covariances and (for campos) SH rows of the on-screen lanes only; no Gaussian gradient is formed
+// or stored.  Walking the Gaussians, not the compact list of on-screen pairs (whose order changes from run to run),
+// keeps every float sum in a fixed order.
+constexpr int kCamBwdThreads = 128;
 
-__global__ void __launch_bounds__(kCamFinishThreads) k_camera_finish(Dims d, const float *__restrict__ ws,
-                                                                     ps_raster_camera_grads cg) {
-    __shared__ float part[8][kCamRowFloats];
-    const int vid = blockIdx.x, s = vid / d.V;
-    const int k = threadIdx.x % kCamRowFloats, grp = threadIdx.x / kCamRowFloats;
-    const long long w_lo = ((long long)s * d.P) / 32, w_hi = ((long long)(s + 1) * d.P - 1) / 32;
-    const int nrows = (int)(w_hi - w_lo + 1);
-    const float *rows = ws + (size_t)vid * cam_rows_per_view(d.P) * kCamRowFloats;
+template <bool DEPTH>
+__global__ void __launch_bounds__(kCamBwdThreads, 4)
+k_camera_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, int row_stride, float *cam_ws) {
+    extern __shared__ float s_sh[];    // [warps][32][row_stride] SH coefficients of the on-screen lanes
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int v = (int)(blockIdx.x % (unsigned)d.V);
+    const long long sp = (long long)d.S * d.P;
+    const long long sg0 = (long long)(blockIdx.x / (unsigned)d.V) * kCamBwdThreads + warp * 32;
+    if (sg0 >= sp) return;
+    const int rows = (int)min((long long)32, sp - sg0);
+    const bool live = lane < rows;
+    const uint32_t sgi = (uint32_t)(live ? sg0 + lane : sg0);
+    const uint32_t scene = sgi / (uint32_t)d.P, g = sgi - scene * (uint32_t)d.P;
+    const size_t sg = sgi;
+    const int vid = (int)scene * d.V + v;
+    const size_t vg = (size_t)vid * d.P + g;
+    const int M = d.M, sh_n = 3 * M;
+
+    const bool vis = live && *geo.n_instances <= d.capacity && geo.radii[vg] > 0;
+    const unsigned vis_lanes = __ballot_sync(0xffffffffu, vis);
+    float cam[kCamEntries];
+#pragma unroll
+    for (int k = 0; k < kCamEntries; ++k) cam[k] = 0.0f;
+    if (vis_lanes == 0u) {
+        store_cam_partials(cam, cam_ws, d, v, sg0, rows, scene, lane);
+        return;
+    }
+    float *wrows = s_sh + (size_t)warp * 32 * row_stride;
+    const float *row = wrows + lane * row_stride;
+    if (M > 0) gather_rows_async(in.sh, (unsigned long long)sg, vis_lanes, sh_n, wrows, row_stride, lane);
+
+    float mx0 = 0.0f, my0 = 0.0f, mz0 = 0.0f;
+    const float sc = in.scale ? in.scale[vid] : 1.0f;
+    if (vis) {
+        mx0 = in.means[3 * sg + 0]; my0 = in.means[3 * sg + 1]; mz0 = in.means[3 * sg + 2];
+        const float px = mx0 * sc, py = my0 * sc, pz = mz0 * sc;
+        const float *__restrict__ vm = in.view + 16 * vid;
+        const float *__restrict__ pm = in.proj + 16 * vid;
+        const float tanfovx = in.tanfov[2 * vid], tanfovy = in.tanfov[2 * vid + 1];
+        const float focal_x = (float)d.W / (2.0f * tanfovx), focal_y = (float)d.H / (2.0f * tanfovy);
+        float s6[6];
+        load_cov6(in.cov + sg * (d.cov_layout == PS_COV_TRIU6 ? 6 : 9), d.cov_layout, sc * sc, s6);
+        Cov2D cv;
+        compute_cov2d(px, py, pz, s6, vm, focal_x, focal_y, tanfovx, tanfovy, cv);
+        const float2 g2 = vgr.d_mean2d[vg];
+        const float4 gc = vgr.d_conic[vg];
+
+        // the CAM path of k_preprocess_bwd, term for term
+        const float a = cv.a, b = cv.b, c = cv.c;
+        const float denom = a * c - b * b;
+        const float denom2inv = 1.0f / (denom * denom + 0.0000001f);
+        float dL_da = 0.0f, dL_db = 0.0f, dL_dc = 0.0f;
+        const float *m0 = cv.m0, *m1 = cv.m1;
+        if (denom2inv != 0.0f) {
+            dL_da = denom2inv * (-c * c * gc.x + 2.0f * b * c * gc.y + (denom - a * c) * gc.z);
+            dL_dc = denom2inv * (-a * a * gc.z + 2.0f * a * b * gc.y + (denom - a * c) * gc.x);
+            dL_db = denom2inv * 2.0f * (b * c * gc.x - (denom + 2.0f * b * b) * gc.y + a * b * gc.z);
+        }
+        const float S[3][3] = {{s6[0], s6[1], s6[2]}, {s6[1], s6[3], s6[4]}, {s6[2], s6[4], s6[5]}};
+        float dM0[3], dM1[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            const float sm0 = m0[0] * S[k][0] + m0[1] * S[k][1] + m0[2] * S[k][2];
+            const float sm1 = m1[0] * S[k][0] + m1[1] * S[k][1] + m1[2] * S[k][2];
+            dM0[k] = 2.0f * sm0 * dL_da + sm1 * dL_db;
+            dM1[k] = 2.0f * sm1 * dL_dc + sm0 * dL_db;
+        }
+        const float dJ00 = vm[0] * dM0[0] + vm[4] * dM0[1] + vm[8] * dM0[2];
+        const float dJ02 = vm[2] * dM0[0] + vm[6] * dM0[1] + vm[10] * dM0[2];
+        const float dJ11 = vm[1] * dM1[0] + vm[5] * dM1[1] + vm[9] * dM1[2];
+        const float dJ12 = vm[2] * dM1[0] + vm[6] * dM1[1] + vm[10] * dM1[2];
+        const float tz = 1.0f / cv.tz, tz2 = tz * tz, tz3 = tz2 * tz;
+        const float dL_dtx = cv.clamp_x ? 0.0f : -focal_x * tz2 * dJ02;
+        const float dL_dty = cv.clamp_y ? 0.0f : -focal_y * tz2 * dJ12;
+        const float dL_dtz = -focal_x * tz2 * dJ00 - focal_y * tz2 * dJ11 +
+                             (2.0f * focal_x * cv.ctx) * tz3 * dJ02 + (2.0f * focal_y * cv.cty) * tz3 * dJ12;
+        const float hx = pm[0] * px + pm[4] * py + pm[8] * pz + pm[12];
+        const float hy = pm[1] * px + pm[5] * py + pm[9] * pz + pm[13];
+        const float hw = pm[3] * px + pm[7] * py + pm[11] * pz + pm[15];
+        const float m_w = 1.0f / (hw + 0.0000001f);
+        const float mul1 = hx * m_w * m_w, mul2 = hy * m_w * m_w;
+        const float j00 = focal_x * tz, j02 = -focal_x * cv.ctx * tz2;
+        const float j11 = focal_y * tz, j12 = -focal_y * cv.cty * tz2;
+        const float p[3] = {px, py, pz};
+        const float dhx = g2.x * m_w, dhy = g2.y * m_w, dhw = -(mul1 * g2.x + mul2 * g2.y);
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            cam[3 * j + 0] = dM0[j] * j00 + dL_dtx * p[j];
+            cam[3 * j + 1] = dM1[j] * j11 + dL_dty * p[j];
+            cam[3 * j + 2] = dM0[j] * j02 + dM1[j] * j12 + dL_dtz * p[j];
+            cam[12 + 3 * j + 0] = dhx * p[j];
+            cam[12 + 3 * j + 1] = dhy * p[j];
+            cam[12 + 3 * j + 2] = dhw * p[j];
+        }
+        cam[9] = dL_dtx; cam[10] = dL_dty; cam[11] = dL_dtz;
+        cam[21] = dhx; cam[22] = dhy; cam[23] = dhw;
+        cam[27] = (dJ00 * tz - dJ02 * cv.ctx * tz2) * (-focal_x / tanfovx);
+        cam[28] = (dJ11 * tz - dJ12 * cv.cty * tz2) * (-focal_y / tanfovy);
+    }
+    if (M > 0) gather_rows_wait();         // warp-uniform
+    if (M > 0 && vis) {
+        // campos: minus the gradient of the view direction p - campos through the SH evaluation
+        const float px = mx0 * sc, py = my0 * sc, pz = mz0 * sc;
+        const float4 gcol = vgr.d_color[vg];
+        const float cx = in.campos[3 * vid], cy = in.campos[3 * vid + 1], cz = in.campos[3 * vid + 2];
+        const float ddx = px - cx, ddy = py - cy, ddz = pz - cz;
+        const float len2 = ddx * ddx + ddy * ddy + ddz * ddz;
+        const float len = sqrtf(len2);
+        const float x = ddx / len, y = ddy / len, z = ddz / len;
+        const uint8_t cl = geo.clamped[vg];
+        const float dl[3] = {(cl & 1) ? 0.0f : gcol.x, (cl & 2) ? 0.0f : gcol.y, (cl & 4) ? 0.0f : gcol.z};
+        float dLda = 0.0f, dLdb = 0.0f, dLdc = 0.0f;
+        const float3 sa = sh_arg(d.sh_basis, x, y, z);
+        const uint32_t flip = sh_flip_mask(d.sh_basis);
+        const int layout = d.sh_layout;
+        sh_for_each(d.deg, sa.x, sa.y, sa.z, [&](int k, float Y, float Ya, float Yb, float Yc) {
+#pragma unroll
+            for (int ch = 0; ch < 3; ++ch) {
+                const float cd = row[sh_index(layout, M, k, ch)] * sh_sign(flip, k, dl[ch]);
+                dLda += Ya * cd; dLdb += Yb * cd; dLdc += Yc * cd;
+            }
+        });
+        const float3 dLd = sh_grad_unpermute(d.sh_basis, dLda, dLdb, dLdc);
+        const float dLdx = dLd.x, dLdy = dLd.y, dLdz = dLd.z;
+        const float inv3 = 1.0f / (len2 * len);
+        const float xx = __fmul_rn(ddx, ddx), yy = __fmul_rn(ddy, ddy), zz = __fmul_rn(ddz, ddz);
+        const float xy = __fmul_rn(ddx, ddy), xz = __fmul_rn(ddx, ddz), yz = __fmul_rn(ddy, ddz);
+        const float ex = __fadd_rn(__fadd_rn(__fmul_rn(__fsub_rn(len2, xx), dLdx), -__fmul_rn(xy, dLdy)), -__fmul_rn(xz, dLdz));
+        const float ey = __fadd_rn(__fadd_rn(-__fmul_rn(xy, dLdx), __fmul_rn(__fsub_rn(len2, yy), dLdy)), -__fmul_rn(yz, dLdz));
+        const float ez = __fadd_rn(__fadd_rn(-__fmul_rn(xz, dLdx), -__fmul_rn(yz, dLdy)), __fmul_rn(__fsub_rn(len2, zz), dLdz));
+        cam[24] = -__fmul_rn(ex, inv3); cam[25] = -__fmul_rn(ey, inv3); cam[26] = -__fmul_rn(ez, inv3);
+    }
+    if (DEPTH && vis) {   // z = (vm[2], vm[6], vm[10]) . mean + vm[14] / sc
+        const float dz = vgr.d_color[vg].w * depth_value_grad(d.depth_mode, geo.depth[vg], in.scale, in.near_far, vid);
+        cam[2] += dz * mx0; cam[5] += dz * my0; cam[8] += dz * mz0; cam[11] += dz / sc;
+    }
+    store_cam_partials(cam, cam_ws, d, v, sg0, rows, scene, lane);
+}
+
+// Sums the partial rows of every flat view in a fixed order over many CTAs (grid: kCamFinishRows-row chunks x views).
+// CTA c of a view adds rows [c R, (c + 1) R) -- 8 strided running sums, then a fixed tree over the 8 -- and, when the
+// view has more than one chunk, stores its sum over row c R (which only it has read) and counts itself in on the
+// view's counter (cam_counter).  The CTA that arrives last adds the chunk sums in chunk order, the same way.  Which
+// CTA that is does not change the order of any float sum, so the same rows give the same bits.  Writes all 16 / 16 /
+// 3 / 2 entries of the four camera gradients (the entries the forward never reads get 0).
+constexpr int kCamFinishThreads = 8 * kCamRowFloats;
+constexpr int kCamFinishRows = 256;
+
+__device__ __forceinline__ void cam_finish_sum(const float *rows, size_t step, int n, int k, int grp,
+                                               float (&part)[8][kCamRowFloats]) {
     float acc = 0.0f;
-    for (int r = grp; r < nrows; r += 8) acc += rows[(size_t)r * kCamRowFloats + k];
+    for (int r = grp; r < n; r += 8) acc += __ldcg(rows + (size_t)r * step + k);
     part[grp][k] = acc;
     __syncthreads();
 #pragma unroll
     for (int stride = 4; stride > 0; stride >>= 1) {
         if (grp < stride) part[grp][k] += part[grp + stride][k];
         __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(kCamFinishThreads) k_camera_finish(Dims d, float *__restrict__ ws,
+                                                                     ps_raster_camera_grads cg) {
+    __shared__ float part[8][kCamRowFloats];
+    __shared__ bool last;
+    const int vid = blockIdx.y, s = vid / d.V, chunk = blockIdx.x, chunks = gridDim.x;
+    const int k = threadIdx.x % kCamRowFloats, grp = threadIdx.x / kCamRowFloats;
+    const long long w_lo = ((long long)s * d.P) / 32, w_hi = ((long long)(s + 1) * d.P - 1) / 32;
+    const int nrows = (int)(w_hi - w_lo + 1);
+    float *rows = ws + (size_t)vid * cam_rows_per_view(d.P) * kCamRowFloats;
+    float *mine = rows + (size_t)chunk * kCamFinishRows * kCamRowFloats;
+    cam_finish_sum(mine, kCamRowFloats, min(kCamFinishRows, nrows - chunk * kCamFinishRows), k, grp, part);
+    if (chunks > 1) {
+        if (threadIdx.x < kCamEntries) mine[threadIdx.x] = part[0][threadIdx.x];   // word kCamEntries: the counter
+        __threadfence();
+        __syncthreads();
+        if (threadIdx.x == 0) last = atomicAdd(cam_counter(ws, d, vid), 1u) == (unsigned)chunks - 1u;
+        __syncthreads();
+        if (!last) return;
+        __threadfence();
+        cam_finish_sum(rows, (size_t)kCamFinishRows * kCamRowFloats, chunks, k, grp, part);
     }
     const int t = threadIdx.x;
     if (t < 16) {
@@ -391,15 +573,25 @@ int launch_preprocess_backward(const Dims &d, const Inputs &in, const Geom &g, c
     const GaussGrads out{grads.d_means, grads.d_cov, grads.d_opacities, grads.d_sh, grads.d_means2d};
     const ps_raster_camera_grads *cg = grads.camera;
     float *ws = cg ? static_cast<float *>(cg->workspace) : nullptr;
-    int rc;
-    if (d.depth_mode)
+    int rc = PS_OK;
+    if (!grads.d_means) {               // camera-only backward (the caller checked that cg is set)
+        const unsigned cam_blocks = (unsigned)((sp + kCamBwdThreads - 1) / kCamBwdThreads) * (unsigned)d.V;
+        const size_t cam_smem = d.M > 0 ? sizeof(float) * kCamBwdThreads * row_stride : 0;
+        if (d.depth_mode)
+            k_camera_bwd<true><<<cam_blocks, kCamBwdThreads, cam_smem, st>>>(d, in, g, vg, row_stride, ws);
+        else
+            k_camera_bwd<false><<<cam_blocks, kCamBwdThreads, cam_smem, st>>>(d, in, g, vg, row_stride, ws);
+        PS_LAUNCH_CHECK("k_camera_bwd");
+    } else if (d.depth_mode)
         rc = cg ? launch_preprocess_bwd_kernel<true, true>(blocks, smem, d, in, g, vg, out, row_stride, ws, st)
                 : launch_preprocess_bwd_kernel<true, false>(blocks, smem, d, in, g, vg, out, row_stride, ws, st);
     else
         rc = cg ? launch_preprocess_bwd_kernel<false, true>(blocks, smem, d, in, g, vg, out, row_stride, ws, st)
                 : launch_preprocess_bwd_kernel<false, false>(blocks, smem, d, in, g, vg, out, row_stride, ws, st);
     if (rc || !cg) return rc;
-    k_camera_finish<<<(unsigned)(d.S * d.V), kCamFinishThreads, 0, st>>>(d, ws, *cg);
+    const dim3 finish_grid((unsigned)((cam_rows_per_view(d.P) + kCamFinishRows - 1) / kCamFinishRows),
+                           (unsigned)(d.S * d.V));
+    k_camera_finish<<<finish_grid, kCamFinishThreads, 0, st>>>(d, ws, *cg);
     PS_LAUNCH_CHECK("k_camera_finish");
     return PS_OK;
 }

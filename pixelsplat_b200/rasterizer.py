@@ -328,8 +328,10 @@ class _Rasterize(torch.autograd.Function):
     (ps_raster_backward without a target, ps_raster_backward_loss with one).
     The four camera arrays (viewmatrix, projmatrix, campos, tanfov; the same tensors as in `cams`) are inputs of the
     Function: when one of them requires grad the backward also returns the camera gradients (ps_raster_camera_grads,
-    include/pixelsplat_b200.h); otherwise its launches and bits are those of the Gaussian-only backward.  background,
-    scene_scale and near_far are not differentiated."""
+    include/pixelsplat_b200.h); otherwise its launches and bits are those of the Gaussian-only backward.  When a
+    camera array requires grad and none of means, cov, opac, sh and means2d does, the backward is the camera-only one:
+    no Gaussian gradient is allocated or formed, and None is returned for each.  background, scene_scale and near_far
+    are not differentiated."""
 
     @staticmethod
     def forward(ctx, means, cov, opac, sh, means2d, target, viewmatrix, projmatrix, campos, tanfov, cams,
@@ -370,13 +372,16 @@ class _Rasterize(torch.autograd.Function):
                      else (2.0 * d_sse).to(torch.float32).contiguous())
         _sync_deterministic()               # before the sizes: the mode changes the backward scratch
         scratch = torch.empty(_lib.sizes(desc).backward_bytes, dtype=torch.uint8, device=dev)
-        d_means, d_cov = torch.empty_like(means), torch.empty_like(cov)
-        d_opac, d_sh = torch.empty_like(opac), torch.empty_like(sh)
-        d_m2d = (torch.empty((VT, desc.n_gaussians, 3), dtype=torch.float32, device=dev)
-                 if ctx.needs_input_grad[4] else None)
+        if any(ctx.needs_input_grad[:5]) or not any(ctx.needs_input_grad[6:10]):
+            d_means, d_cov = torch.empty_like(means), torch.empty_like(cov)
+            d_opac, d_sh = torch.empty_like(opac), torch.empty_like(sh)
+            d_m2d = (torch.empty((VT, desc.n_gaussians, 3), dtype=torch.float32, device=dev)
+                     if ctx.needs_input_grad[4] else None)
+        else:
+            # frozen Gaussians (test-time pose alignment): the camera-only backward forms no Gaussian gradient
+            d_means = d_cov = d_opac = d_sh = d_m2d = None
         inputs = _raster_inputs(means, cov, opac, sh, ctx.cams)
-        grads = _lib.RasterGrads(d_means.data_ptr(), d_cov.data_ptr(), d_opac.data_ptr(), d_sh.data_ptr(),
-                                 d_m2d.data_ptr() if d_m2d is not None else None)
+        grads = _lib.RasterGrads(*[None if t is None else t.data_ptr() for t in (d_means, d_cov, d_opac, d_sh, d_m2d)])
         d_cams = [None] * 4                 # viewmatrix, projmatrix, campos, tanfov
         if any(ctx.needs_input_grad[6:10]):
             widths = (16, 16, 3, 2)
