@@ -509,6 +509,57 @@ PS_API int ps_ssim_backward(int32_t n_planes, int32_t H, int32_t W, const float 
                             const float *d_mean, float *d_x /* or NULL */, float *d_y, void *workspace,
                             size_t workspace_bytes, void *stream);
 
+/* ---- LPIPS distance head (csrc/lpips.cu) ---------------------------------------------------------------------
+ * The head of the lpips package's LPIPS(net="vgg") (version 0.1) on up to five feature layers.  For layer l with
+ * features x0, x1 [N, C, H, W] (contiguous NCHW) and the 1x1 `lin` weight w [C] (no bias), per image n and pixel p:
+ *   f^ = f / (sqrt(sum_c f_c^2) + 1e-10)   (each side),   u = f^0 - f^1,
+ *   d_l[n] = (1 / (H W)) sum_p sum_c w_c m_{l,n,c,p} u_c^2,        out[n] = sum_l d_l[n].
+ * u is formed from the normalised features directly (never from expanded moment sums), so identical inputs give
+ * exactly 0 and a zero gradient.
+ * Dropout: m = 1 when dropout_seed is NULL (eval).  Otherwise m = 2 * keep with keep a fair bit, the top bit of
+ *   h = mix(key_l + (i + 1) * G),  key_l = mix(seed + (l + 1) * G),  G = 0x9E3779B97F4A7C15,
+ * where seed is *dropout_seed read as uint64, i = ((n * C + c) * H + y) * W + x the flat index in the layer, all
+ * arithmetic mod 2^64, and mix the splitmix64 finaliser: z ^= z >> 30; z *= 0xBF58476D1CE4E5B9; z ^= z >> 27;
+ * z *= 0x94D049BB133111EB; z ^= z >> 31.  The seed is read on the device, so a call can be captured in a graph with
+ * the seed drawn inside the capture; the backward recomputes the mask from the same seed.
+ * No float atomics: forward and backward give the same bits on every run.  No call synchronises the host.
+ * Every entry point rejects n_layers outside [1, 5], N < 1, C outside [1, 8192], H or W < 1, a layer with more
+ * than 2^31 - 1 elements, NULL required pointers and a short workspace with PS_ERR_INVALID_ARGUMENT before anything is
+ * enqueued. */
+#define PS_LPIPS_MAX_LAYERS 5
+
+typedef struct {
+    const float *x0, *x1;   /* [N, C, H, W] */
+    const float *weight;    /* [C] */
+    int32_t C, H, W;
+} ps_lpips_layer;
+
+typedef struct {
+    int32_t n_layers, N;
+    ps_lpips_layer layers[PS_LPIPS_MAX_LAYERS];
+    const int64_t *dropout_seed;   /* device pointer to one int64, or NULL: eval mode (no dropout) */
+} ps_lpips_desc;
+
+/* Per layer, dL/dx0 and dL/dx1 ([N, C, H, W], fully written: no zero-fill needed).  Either may be NULL, not both. */
+typedef struct {
+    float *d_x0[PS_LPIPS_MAX_LAYERS];
+    float *d_x1[PS_LPIPS_MAX_LAYERS];
+} ps_lpips_grads;
+
+PS_API int ps_lpips_workspace_bytes(const ps_lpips_desc *desc, size_t *out);
+
+/* out [N] = sum over layers of d_l.  The workspace (ps_lpips_workspace_bytes) holds per-tile partial sums, which a
+ * second kernel adds in a fixed order. */
+PS_API int ps_lpips_forward(const ps_lpips_desc *desc, float *out, void *workspace, size_t workspace_bytes,
+                            void *stream);
+
+/* Given d_out [N] = dL/dout, writes the gradients of `grads`.  With z_c = 2 k_c u_c, k = w m d_out / (H W) and n the
+ * norm of the side's column: d f_j = +-[z_j / (n + eps) - f_j (sum_c z_c f_c) / (n (n + eps)^2)] (+ for x0, - for
+ * x1).  At an all-zero column (n = 0) this is the analytic limit +-z_j / eps (the second term is 0), where autograd
+ * of the formula gives NaN (sqrt's derivative at 0).  No workspace. */
+PS_API int ps_lpips_backward(const ps_lpips_desc *desc, const float *d_out, const ps_lpips_grads *grads,
+                             void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -87,6 +87,21 @@ class RasterLoss(ctypes.Structure):
 
 
 LOSS_SLOTS = 64
+LPIPS_MAX_LAYERS = 5
+
+
+class LpipsLayer(ctypes.Structure):
+    _fields_ = [("x0", ctypes.c_void_p), ("x1", ctypes.c_void_p), ("weight", ctypes.c_void_p),
+                ("C", ctypes.c_int32), ("H", ctypes.c_int32), ("W", ctypes.c_int32)]
+
+
+class LpipsDesc(ctypes.Structure):
+    _fields_ = [("n_layers", ctypes.c_int32), ("N", ctypes.c_int32), ("layers", LpipsLayer * LPIPS_MAX_LAYERS),
+                ("dropout_seed", ctypes.c_void_p)]
+
+
+class LpipsGrads(ctypes.Structure):
+    _fields_ = [("d_x0", ctypes.c_void_p * LPIPS_MAX_LAYERS), ("d_x1", ctypes.c_void_p * LPIPS_MAX_LAYERS)]
 
 
 class RasterCameraGrads(ctypes.Structure):
@@ -108,7 +123,8 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_self_attention_forward_stats", "ps_self_attention_backward", "ps_get_option",
            "ps_raster_backward_depth", "ps_ssim_workspace_bytes", "ps_ssim_forward", "ps_ssim_backward",
            "ps_epipolar_attention_backward_workspace_bytes", "ps_epipolar_attention_backward_deterministic",
-           "ps_raster_camera_workspace_bytes", "ps_camera_setup_backward")
+           "ps_raster_camera_workspace_bytes", "ps_camera_setup_backward", "ps_lpips_workspace_bytes",
+           "ps_lpips_forward", "ps_lpips_backward")
 
 
 class NativeLibraryMissing(ImportError):
@@ -189,6 +205,12 @@ def _load() -> ctypes.CDLL:
     lib.ps_ssim_forward.restype = ctypes.c_int
     lib.ps_ssim_backward.argtypes = [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 6 + [ctypes.c_size_t, ctypes.c_void_p]
     lib.ps_ssim_backward.restype = ctypes.c_int
+    lib.ps_lpips_workspace_bytes.argtypes = [P(LpipsDesc), P(ctypes.c_size_t)]
+    lib.ps_lpips_workspace_bytes.restype = ctypes.c_int
+    lib.ps_lpips_forward.argtypes = [P(LpipsDesc), ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
+    lib.ps_lpips_forward.restype = ctypes.c_int
+    lib.ps_lpips_backward.argtypes = [P(LpipsDesc), ctypes.c_void_p, P(LpipsGrads), ctypes.c_void_p]
+    lib.ps_lpips_backward.restype = ctypes.c_int
     for f in ("ps_raster_sizes_query", "ps_raster_layout_query", "ps_raster_forward", "ps_raster_backward"):
         getattr(lib, f).restype = ctypes.c_int
     return lib

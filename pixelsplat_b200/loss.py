@@ -16,6 +16,10 @@ sm_90a kernels of csrc/ssim.cu (`ps_ssim_forward` / `ps_ssim_backward`) instead 
 loop over images.  `ssim` is differentiable in both images (1 - ssim is the usual partner of the photometric loss);
 `compute_ssim` is the no-grad metric.
 
+`LossLpips` / `LossLpipsCfg` / `LossLpipsCfgWrapper` and `compute_lpips` are the drop-ins for
+/root/reference/src/loss/loss_lpips.py and evaluation/metrics.py:22-33, on `pixelsplat_b200.lpips.Lpips` (VGG16 trunk
+in torch, the distance head fused in csrc/lpips.cu).
+
 `LossDepth` / `LossDepthCfg` / `LossDepthCfgWrapper` are the drop-in for /root/reference/src/loss/loss_depth.py: an
 edge-aware smoothness penalty on the rendered depth map (`DecoderOutput.depth`), which the fused depth channel
 (`DecoderSplattingCUDA.forward(depth_mode=...)`) provides.
@@ -146,6 +150,72 @@ def ssim(ground_truth: Tensor, predicted: Tensor) -> Tensor:
 def compute_ssim(ground_truth: Tensor, predicted: Tensor) -> Tensor:
     """[batch, c, h, w] x 2 -> [batch] (metrics.py:36-52), on the prediction's device, without a host copy."""
     return ssim(ground_truth, predicted).to(predicted.dtype)
+
+
+@dataclass
+class LossLpipsCfg:
+    weight: float
+    apply_after_step: int
+
+
+@dataclass
+class LossLpipsCfgWrapper:
+    lpips: LossLpipsCfg
+
+
+def convert_to_buffer(module: nn.Module, persistent: bool = True) -> None:
+    """Re-registers every parameter and buffer of `module` and its children as a buffer of the given persistence
+    (what the reference's misc/nn_module_tools.py does to its LPIPS network)."""
+    for child in module.children():
+        convert_to_buffer(child, persistent)
+    for name, value in (*module.named_parameters(recurse=False), *module.named_buffers(recurse=False)):
+        value = value.detach().clone()
+        delattr(module, name)
+        module.register_buffer(name, value, persistent=persistent)
+
+
+class LossLpips(nn.Module):
+    """Same constructor and forward signature as the reference's LossLpips: weight * LPIPS(prediction.color,
+    batch["target"]["image"], normalize=True).mean() over the (b v) images, or a float32 zero on the image's device
+    before `apply_after_step`.  The LPIPS network's tensors are non-persistent buffers, so the loss adds no
+    state-dict keys (a checkpoint never held them).  `lpips` defaults to `Lpips.from_files()` (the weights already
+    on disk; nothing is downloaded).  In train mode the head applies the package's dropout, as the reference's
+    does when its LightningModule is in train mode."""
+
+    def __init__(self, cfg: LossLpipsCfgWrapper, lpips=None) -> None:
+        super().__init__()
+        from .lpips import Lpips
+        (field,) = fields(type(cfg))
+        self.cfg = getattr(cfg, field.name)
+        self.name = field.name
+        self.lpips = lpips if lpips is not None else Lpips.from_files()
+        convert_to_buffer(self.lpips, persistent=False)
+
+    def forward(self, prediction, batch, gaussians=None, global_step: int = 0) -> Tensor:
+        image = batch["target"]["image"]
+        if global_step < self.cfg.apply_after_step:
+            return torch.tensor(0, dtype=torch.float32, device=image.device)
+        loss = self.lpips(prediction.color.flatten(0, 1), image.flatten(0, 1), normalize=True)
+        return self.cfg.weight * loss.mean()
+
+
+_LPIPS_BY_DEVICE: dict = {}
+
+
+def get_lpips(device) -> nn.Module:
+    """One eval-mode `Lpips.from_files()` per device, created on first use (metrics.py's get_lpips)."""
+    from .lpips import Lpips
+    device = torch.device(device)
+    if device not in _LPIPS_BY_DEVICE:
+        _LPIPS_BY_DEVICE[device] = Lpips.from_files().to(device)
+    return _LPIPS_BY_DEVICE[device].eval()
+
+
+@torch.no_grad()
+def compute_lpips(ground_truth: Tensor, predicted: Tensor) -> Tensor:
+    """[batch, 3, h, w] x 2 in [0, 1] -> [batch] (metrics.py:22-33), always in eval mode (no dropout)."""
+    value = get_lpips(predicted.device).forward(ground_truth, predicted, normalize=True)
+    return value[:, 0, 0, 0].to(predicted.dtype)
 
 
 @dataclass

@@ -49,6 +49,9 @@ def main():
                     help="add LossDepth (re10k_depth_loss: weight 0.25, sigma 12, second derivative) on the fused depth")
     ap.add_argument("--two-pass-depth", action="store_true",
                     help="with --depth-loss: render the depth as a second pass (render_depth) instead (A/B)")
+    ap.add_argument("--lpips", action="store_true",
+                    help="add LossLpips (weight 0.05, active, dropout on) on the rendered image; the MSE is then "
+                         "taken in torch on that image (the fused epilogue returns no colour to differentiate)")
     ap.add_argument("--deterministic", action="store_true",
                     help="torch.use_deterministic_algorithms(True): fixed-order encoder and rasterizer gradients")
     args = ap.parse_args()
@@ -90,6 +93,11 @@ def main():
     context = dict(image=images, extrinsics=ctx_e, intrinsics=ctx_k, near=near_c, far=far_c)
     loss_depth = LossDepth(LossDepthCfgWrapper(LossDepthCfg(0.25, 12.0, True)))
     depth_batch = {"target": {"near": near_t, "far": far_t, "image": target}}
+    loss_lpips = None
+    if args.lpips:   # torch's default init (seeded above): the time does not depend on the weights
+        from pixelsplat_b200.loss import LossLpips, LossLpipsCfg, LossLpipsCfgWrapper
+        from pixelsplat_b200.lpips import Lpips
+        loss_lpips = LossLpips(LossLpipsCfgWrapper(LossLpipsCfg(0.05, 0)), lpips=Lpips()).to(dev).train()
     phases = ["encoder", "head", "render", "backward", "allreduce", "optimizer"]
     acc = {p: 0.0 for p in phases}
 
@@ -106,9 +114,11 @@ def main():
         f, _ = enc(feats, ctx_e, ctx_k, near_c, far_c); mark(1)
         gs = head(f, context, global_step=0); mark(2)
         fused_depth = "depth" if args.depth_loss and not args.two_pass_depth else None
-        if args.unfused_loss:
+        if args.unfused_loss or args.lpips:
             out = dec(gs, tgt_e, tgt_k, near_t, far_t, (HW, HW), depth_mode=fused_depth)
             loss = (out.color - target).square().mean()
+            if loss_lpips is not None:
+                loss = loss + loss_lpips(out, depth_batch, None, 0)
         else:   # LossMse from the compositor's epilogue: no image tensor, no dL/dC tensor (row f-4)
             out, sse, _ = dec.forward_mse(gs, tgt_e, tgt_k, near_t, far_t, (HW, HW), target, want_color=False,
                                           depth_mode=fused_depth)
@@ -180,7 +190,9 @@ def main():
             "scenes_per_s": world * B * args.steps / sec, "views_per_s": world * B * T * args.steps / sec,
             "ms_per_step": 1e3 * sec / args.steps,
             "phase_ms": ({p: acc[p] / len(timeline) for p in phases} if timeline else None),
-            "launch": launch, "loss_path": "torch MSE on the rendered image" if args.unfused_loss else "fused compositor epilogue",
+            "launch": launch, "loss_path": ("torch MSE on the rendered image" if args.unfused_loss or args.lpips
+                                            else "fused compositor epilogue"),
+            "lpips": "LossLpips weight 0.05, train mode (dropout), fused head" if args.lpips else None,
             "depth_loss": None if not args.depth_loss else ("two-pass render_depth" if args.two_pass_depth
                                                             else "fused depth channel"),
             "allreduce": ("after backward, torch.cat buckets (round-1 path)" if reducer is None else
