@@ -121,8 +121,8 @@ __device__ __forceinline__ void sh_rotate_row(float *row, const float *sD, int n
 }
 
 // Coalesced copy of `rows` consecutive n-float rows into padded shared rows, four independent 32-wide
-// loads in flight per lane (stage_sh_rows issues them one at a time; this kernel is latency-bound at
-// ~20 warps per SM, so memory-level parallelism per warp is what moves it).
+// loads in flight per lane rather than one at a time (this kernel is latency-bound at ~20 warps per SM,
+// so memory-level parallelism per warp is what moves it).
 __device__ __forceinline__ void stage_rows_x4(const float *__restrict__ src, float *dst, int rows, int n,
                                               int row_stride, int lane) {
     const int total = rows * n;

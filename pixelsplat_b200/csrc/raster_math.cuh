@@ -142,33 +142,8 @@ __device__ __forceinline__ float3 sh_grad_unpermute(int basis, float da, float d
     return basis == PS_SH_BASIS_E3NN ? make_float3(db, dc, da) : make_float3(da, db, dc);
 }
 
-// Cooperative, coalesced copy of one warp's 32 consecutive SH rows (3M floats each) from global
-// to shared memory (row stride padded to an odd word count -> the per-lane row reads that follow
-// are bank-conflict free).  A per-lane `__ldg(sh + k)` walk instead costs 32 L1 wavefronts per
-// load instruction (300-byte lane stride): 2400 wavefronts per warp vs ~150 this way.
-__device__ __forceinline__ void stage_sh_rows(const float *__restrict__ src, float *dst, int rows, int sh_n,
-                                              int row_stride, int lane) {
-    const int total = rows * sh_n;
-    const bool vec_ok = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0;
-    if (row_stride == sh_n) {
-        // odd row length (M = 1, 9, 25): rows are already conflict-free, the copy is linear
-        const int nvec = vec_ok ? total >> 2 : 0;
-        for (int i = lane; i < nvec; i += 32)
-            reinterpret_cast<float4 *>(dst)[i] = __ldg(reinterpret_cast<const float4 *>(src) + i);
-        for (int e = 4 * nvec + lane; e < total; e += 32) dst[e] = __ldg(src + e);
-        return;
-    }
-    // even row length: pad each row by one word; (row, column) advance incrementally (no division)
-    int e = lane, r = e / sh_n, c = e - r * sh_n;
-    const int step_r = 32 / sh_n, step_c = 32 - step_r * sh_n;
-    for (; e < total; e += 32) {
-        dst[r * row_stride + c] = __ldg(src + e);
-        r += step_r; c += step_c;
-        if (c >= sh_n) { c -= sh_n; ++r; }
-    }
-}
-
-// Inverse of stage_sh_rows: one contiguous, coalesced run of rows*sh_n floats back to global.
+// One warp's `rows` staged rows of sh_n floats (shared memory, row stride padded to an odd word count so that
+// per-lane row accesses are bank-conflict free) back to global as one contiguous, coalesced run of rows*sh_n floats.
 __device__ __forceinline__ void unstage_sh_rows(const float *src, float *__restrict__ dst, int rows, int sh_n,
                                                 int row_stride, int lane) {
     const int total = rows * sh_n;
@@ -189,48 +164,11 @@ __device__ __forceinline__ void unstage_sh_rows(const float *src, float *__restr
     }
 }
 
-// Gather 32 scattered rows (one per lane's Gaussian, `row_of_lane` = flat row index held by each
-// lane) of sh_n floats into the warp's shared staging area, row-wise coalesced.  Rows are
-// processed four at a time so that 4 x ceil(sh_n/32) loads are in flight before the first store.
-__device__ __forceinline__ void gather_rows(const float *__restrict__ base, unsigned long long row_of_lane,
-                                            int rows_valid, int sh_n, float *wrows, int row_stride, int lane) {
-    constexpr int kBatch = 4;        // rows per batch: 4 x ceil(sh_n/32) <= 12 loads in flight per lane
-                                     // (8 was slower: register pressure cost more occupancy than it hid latency)
-    for (int r0 = 0; r0 < rows_valid; r0 += kBatch) {
-        if (sh_n <= 96) {
-            float v[kBatch][3];
-#pragma unroll
-            for (int q = 0; q < kBatch; ++q) {
-                const unsigned long long rs = __shfl_sync(0xffffffffu, row_of_lane, min(r0 + q, 31));
-                const float *src = base + rs * (unsigned long long)sh_n;
-#pragma unroll
-                for (int t = 0; t < 3; ++t) {
-                    const int c = lane + 32 * t;
-                    v[q][t] = (r0 + q < rows_valid && c < sh_n) ? __ldg(src + c) : 0.0f;
-                }
-            }
-#pragma unroll
-            for (int q = 0; q < kBatch; ++q)
-#pragma unroll
-                for (int t = 0; t < 3; ++t) {
-                    const int c = lane + 32 * t;
-                    if (r0 + q < rows_valid && c < sh_n) wrows[(r0 + q) * row_stride + c] = v[q][t];
-                }
-        } else {
-            for (int q = 0; q < kBatch; ++q) {
-                const unsigned long long rs = __shfl_sync(0xffffffffu, row_of_lane, min(r0 + q, 31));
-                if (r0 + q < rows_valid)
-                    for (int c = lane; c < sh_n; c += 32)
-                        wrows[(r0 + q) * row_stride + c] = __ldg(base + rs * (unsigned long long)sh_n + c);
-            }
-        }
-    }
-}
-
-// Asynchronous form of gather_rows: every element is one cp.async (LDGSTS, 4 bytes -- rows start on 4-byte
-// boundaries only), so the whole warp's 32 x sh_n floats are in flight at once instead of one L2 / HBM round
-// trip per batch of four rows, and the caller can do unrelated work before gather_rows_wait().  Only the rows of
-// the lanes set in `rows` are fetched; the others are left as they are.
+// Gathers 32 scattered rows of sh_n floats (one per lane's Gaussian, `row_of_lane` = the flat row index held by
+// each lane) into the warp's shared staging area, one padded row per lane.  Every element is one cp.async (LDGSTS,
+// 4 bytes -- rows start on 4-byte boundaries only), so the whole warp's 32 x sh_n floats are in flight at once and
+// the caller can do unrelated work before gather_rows_wait().  Only the rows of the lanes set in `rows` are fetched;
+// the others are left as they are.
 __device__ __forceinline__ void gather_rows_async(const float *__restrict__ base, unsigned long long row_of_lane,
                                                   unsigned rows, int sh_n, float *wrows, int row_stride, int lane) {
     for (unsigned m = rows; m != 0u; m &= m - 1u) {

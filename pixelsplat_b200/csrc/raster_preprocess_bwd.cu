@@ -56,6 +56,133 @@ __device__ __forceinline__ void store_cam_partials(const float (&cam)[kCamEntrie
     }
 }
 
+// The gradient math of one on-screen (view, Gaussian) pair, shared by k_preprocess_bwd and k_camera_bwd so that the
+// camera gradients of both come out of the same expressions.  The statement order is the one the kernels were tuned
+// with (the dcov sums inside the denom2inv branch, then dM, dJ, dL/dt, g, then the perspective terms): computing all
+// of dM, dJ and dL/dt before the dcov sums makes k_preprocess_bwd<false, false> spill.  The SH walk that forms
+// dL/d(direction) for the campos entries stays written out in each kernel: moved into a shared function or visitor,
+// it changed the register allocation and instruction count of every k_preprocess_bwd instantiation.
+
+// What the projection backward of a pair leaves for its callers: dL/dM (rows of M = J W), dL/dJ, the view-space
+// gradient dL/dt, the perspective-divide terms, and the pair's gradient (gx, gy, gz) with respect to the scaled mean.
+struct PairGrad {
+    float dM0[3], dM1[3];
+    float dJ00, dJ02, dJ11, dJ12;
+    float tz, tz2;                 // 1 / t.z and its square
+    float dL_dtx, dL_dty, dL_dtz;
+    float m_w, mul1, mul2;         // 1 / (hw + 1e-7), hx m_w^2, hy m_w^2
+    float gx, gy, gz;
+};
+
+// dL/dconic -> dL/dcov2D -> dL/dM, dL/dJ -> dL/dt -> dL/dmean, plus dL/dmean2D through the perspective divide.
+// COV: also adds the pair's dL/dcov3D (upper triangle, unscaled covariance) to dcov.
+template <bool COV>
+__device__ __forceinline__ PairGrad projection_bwd(const Cov2D &cv, const float (&s6)[6], float sc,
+                                                   const float *__restrict__ vm, const float *__restrict__ pm,
+                                                   float focal_x, float focal_y, float px, float py, float pz,
+                                                   float4 gc, float2 g2, float *dcov) {
+    PairGrad q;
+    const float a = cv.a, b = cv.b, c = cv.c;
+    const float denom = a * c - b * b;
+    const float denom2inv = 1.0f / (denom * denom + 0.0000001f);
+    float dL_da = 0.0f, dL_db = 0.0f, dL_dc = 0.0f;
+    const float *m0 = cv.m0, *m1 = cv.m1;
+    if (denom2inv != 0.0f) {
+        dL_da = denom2inv * (-c * c * gc.x + 2.0f * b * c * gc.y + (denom - a * c) * gc.z);
+        dL_dc = denom2inv * (-a * a * gc.z + 2.0f * a * b * gc.y + (denom - a * c) * gc.x);
+        dL_db = denom2inv * 2.0f * (b * c * gc.x - (denom + 2.0f * b * b) * gc.y + a * b * gc.z);
+        if constexpr (COV) {
+            const float s2 = sc * sc;
+            dcov[0] += s2 * (m0[0] * m0[0] * dL_da + m0[0] * m1[0] * dL_db + m1[0] * m1[0] * dL_dc);
+            dcov[3] += s2 * (m0[1] * m0[1] * dL_da + m0[1] * m1[1] * dL_db + m1[1] * m1[1] * dL_dc);
+            dcov[5] += s2 * (m0[2] * m0[2] * dL_da + m0[2] * m1[2] * dL_db + m1[2] * m1[2] * dL_dc);
+            dcov[1] += s2 * (2.0f * m0[0] * m0[1] * dL_da + (m0[0] * m1[1] + m0[1] * m1[0]) * dL_db + 2.0f * m1[0] * m1[1] * dL_dc);
+            dcov[2] += s2 * (2.0f * m0[0] * m0[2] * dL_da + (m0[0] * m1[2] + m0[2] * m1[0]) * dL_db + 2.0f * m1[0] * m1[2] * dL_dc);
+            dcov[4] += s2 * (2.0f * m0[2] * m0[1] * dL_da + (m0[1] * m1[2] + m0[2] * m1[1]) * dL_db + 2.0f * m1[1] * m1[2] * dL_dc);
+        }
+    }
+    // dL/dM (rows) from a = m0 S m0, b = m0 S m1, c = m1 S m1
+    const float S[3][3] = {{s6[0], s6[1], s6[2]}, {s6[1], s6[3], s6[4]}, {s6[2], s6[4], s6[5]}};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const float sm0 = m0[0] * S[k][0] + m0[1] * S[k][1] + m0[2] * S[k][2];
+        const float sm1 = m1[0] * S[k][0] + m1[1] * S[k][1] + m1[2] * S[k][2];
+        q.dM0[k] = 2.0f * sm0 * dL_da + sm1 * dL_db;
+        q.dM1[k] = 2.0f * sm1 * dL_dc + sm0 * dL_db;
+    }
+    q.dJ00 = vm[0] * q.dM0[0] + vm[4] * q.dM0[1] + vm[8] * q.dM0[2];
+    q.dJ02 = vm[2] * q.dM0[0] + vm[6] * q.dM0[1] + vm[10] * q.dM0[2];
+    q.dJ11 = vm[1] * q.dM1[0] + vm[5] * q.dM1[1] + vm[9] * q.dM1[2];
+    q.dJ12 = vm[2] * q.dM1[0] + vm[6] * q.dM1[1] + vm[10] * q.dM1[2];
+    q.tz = 1.0f / cv.tz; q.tz2 = q.tz * q.tz;
+    const float tz3 = q.tz2 * q.tz;
+    q.dL_dtx = cv.clamp_x ? 0.0f : -focal_x * q.tz2 * q.dJ02;
+    q.dL_dty = cv.clamp_y ? 0.0f : -focal_y * q.tz2 * q.dJ12;
+    q.dL_dtz = -focal_x * q.tz2 * q.dJ00 - focal_y * q.tz2 * q.dJ11 +
+               (2.0f * focal_x * cv.ctx) * tz3 * q.dJ02 + (2.0f * focal_y * cv.cty) * tz3 * q.dJ12;
+    q.gx = vm[0] * q.dL_dtx + vm[1] * q.dL_dty + vm[2] * q.dL_dtz;
+    q.gy = vm[4] * q.dL_dtx + vm[5] * q.dL_dty + vm[6] * q.dL_dtz;
+    q.gz = vm[8] * q.dL_dtx + vm[9] * q.dL_dty + vm[10] * q.dL_dtz;
+
+    // screen-space mean through the perspective divide
+    const float hx = pm[0] * px + pm[4] * py + pm[8] * pz + pm[12];
+    const float hy = pm[1] * px + pm[5] * py + pm[9] * pz + pm[13];
+    const float hw = pm[3] * px + pm[7] * py + pm[11] * pz + pm[15];
+    q.m_w = 1.0f / (hw + 0.0000001f);
+    q.mul1 = hx * q.m_w * q.m_w; q.mul2 = hy * q.m_w * q.m_w;
+    q.gx += (pm[0] * q.m_w - pm[3] * q.mul1) * g2.x + (pm[1] * q.m_w - pm[3] * q.mul2) * g2.y;
+    q.gy += (pm[4] * q.m_w - pm[7] * q.mul1) * g2.x + (pm[5] * q.m_w - pm[7] * q.mul2) * g2.y;
+    q.gz += (pm[8] * q.m_w - pm[11] * q.mul1) * g2.x + (pm[9] * q.m_w - pm[11] * q.mul2) * g2.y;
+    return q;
+}
+
+// The pair's share of the 26 geometric camera entries (cam_row order: [0..23] and [27..28]):
+//   viewmatrix: t = W p + (vm[12], vm[13], vm[14]) and M = J W (W[i][j] = vm[4j+i]);
+//   projmatrix: h = pm p (p.w = 1), screen xy from (hx, hy) / (hw + 1e-7);
+//   tanfov: only through the focal lengths in J (f = size / (2 tanfov); the clamp limit passes nothing).
+__device__ __forceinline__ void camera_geometry_grads(const PairGrad &q, const Cov2D &cv, float px, float py, float pz,
+                                                      float2 g2, float focal_x, float focal_y, float tanfovx,
+                                                      float tanfovy, float (&cam)[kCamEntries]) {
+    const float j00 = focal_x * q.tz, j02 = -focal_x * cv.ctx * q.tz2;
+    const float j11 = focal_y * q.tz, j12 = -focal_y * cv.cty * q.tz2;
+    const float p[3] = {px, py, pz};
+    const float dhx = g2.x * q.m_w, dhy = g2.y * q.m_w, dhw = -(q.mul1 * g2.x + q.mul2 * g2.y);
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        cam[3 * j + 0] = q.dM0[j] * j00 + q.dL_dtx * p[j];
+        cam[3 * j + 1] = q.dM1[j] * j11 + q.dL_dty * p[j];
+        cam[3 * j + 2] = q.dM0[j] * j02 + q.dM1[j] * j12 + q.dL_dtz * p[j];
+        cam[12 + 3 * j + 0] = dhx * p[j];
+        cam[12 + 3 * j + 1] = dhy * p[j];
+        cam[12 + 3 * j + 2] = dhw * p[j];
+    }
+    cam[9] = q.dL_dtx; cam[10] = q.dL_dty; cam[11] = q.dL_dtz;
+    cam[21] = dhx; cam[22] = dhy; cam[23] = dhw;
+    cam[27] = (q.dJ00 * q.tz - q.dJ02 * cv.ctx * q.tz2) * (-focal_x / tanfovx);
+    cam[28] = (q.dJ11 * q.tz - q.dJ12 * cv.cty * q.tz2) * (-focal_y / tanfovy);
+}
+
+// campos entries [24..26]: minus the gradient of the view direction p - campos (dd = p - campos, len2 = |dd|^2,
+// inv3 = 1 / |dd|^3, dLd = dL/d(normalised direction) from the SH walk).  Rounded intrinsics: plain products shared
+// with the Gaussian's own direction chain in k_preprocess_bwd would change how that is contracted, and the Gaussian
+// gradients must keep their bits.
+__device__ __forceinline__ void camera_campos_grads(float ddx, float ddy, float ddz, float len2, float inv3,
+                                                    float3 dLd, float (&cam)[kCamEntries]) {
+    const float dLdx = dLd.x, dLdy = dLd.y, dLdz = dLd.z;
+    const float xx = __fmul_rn(ddx, ddx), yy = __fmul_rn(ddy, ddy), zz = __fmul_rn(ddz, ddz);
+    const float xy = __fmul_rn(ddx, ddy), xz = __fmul_rn(ddx, ddz), yz = __fmul_rn(ddy, ddz);
+    const float ex = __fadd_rn(__fadd_rn(__fmul_rn(__fsub_rn(len2, xx), dLdx), -__fmul_rn(xy, dLdy)), -__fmul_rn(xz, dLdz));
+    const float ey = __fadd_rn(__fadd_rn(-__fmul_rn(xy, dLdx), __fmul_rn(__fsub_rn(len2, yy), dLdy)), -__fmul_rn(yz, dLdz));
+    const float ez = __fadd_rn(__fadd_rn(-__fmul_rn(xz, dLdx), -__fmul_rn(yz, dLdy)), __fmul_rn(__fsub_rn(len2, zz), dLdz));
+    cam[24] = -__fmul_rn(ex, inv3); cam[25] = -__fmul_rn(ey, inv3); cam[26] = -__fmul_rn(ez, inv3);
+}
+
+// The depth chain's camera terms: z = (vm[2], vm[6], vm[10]) . mean + vm[14] / sc, dz = dL/dz.
+__device__ __forceinline__ void camera_depth_grads(float dz, float mx0, float my0, float mz0, float sc,
+                                                   float (&cam)[kCamEntries]) {
+    cam[2] += dz * mx0; cam[5] += dz * my0; cam[8] += dz * mz0; cam[11] += dz / sc;
+}
+
 // Each warp owns 32 consecutive (scene, Gaussian) indices of S*P and writes every element of their rows of every
 // output gradient, which the caller may hand over uninitialised: a Gaussian that is on screen in no view gets zeros,
 // and so does every Gaussian when the binning overflowed its capacity (the composite backward then did not run).  A
@@ -160,77 +287,9 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int
         gcol = vgr.d_color[vg];
         dop += gc.w;
 
-        const float a = cv.a, b = cv.b, c = cv.c;
-        const float denom = a * c - b * b;
-        const float denom2inv = 1.0f / (denom * denom + 0.0000001f);
-        float dL_da = 0.0f, dL_db = 0.0f, dL_dc = 0.0f;
-        const float *m0 = cv.m0, *m1 = cv.m1;
-        if (denom2inv != 0.0f) {
-            dL_da = denom2inv * (-c * c * gc.x + 2.0f * b * c * gc.y + (denom - a * c) * gc.z);
-            dL_dc = denom2inv * (-a * a * gc.z + 2.0f * a * b * gc.y + (denom - a * c) * gc.x);
-            dL_db = denom2inv * 2.0f * (b * c * gc.x - (denom + 2.0f * b * b) * gc.y + a * b * gc.z);
-            const float s2 = sc * sc;
-            dcov[0] += s2 * (m0[0] * m0[0] * dL_da + m0[0] * m1[0] * dL_db + m1[0] * m1[0] * dL_dc);
-            dcov[3] += s2 * (m0[1] * m0[1] * dL_da + m0[1] * m1[1] * dL_db + m1[1] * m1[1] * dL_dc);
-            dcov[5] += s2 * (m0[2] * m0[2] * dL_da + m0[2] * m1[2] * dL_db + m1[2] * m1[2] * dL_dc);
-            dcov[1] += s2 * (2.0f * m0[0] * m0[1] * dL_da + (m0[0] * m1[1] + m0[1] * m1[0]) * dL_db + 2.0f * m1[0] * m1[1] * dL_dc);
-            dcov[2] += s2 * (2.0f * m0[0] * m0[2] * dL_da + (m0[0] * m1[2] + m0[2] * m1[0]) * dL_db + 2.0f * m1[0] * m1[2] * dL_dc);
-            dcov[4] += s2 * (2.0f * m0[2] * m0[1] * dL_da + (m0[1] * m1[2] + m0[2] * m1[1]) * dL_db + 2.0f * m1[1] * m1[2] * dL_dc);
-        }
-        // dL/dM (rows) from a = m0 S m0, b = m0 S m1, c = m1 S m1
-        const float S[3][3] = {{s6[0], s6[1], s6[2]}, {s6[1], s6[3], s6[4]}, {s6[2], s6[4], s6[5]}};
-        float dM0[3], dM1[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            const float sm0 = m0[0] * S[k][0] + m0[1] * S[k][1] + m0[2] * S[k][2];
-            const float sm1 = m1[0] * S[k][0] + m1[1] * S[k][1] + m1[2] * S[k][2];
-            dM0[k] = 2.0f * sm0 * dL_da + sm1 * dL_db;
-            dM1[k] = 2.0f * sm1 * dL_dc + sm0 * dL_db;
-        }
-        const float dJ00 = vm[0] * dM0[0] + vm[4] * dM0[1] + vm[8] * dM0[2];
-        const float dJ02 = vm[2] * dM0[0] + vm[6] * dM0[1] + vm[10] * dM0[2];
-        const float dJ11 = vm[1] * dM1[0] + vm[5] * dM1[1] + vm[9] * dM1[2];
-        const float dJ12 = vm[2] * dM1[0] + vm[6] * dM1[1] + vm[10] * dM1[2];
-        const float tz = 1.0f / cv.tz, tz2 = tz * tz, tz3 = tz2 * tz;
-        const float dL_dtx = cv.clamp_x ? 0.0f : -focal_x * tz2 * dJ02;
-        const float dL_dty = cv.clamp_y ? 0.0f : -focal_y * tz2 * dJ12;
-        const float dL_dtz = -focal_x * tz2 * dJ00 - focal_y * tz2 * dJ11 +
-                             (2.0f * focal_x * cv.ctx) * tz3 * dJ02 + (2.0f * focal_y * cv.cty) * tz3 * dJ12;
-        gx = vm[0] * dL_dtx + vm[1] * dL_dty + vm[2] * dL_dtz;
-        gy = vm[4] * dL_dtx + vm[5] * dL_dty + vm[6] * dL_dtz;
-        gz = vm[8] * dL_dtx + vm[9] * dL_dty + vm[10] * dL_dtz;
-
-        // screen-space mean through the perspective divide
-        const float hx = pm[0] * px + pm[4] * py + pm[8] * pz + pm[12];
-        const float hy = pm[1] * px + pm[5] * py + pm[9] * pz + pm[13];
-        const float hw = pm[3] * px + pm[7] * py + pm[11] * pz + pm[15];
-        const float m_w = 1.0f / (hw + 0.0000001f);
-        const float mul1 = hx * m_w * m_w, mul2 = hy * m_w * m_w;
-        gx += (pm[0] * m_w - pm[3] * mul1) * g2.x + (pm[1] * m_w - pm[3] * mul2) * g2.y;
-        gy += (pm[4] * m_w - pm[7] * mul1) * g2.x + (pm[5] * m_w - pm[7] * mul2) * g2.y;
-        gz += (pm[8] * m_w - pm[11] * mul1) * g2.x + (pm[9] * m_w - pm[11] * mul2) * g2.y;
-        if (CAM) {
-            // viewmatrix: t = W p + (vm[12], vm[13], vm[14]) and M = J W (W[i][j] = vm[4j+i]);
-            // projmatrix: h = pm p (p.w = 1), screen xy from (hx, hy) / (hw + 1e-7);
-            // tanfov: only through the focal lengths in J (f = size / (2 tanfov); the clamp limit passes nothing)
-            const float j00 = focal_x * tz, j02 = -focal_x * cv.ctx * tz2;
-            const float j11 = focal_y * tz, j12 = -focal_y * cv.cty * tz2;
-            const float p[3] = {px, py, pz};
-            const float dhx = g2.x * m_w, dhy = g2.y * m_w, dhw = -(mul1 * g2.x + mul2 * g2.y);
-#pragma unroll
-            for (int j = 0; j < 3; ++j) {
-                cam[3 * j + 0] = dM0[j] * j00 + dL_dtx * p[j];
-                cam[3 * j + 1] = dM1[j] * j11 + dL_dty * p[j];
-                cam[3 * j + 2] = dM0[j] * j02 + dM1[j] * j12 + dL_dtz * p[j];
-                cam[12 + 3 * j + 0] = dhx * p[j];
-                cam[12 + 3 * j + 1] = dhy * p[j];
-                cam[12 + 3 * j + 2] = dhw * p[j];
-            }
-            cam[9] = dL_dtx; cam[10] = dL_dty; cam[11] = dL_dtz;
-            cam[21] = dhx; cam[22] = dhy; cam[23] = dhw;
-            cam[27] = (dJ00 * tz - dJ02 * cv.ctx * tz2) * (-focal_x / tanfovx);
-            cam[28] = (dJ11 * tz - dJ12 * cv.cty * tz2) * (-focal_y / tanfovy);
-        }
+        const PairGrad q = projection_bwd<true>(cv, s6, sc, vm, pm, focal_x, focal_y, px, py, pz, gc, g2, dcov);
+        gx = q.gx; gy = q.gy; gz = q.gz;
+        if constexpr (CAM) camera_geometry_grads(q, cv, px, py, pz, g2, focal_x, focal_y, tanfovx, tanfovy, cam);
         }   // vis (geometry part)
 
         if (M > 0 && !sh_ready) {          // warp-uniform; the rows have had the geometry math to arrive
@@ -273,16 +332,7 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int
             gx += ((len2 - ddx * ddx) * dLdx - ddy * ddx * dLdy - ddz * ddx * dLdz) * inv3;
             gy += (-ddx * ddy * dLdx + (len2 - ddy * ddy) * dLdy - ddz * ddy * dLdz) * inv3;
             gz += (-ddx * ddz * dLdx - ddy * ddz * dLdy + (len2 - ddz * ddz) * dLdz) * inv3;
-            if (CAM) {
-                // the direction is p - campos.  Rounded intrinsics: plain products shared with the lines above
-                // would change how those are contracted, and the Gaussian gradients must keep their bits.
-                const float xx = __fmul_rn(ddx, ddx), yy = __fmul_rn(ddy, ddy), zz = __fmul_rn(ddz, ddz);
-                const float xy = __fmul_rn(ddx, ddy), xz = __fmul_rn(ddx, ddz), yz = __fmul_rn(ddy, ddz);
-                const float ex = __fadd_rn(__fadd_rn(__fmul_rn(__fsub_rn(len2, xx), dLdx), -__fmul_rn(xy, dLdy)), -__fmul_rn(xz, dLdz));
-                const float ey = __fadd_rn(__fadd_rn(-__fmul_rn(xy, dLdx), __fmul_rn(__fsub_rn(len2, yy), dLdy)), -__fmul_rn(yz, dLdz));
-                const float ez = __fadd_rn(__fadd_rn(-__fmul_rn(xz, dLdx), -__fmul_rn(yz, dLdy)), __fmul_rn(__fsub_rn(len2, zz), dLdz));
-                cam[24] = -__fmul_rn(ex, inv3); cam[25] = -__fmul_rn(ey, inv3); cam[26] = -__fmul_rn(ez, inv3);
-            }
+            if constexpr (CAM) camera_campos_grads(ddx, ddy, ddz, len2, inv3, dLd, cam);
         } else if (vis) {
             dcol[0] += gcol.x; dcol[1] += gcol.y; dcol[2] += gcol.z;
         }
@@ -293,9 +343,7 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int
             const float *__restrict__ vm = in.view + 16 * vid;
             const float dz = vgr.d_color[vg].w * depth_value_grad(d.depth_mode, geo.depth[vg], in.scale, in.near_far, vid);
             dmx += dz * vm[2]; dmy += dz * vm[6]; dmz += dz * vm[10];
-            if (CAM) {   // z = (vm[2], vm[6], vm[10]) . mean + vm[14] / sc
-                cam[2] += dz * mx0; cam[5] += dz * my0; cam[8] += dz * mz0; cam[11] += dz / sc;
-            }
+            if constexpr (CAM) camera_depth_grads(dz, mx0, my0, mz0, sc, cam);
         }
         if constexpr (CAM) store_cam_partials(cam, cam_ws, d, v, sg0, rows, scene, lane);
     }
@@ -350,7 +398,7 @@ int launch_clear_pair_grads(const Dims &d, const Geom &g, const ViewGrads &vg, c
 }
 
 // Camera-only backward (ps_raster_grads with every Gaussian gradient NULL): the 29 camera entries of k_preprocess_bwd's
-// CAM path, and nothing else.  One thread per (view, Gaussian) pair; a CTA covers kCamBwdThreads consecutive (scene,
+// CAM path, formed by the same functions, and nothing else.  One thread per (view, Gaussian) pair; a CTA covers kCamBwdThreads consecutive (scene,
 // Gaussian) indices of S*P for ONE view v (blockIdx.x = chunk * V + v: the V CTAs of a chunk run side by side and share
 // its SH rows in L2), so each warp stores exactly the partial rows k_preprocess_bwd<·, true> stores for (its 32
 // indices, v), summed in the same order, and the same k_camera_finish adds them.  It reads the scratch of the on-screen
@@ -405,58 +453,8 @@ k_camera_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, int row_stride, float *
         compute_cov2d(px, py, pz, s6, vm, focal_x, focal_y, tanfovx, tanfovy, cv);
         const float2 g2 = vgr.d_mean2d[vg];
         const float4 gc = vgr.d_conic[vg];
-
-        // the CAM path of k_preprocess_bwd, term for term
-        const float a = cv.a, b = cv.b, c = cv.c;
-        const float denom = a * c - b * b;
-        const float denom2inv = 1.0f / (denom * denom + 0.0000001f);
-        float dL_da = 0.0f, dL_db = 0.0f, dL_dc = 0.0f;
-        const float *m0 = cv.m0, *m1 = cv.m1;
-        if (denom2inv != 0.0f) {
-            dL_da = denom2inv * (-c * c * gc.x + 2.0f * b * c * gc.y + (denom - a * c) * gc.z);
-            dL_dc = denom2inv * (-a * a * gc.z + 2.0f * a * b * gc.y + (denom - a * c) * gc.x);
-            dL_db = denom2inv * 2.0f * (b * c * gc.x - (denom + 2.0f * b * b) * gc.y + a * b * gc.z);
-        }
-        const float S[3][3] = {{s6[0], s6[1], s6[2]}, {s6[1], s6[3], s6[4]}, {s6[2], s6[4], s6[5]}};
-        float dM0[3], dM1[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            const float sm0 = m0[0] * S[k][0] + m0[1] * S[k][1] + m0[2] * S[k][2];
-            const float sm1 = m1[0] * S[k][0] + m1[1] * S[k][1] + m1[2] * S[k][2];
-            dM0[k] = 2.0f * sm0 * dL_da + sm1 * dL_db;
-            dM1[k] = 2.0f * sm1 * dL_dc + sm0 * dL_db;
-        }
-        const float dJ00 = vm[0] * dM0[0] + vm[4] * dM0[1] + vm[8] * dM0[2];
-        const float dJ02 = vm[2] * dM0[0] + vm[6] * dM0[1] + vm[10] * dM0[2];
-        const float dJ11 = vm[1] * dM1[0] + vm[5] * dM1[1] + vm[9] * dM1[2];
-        const float dJ12 = vm[2] * dM1[0] + vm[6] * dM1[1] + vm[10] * dM1[2];
-        const float tz = 1.0f / cv.tz, tz2 = tz * tz, tz3 = tz2 * tz;
-        const float dL_dtx = cv.clamp_x ? 0.0f : -focal_x * tz2 * dJ02;
-        const float dL_dty = cv.clamp_y ? 0.0f : -focal_y * tz2 * dJ12;
-        const float dL_dtz = -focal_x * tz2 * dJ00 - focal_y * tz2 * dJ11 +
-                             (2.0f * focal_x * cv.ctx) * tz3 * dJ02 + (2.0f * focal_y * cv.cty) * tz3 * dJ12;
-        const float hx = pm[0] * px + pm[4] * py + pm[8] * pz + pm[12];
-        const float hy = pm[1] * px + pm[5] * py + pm[9] * pz + pm[13];
-        const float hw = pm[3] * px + pm[7] * py + pm[11] * pz + pm[15];
-        const float m_w = 1.0f / (hw + 0.0000001f);
-        const float mul1 = hx * m_w * m_w, mul2 = hy * m_w * m_w;
-        const float j00 = focal_x * tz, j02 = -focal_x * cv.ctx * tz2;
-        const float j11 = focal_y * tz, j12 = -focal_y * cv.cty * tz2;
-        const float p[3] = {px, py, pz};
-        const float dhx = g2.x * m_w, dhy = g2.y * m_w, dhw = -(mul1 * g2.x + mul2 * g2.y);
-#pragma unroll
-        for (int j = 0; j < 3; ++j) {
-            cam[3 * j + 0] = dM0[j] * j00 + dL_dtx * p[j];
-            cam[3 * j + 1] = dM1[j] * j11 + dL_dty * p[j];
-            cam[3 * j + 2] = dM0[j] * j02 + dM1[j] * j12 + dL_dtz * p[j];
-            cam[12 + 3 * j + 0] = dhx * p[j];
-            cam[12 + 3 * j + 1] = dhy * p[j];
-            cam[12 + 3 * j + 2] = dhw * p[j];
-        }
-        cam[9] = dL_dtx; cam[10] = dL_dty; cam[11] = dL_dtz;
-        cam[21] = dhx; cam[22] = dhy; cam[23] = dhw;
-        cam[27] = (dJ00 * tz - dJ02 * cv.ctx * tz2) * (-focal_x / tanfovx);
-        cam[28] = (dJ11 * tz - dJ12 * cv.cty * tz2) * (-focal_y / tanfovy);
+        const PairGrad q = projection_bwd<false>(cv, s6, sc, vm, pm, focal_x, focal_y, px, py, pz, gc, g2, nullptr);
+        camera_geometry_grads(q, cv, px, py, pz, g2, focal_x, focal_y, tanfovx, tanfovy, cam);
     }
     if (M > 0) gather_rows_wait();         // warp-uniform
     if (M > 0 && vis) {
@@ -482,18 +480,12 @@ k_camera_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, int row_stride, float *
             }
         });
         const float3 dLd = sh_grad_unpermute(d.sh_basis, dLda, dLdb, dLdc);
-        const float dLdx = dLd.x, dLdy = dLd.y, dLdz = dLd.z;
         const float inv3 = 1.0f / (len2 * len);
-        const float xx = __fmul_rn(ddx, ddx), yy = __fmul_rn(ddy, ddy), zz = __fmul_rn(ddz, ddz);
-        const float xy = __fmul_rn(ddx, ddy), xz = __fmul_rn(ddx, ddz), yz = __fmul_rn(ddy, ddz);
-        const float ex = __fadd_rn(__fadd_rn(__fmul_rn(__fsub_rn(len2, xx), dLdx), -__fmul_rn(xy, dLdy)), -__fmul_rn(xz, dLdz));
-        const float ey = __fadd_rn(__fadd_rn(-__fmul_rn(xy, dLdx), __fmul_rn(__fsub_rn(len2, yy), dLdy)), -__fmul_rn(yz, dLdz));
-        const float ez = __fadd_rn(__fadd_rn(-__fmul_rn(xz, dLdx), -__fmul_rn(yz, dLdy)), __fmul_rn(__fsub_rn(len2, zz), dLdz));
-        cam[24] = -__fmul_rn(ex, inv3); cam[25] = -__fmul_rn(ey, inv3); cam[26] = -__fmul_rn(ez, inv3);
+        camera_campos_grads(ddx, ddy, ddz, len2, inv3, dLd, cam);
     }
-    if (DEPTH && vis) {   // z = (vm[2], vm[6], vm[10]) . mean + vm[14] / sc
+    if (DEPTH && vis) {
         const float dz = vgr.d_color[vg].w * depth_value_grad(d.depth_mode, geo.depth[vg], in.scale, in.near_far, vid);
-        cam[2] += dz * mx0; cam[5] += dz * my0; cam[8] += dz * mz0; cam[11] += dz / sc;
+        camera_depth_grads(dz, mx0, my0, mz0, sc, cam);
     }
     store_cam_partials(cam, cam_ws, d, v, sg0, rows, scene, lane);
 }
