@@ -509,7 +509,29 @@ PS_API int ps_ssim_backward(int32_t n_planes, int32_t H, int32_t W, const float 
                             const float *d_mean, float *d_x /* or NULL */, float *d_y, void *workspace,
                             size_t workspace_bytes, void *stream);
 
-/* ---- LPIPS distance head (csrc/lpips.cu) ---------------------------------------------------------------------
+/* ---- ViT self-attention, flash-style (csrc/vit_attention.cu; wgmma, TF32 operands, FP32 accumulate) --------
+ * The attention of DINO's ViT blocks, softmax(q k^T * scale) v, without any L x L tensor:
+ *   qkv  [n_images, tokens, 3 * heads * 64]   "(qkv h d)": DINO's qkv(x).reshape(B, N, 3, H, C // H)
+ *   out  [n_images, tokens, heads * 64]       "(h d)": (attn @ v).transpose(1, 2).reshape(B, N, C)
+ *   lse  [n_images, heads, tokens]            ln sum_j exp(q_i . k_j * scale), saved for the backward
+ * Supported: dim_head == 64, 1 <= tokens <= 16384 (any count, no tile multiple), 1 <= heads <= 16,
+ * n_images <= 65535; anything else returns PS_ERR_UNSUPPORTED (counts < 1: PS_ERR_INVALID_ARGUMENT).  qkv, out,
+ * d_out and d_qkv must be 16-byte aligned.  No host synchronisation: both calls can be captured in a CUDA graph. */
+PS_API int ps_vit_attention_forward(int32_t n_images, int32_t tokens, int32_t heads, int32_t dim_head,
+                                    const float *qkv, float scale, float *out, float *lse, void *stream);
+
+/* Bytes of workspace ps_vit_attention_backward needs (D = rowsum(dO o O), n_images * heads * tokens floats). */
+PS_API int ps_vit_attention_backward_workspace_bytes(int32_t n_images, int32_t tokens, int32_t heads,
+                                                     int32_t dim_head, size_t *out);
+
+/* Backward of the forward above, with P recomputed from lse.  d_qkv has qkv's layout and is fully written; there
+ * are no float atomics, so the result is the same bits on every run. */
+PS_API int ps_vit_attention_backward(int32_t n_images, int32_t tokens, int32_t heads, int32_t dim_head,
+                                     const float *qkv, const float *out, const float *d_out, const float *lse,
+                                     float scale, float *d_qkv, void *workspace, size_t workspace_bytes,
+                                     void *stream);
+
+/* ---- LPIPS distance head (csrc/lpips.cu)---------------------------------------------------------------------
  * The head of the lpips package's LPIPS(net="vgg") (version 0.1) on up to five feature layers.  For layer l with
  * features x0, x1 [N, C, H, W] (contiguous NCHW) and the 1x1 `lin` weight w [C] (no bias), per image n and pixel p:
  *   f^ = f / (sqrt(sum_c f_c^2) + 1e-10)   (each side),   u = f^0 - f^1,

@@ -124,7 +124,8 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_raster_backward_depth", "ps_ssim_workspace_bytes", "ps_ssim_forward", "ps_ssim_backward",
            "ps_epipolar_attention_backward_workspace_bytes", "ps_epipolar_attention_backward_deterministic",
            "ps_raster_camera_workspace_bytes", "ps_camera_setup_backward", "ps_lpips_workspace_bytes",
-           "ps_lpips_forward", "ps_lpips_backward")
+           "ps_lpips_forward", "ps_lpips_backward", "ps_vit_attention_forward",
+           "ps_vit_attention_backward_workspace_bytes", "ps_vit_attention_backward")
 
 
 class NativeLibraryMissing(ImportError):
@@ -211,6 +212,14 @@ def _load() -> ctypes.CDLL:
     lib.ps_lpips_forward.restype = ctypes.c_int
     lib.ps_lpips_backward.argtypes = [P(LpipsDesc), ctypes.c_void_p, P(LpipsGrads), ctypes.c_void_p]
     lib.ps_lpips_backward.restype = ctypes.c_int
+    lib.ps_vit_attention_forward.argtypes = [ctypes.c_int32] * 4 + [ctypes.c_void_p, ctypes.c_float] + \
+        [ctypes.c_void_p] * 3
+    lib.ps_vit_attention_forward.restype = ctypes.c_int
+    lib.ps_vit_attention_backward_workspace_bytes.argtypes = [ctypes.c_int32] * 4 + [P(ctypes.c_size_t)]
+    lib.ps_vit_attention_backward_workspace_bytes.restype = ctypes.c_int
+    lib.ps_vit_attention_backward.argtypes = [ctypes.c_int32] * 4 + [ctypes.c_void_p] * 4 + \
+        [ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
+    lib.ps_vit_attention_backward.restype = ctypes.c_int
     for f in ("ps_raster_sizes_query", "ps_raster_layout_query", "ps_raster_forward", "ps_raster_backward"):
         getattr(lib, f).restype = ctypes.c_int
     return lib
