@@ -582,6 +582,37 @@ PS_API int ps_lpips_forward(const ps_lpips_desc *desc, float *out, void *workspa
 PS_API int ps_lpips_backward(const ps_lpips_desc *desc, const float *d_out, const ps_lpips_grads *grads,
                              void *stream);
 
+/* ---- Crop shim of the data pipeline (csrc/image_resample.cu) --------------------------------------------------
+ * Replaces the reference's per-view host route src/dataset/shims/crop_shim.py (rescale: float -> uint8 -> PIL
+ * Image.resize(LANCZOS) -> / 255; center_crop) with the flip of augmentation_shim.py applied first, for a batch of
+ * decoded views in one launch:
+ *   images [n_images, in_h, in_w, 3] uint8 (HWC, as PIL decodes them)  ->  out [n_images, 3, out_h, out_w] float32.
+ * Per image: flip horizontally when flip[i] != 0 (flip NULL: no image is flipped); resample exactly as Pillow's
+ * ImagingResample does for 8-bit images (a horizontal pass, then a vertical one, each summing in int32 from 2^21
+ * and clipping to uint8, coefficients with 22 fraction bits); keep only the crop; write u / 255.0f.
+ * The coefficient tables cover the crop only.  Output column j reads input columns [bounds_h[2j], + bounds_h[2j+1])
+ * with weights weights_h[j * taps_h + ...]; output row i reads intermediate rows [bounds_v[2i], + bounds_v[2i+1])
+ * with weights_v[i * taps_v + ...].  A pass Pillow skips (its axis keeps its size) is an identity table: taps 1,
+ * bounds (crop offset + j, 1), weight 1 << 22.  pixelsplat_b200/data/crop_shim.py builds the tables in float64 on
+ * the host, as Pillow does; the kernel clamps each window to the image and never evaluates a filter.
+ * All arithmetic after the tables is integer: the same bits as Pillow on every run.  No host synchronisation and
+ * no host memory, so a call can be captured in a CUDA graph.  Rejects n_images outside [1, 65535], non-positive
+ * sizes, an output larger than the input, taps_h outside [1, in_w] or taps_v outside [1, in_h], and NULL pointers
+ * (flip excepted) with PS_ERR_INVALID_ARGUMENT before anything is enqueued. */
+typedef struct {
+    int32_t n_images, in_h, in_w;
+    int32_t out_h, out_w;               /* the crop */
+    int32_t taps_h, taps_v;             /* coefficients per output column / row */
+    const uint8_t *images;              /* [n_images, in_h, in_w, 3] */
+    const uint8_t *flip;                /* [n_images] or NULL */
+    const int32_t *bounds_h;            /* [out_w, 2] first input column, count */
+    const int32_t *weights_h;           /* [out_w, taps_h] */
+    const int32_t *bounds_v;            /* [out_h, 2] first input row, count */
+    const int32_t *weights_v;           /* [out_h, taps_v] */
+} ps_resample_desc;
+
+PS_API int ps_image_resample(const ps_resample_desc *desc, float *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -104,6 +104,11 @@ class LpipsGrads(ctypes.Structure):
     _fields_ = [("d_x0", ctypes.c_void_p * LPIPS_MAX_LAYERS), ("d_x1", ctypes.c_void_p * LPIPS_MAX_LAYERS)]
 
 
+class ResampleDesc(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("n_images", "in_h", "in_w", "out_h", "out_w", "taps_h", "taps_v")] + \
+        [(n, ctypes.c_void_p) for n in ("images", "flip", "bounds_h", "weights_h", "bounds_v", "weights_v")]
+
+
 class RasterCameraGrads(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in ("d_viewmatrix", "d_projmatrix", "d_campos", "d_tanfov", "workspace")] + \
         [("workspace_bytes", ctypes.c_size_t)]
@@ -125,7 +130,7 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_epipolar_attention_backward_workspace_bytes", "ps_epipolar_attention_backward_deterministic",
            "ps_raster_camera_workspace_bytes", "ps_camera_setup_backward", "ps_lpips_workspace_bytes",
            "ps_lpips_forward", "ps_lpips_backward", "ps_vit_attention_forward",
-           "ps_vit_attention_backward_workspace_bytes", "ps_vit_attention_backward")
+           "ps_vit_attention_backward_workspace_bytes", "ps_vit_attention_backward", "ps_image_resample")
 
 
 class NativeLibraryMissing(ImportError):
@@ -220,6 +225,8 @@ def _load() -> ctypes.CDLL:
     lib.ps_vit_attention_backward.argtypes = [ctypes.c_int32] * 4 + [ctypes.c_void_p] * 4 + \
         [ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
     lib.ps_vit_attention_backward.restype = ctypes.c_int
+    lib.ps_image_resample.argtypes = [P(ResampleDesc), ctypes.c_void_p, ctypes.c_void_p]
+    lib.ps_image_resample.restype = ctypes.c_int
     for f in ("ps_raster_sizes_query", "ps_raster_layout_query", "ps_raster_forward", "ps_raster_backward"):
         getattr(lib, f).restype = ctypes.c_int
     return lib
