@@ -613,6 +613,42 @@ typedef struct {
 
 PS_API int ps_image_resample(const ps_resample_desc *desc, float *out, void *stream);
 
+/* ---- 8-bit frame pass of an evaluation (csrc/eval_images.cu) ------------------------------------------------------
+ * The reference scores 8-bit frames, not float renders: its test step writes each render as a PNG through
+ * src/misc/image_io.py's prep_image, (clip(x, 0, 1) * 255).type(uint8), and its metric computer reads the PNGs back
+ * through ToTensor (u / 255).  One launch per chunk of up to PS_EVAL_MAX_IMAGES images [n, 3, h, w]:
+ *   PS_EVAL_RENDER  render float32 [n, 3, h, w] (CHW): u = the float32 product clip(x, 0, 1) * 255 truncated toward
+ *                   zero (prep_image's cast); NaN, which has no defined value there, gives u = 0;
+ *   PS_EVAL_FRAME   frame_in uint8 [n, h, w, 3] (HWC): u = the decoded bytes as they are.
+ * Outputs, each NULL when not wanted (at least one is required):
+ *   frame_out  uint8 [n, h, w, 3]: u, the byte layout PIL.Image.fromarray takes (render mode only);
+ *   planes     float32 [n, 3, h, w]: u / 255.0f (what ToTensor gives for the PNG);
+ *   sse        float64 [n]: sum over the image's 3 h w values of (u / 255.0f - clip(target, 0, 1))^2 formed in
+ *              float64, with target float32 [n, 3, h, w] (torch's clip: NaN stays NaN).  target and sse go together.
+ * The sum is formed in a fixed order (per-tile partials in `workspace`, then a finish launch), so the same inputs give
+ * the same bits on every run; the workspace (ps_eval_images_workspace_bytes, no initialisation) is needed only with
+ * sse.  No host synchronisation (graph-capturable).  Rejects a NULL desc, an unknown mode, n_images outside
+ * [1, PS_EVAL_MAX_IMAGES], non-positive sizes, more than 2^31 - 1 values, a missing input or an input of the other
+ * mode, no output, frame_out in frame mode, target without sse or sse without target, and a NULL or short workspace
+ * with sse, with PS_ERR_INVALID_ARGUMENT before anything is enqueued. */
+#define PS_EVAL_RENDER 0
+#define PS_EVAL_FRAME 1
+#define PS_EVAL_MAX_IMAGES 32
+
+typedef struct {
+    int32_t mode;                       /* PS_EVAL_* */
+    int32_t n_images, height, width;
+    const float *render;                /* [n, 3, h, w] (render mode) or NULL */
+    const uint8_t *frame_in;            /* [n, h, w, 3] (frame mode) or NULL */
+    const float *target;                /* [n, 3, h, w] or NULL */
+    uint8_t *frame_out;                 /* [n, h, w, 3] or NULL */
+    float *planes;                      /* [n, 3, h, w] or NULL */
+    double *sse;                        /* [n] or NULL */
+} ps_eval_desc;
+
+PS_API int ps_eval_images_workspace_bytes(int32_t n_images, int32_t height, int32_t width, size_t *out);
+PS_API int ps_eval_images(const ps_eval_desc *desc, void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -109,6 +109,15 @@ class ResampleDesc(ctypes.Structure):
         [(n, ctypes.c_void_p) for n in ("images", "flip", "bounds_h", "weights_h", "bounds_v", "weights_v")]
 
 
+PS_EVAL_RENDER, PS_EVAL_FRAME = 0, 1
+EVAL_MAX_IMAGES = 32
+
+
+class EvalDesc(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("mode", "n_images", "height", "width")] + \
+        [(n, ctypes.c_void_p) for n in ("render", "frame_in", "target", "frame_out", "planes", "sse")]
+
+
 class RasterCameraGrads(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in ("d_viewmatrix", "d_projmatrix", "d_campos", "d_tanfov", "workspace")] + \
         [("workspace_bytes", ctypes.c_size_t)]
@@ -130,7 +139,8 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_epipolar_attention_backward_workspace_bytes", "ps_epipolar_attention_backward_deterministic",
            "ps_raster_camera_workspace_bytes", "ps_camera_setup_backward", "ps_lpips_workspace_bytes",
            "ps_lpips_forward", "ps_lpips_backward", "ps_vit_attention_forward",
-           "ps_vit_attention_backward_workspace_bytes", "ps_vit_attention_backward", "ps_image_resample")
+           "ps_vit_attention_backward_workspace_bytes", "ps_vit_attention_backward", "ps_image_resample",
+           "ps_eval_images_workspace_bytes", "ps_eval_images")
 
 
 class NativeLibraryMissing(ImportError):
@@ -227,6 +237,10 @@ def _load() -> ctypes.CDLL:
     lib.ps_vit_attention_backward.restype = ctypes.c_int
     lib.ps_image_resample.argtypes = [P(ResampleDesc), ctypes.c_void_p, ctypes.c_void_p]
     lib.ps_image_resample.restype = ctypes.c_int
+    lib.ps_eval_images_workspace_bytes.argtypes = [ctypes.c_int32] * 3 + [P(ctypes.c_size_t)]
+    lib.ps_eval_images_workspace_bytes.restype = ctypes.c_int
+    lib.ps_eval_images.argtypes = [P(EvalDesc), ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
+    lib.ps_eval_images.restype = ctypes.c_int
     for f in ("ps_raster_sizes_query", "ps_raster_layout_query", "ps_raster_forward", "ps_raster_backward"):
         getattr(lib, f).restype = ctypes.c_int
     return lib
