@@ -649,6 +649,55 @@ typedef struct {
 PS_API int ps_eval_images_workspace_bytes(int32_t n_images, int32_t height, int32_t width, size_t *out);
 PS_API int ps_eval_images(const ps_eval_desc *desc, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- Gradient clipping + Adam over a table of tensors (csrc/optimizer.cu) -----------------------------------------
+ * One optimiser step of the reference's training (gradient_clip_val 0.5, optim.Adam without weight decay or amsgrad,
+ * LinearLR(1 / W, 1, total_iters = W) stepped once per optimiser step) on float32 tensors, in two launches whatever
+ * their number:
+ *   norm    total = L2 norm of the tensors' L2 norms (torch's clip_grad_norm_), written to state->grad_norm;
+ *   update  coef = min(1, max_norm / (total + 1e-6)), g' = coef g (never written back: the gradients are only read),
+ *           t = *state->step + 1, lr_t = lr (1 / W + (1 - 1 / W) min(t - 1, W) / W)  (lr when W = 0),
+ *           m += (1 - beta1) (g' - m),  v = beta2 v + (1 - beta2) g'^2,
+ *           p -= lr_t / (1 - beta1^t) * m / (sqrt(v) / sqrt(1 - beta2^t) + eps);  then *state->step = t.
+ * Everything the step depends on lives on the device (the table, the int64 step counter, the norm), and nothing is
+ * read back: the call can be captured in a CUDA graph, and each replay is one more step.  Every sum has a fixed order:
+ * equal inputs give equal bits.  A NaN gradient makes the norm, the coefficient and so every parameter NaN, as torch
+ * does with error_if_nonfinite=False.  A tensor whose gradient and moments are zero is left bit-unchanged.
+ *
+ * `segments` is a device array of desc->n_segments rows.  Row i's first_chunk is the sum of
+ * ps_clip_adam_segment_chunks(grad, count) over the rows before it, and desc->n_chunks is the sum over all rows (a
+ * tensor is cut into chunks of PS_CLIP_ADAM_CHUNK elements on a grid aligned to its gradient's 16-byte boundary).
+ * count >= 1 in every row; tensors may start at any 4-byte aligned address.  The rows are trusted.
+ * `workspace`: ps_clip_adam_workspace_bytes, 16-byte aligned, zero-filled before the first call and not touched by the
+ * caller afterwards.  Rejects NULL pointers, n_segments < 1, n_chunks outside [n_segments, 2^31 - 1], scalars outside
+ * lr >= 0, 0 <= beta < 1, eps >= 0, max_norm > 0, warm_up_steps >= 0, and a short or misaligned workspace with
+ * PS_ERR_INVALID_ARGUMENT before anything is enqueued. */
+#define PS_CLIP_ADAM_CHUNK 4096
+
+typedef struct {
+    float *param;
+    const float *grad;
+    float *exp_avg, *exp_avg_sq;
+    int64_t count;                      /* elements, >= 1 */
+    int64_t first_chunk;
+} ps_clip_adam_segment;
+
+typedef struct {
+    int32_t n_segments, reserved;
+    int64_t n_chunks;
+    int64_t warm_up_steps;              /* W */
+    double lr, beta1, beta2, eps, max_norm;
+} ps_clip_adam_desc;
+
+typedef struct {
+    int64_t *step;                      /* device: optimiser steps taken so far */
+    float *grad_norm;                   /* device: the last step's total gradient norm (before clipping) */
+} ps_clip_adam_state;
+
+PS_API int64_t ps_clip_adam_segment_chunks(const void *grad, int64_t count);
+PS_API int ps_clip_adam_workspace_bytes(const ps_clip_adam_desc *desc, size_t *out);
+PS_API int ps_clip_adam_step(const ps_clip_adam_desc *desc, const ps_clip_adam_segment *segments,
+                             const ps_clip_adam_state *state, void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -118,6 +118,20 @@ class EvalDesc(ctypes.Structure):
         [(n, ctypes.c_void_p) for n in ("render", "frame_in", "target", "frame_out", "planes", "sse")]
 
 
+CLIP_ADAM_CHUNK = 4096
+CLIP_ADAM_SEGMENT_FIELDS = ("param", "grad", "exp_avg", "exp_avg_sq", "count", "first_chunk")   # 6 x 8 bytes a row
+
+
+class ClipAdamDesc(ctypes.Structure):
+    _fields_ = [("n_segments", ctypes.c_int32), ("reserved", ctypes.c_int32), ("n_chunks", ctypes.c_int64),
+                ("warm_up_steps", ctypes.c_int64)] + \
+        [(n, ctypes.c_double) for n in ("lr", "beta1", "beta2", "eps", "max_norm")]
+
+
+class ClipAdamState(ctypes.Structure):
+    _fields_ = [("step", ctypes.c_void_p), ("grad_norm", ctypes.c_void_p)]
+
+
 class RasterCameraGrads(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in ("d_viewmatrix", "d_projmatrix", "d_campos", "d_tanfov", "workspace")] + \
         [("workspace_bytes", ctypes.c_size_t)]
@@ -140,7 +154,8 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_raster_camera_workspace_bytes", "ps_camera_setup_backward", "ps_lpips_workspace_bytes",
            "ps_lpips_forward", "ps_lpips_backward", "ps_vit_attention_forward",
            "ps_vit_attention_backward_workspace_bytes", "ps_vit_attention_backward", "ps_image_resample",
-           "ps_eval_images_workspace_bytes", "ps_eval_images")
+           "ps_eval_images_workspace_bytes", "ps_eval_images", "ps_clip_adam_segment_chunks",
+           "ps_clip_adam_workspace_bytes", "ps_clip_adam_step")
 
 
 class NativeLibraryMissing(ImportError):
@@ -241,6 +256,13 @@ def _load() -> ctypes.CDLL:
     lib.ps_eval_images_workspace_bytes.restype = ctypes.c_int
     lib.ps_eval_images.argtypes = [P(EvalDesc), ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]
     lib.ps_eval_images.restype = ctypes.c_int
+    lib.ps_clip_adam_segment_chunks.argtypes = [ctypes.c_void_p, ctypes.c_int64]
+    lib.ps_clip_adam_segment_chunks.restype = ctypes.c_int64
+    lib.ps_clip_adam_workspace_bytes.argtypes = [P(ClipAdamDesc), P(ctypes.c_size_t)]
+    lib.ps_clip_adam_workspace_bytes.restype = ctypes.c_int
+    lib.ps_clip_adam_step.argtypes = [P(ClipAdamDesc), ctypes.c_void_p, P(ClipAdamState), ctypes.c_void_p,
+                                      ctypes.c_size_t, ctypes.c_void_p]
+    lib.ps_clip_adam_step.restype = ctypes.c_int
     for f in ("ps_raster_sizes_query", "ps_raster_layout_query", "ps_raster_forward", "ps_raster_backward"):
         getattr(lib, f).restype = ctypes.c_int
     return lib

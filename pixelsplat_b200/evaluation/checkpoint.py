@@ -28,3 +28,33 @@ def load_checkpoint(path: Union[Path, str], encoder: nn.Module) -> int:
                          "a pixelSplat checkpoint holds encoder weights only")
     encoder.load_state_dict({k[len(PREFIX):]: v for k, v in state.items()}, strict=True)
     return int(ckpt.get("global_step", 0))
+
+
+def read_checkpoint(path: Union[Path, str]) -> dict:
+    """The whole checkpoint dictionary, read with `weights_only=True` (what a resumed training needs beside the
+    weights: `global_step`, `epoch`, `optimizer_states`, `rng_state`)."""
+    ckpt = torch.load(path, map_location="cpu", weights_only=True)
+    if not isinstance(ckpt, dict) or "state_dict" not in ckpt:
+        raise ValueError(f"read_checkpoint: {path} is not a Lightning checkpoint (no 'state_dict')")
+    return ckpt
+
+
+def save_checkpoint(path: Union[Path, str], encoder: nn.Module, global_step: int, epoch: int = 0,
+                    optimizer_state: dict | None = None, lr_scheduler_state: dict | None = None,
+                    rng_state: dict | None = None) -> Path:
+    """Writes a checkpoint in Lightning's layout, the one `load_checkpoint` reads: `state_dict` holds the encoder's
+    entries under `encoder.`, `optimizer_states` / `lr_schedulers` one entry each when given.  Only tensors and
+    plain Python values go in, so `weights_only=True` loads it.  The file is written under a temporary name in the
+    same directory and renamed into place: a reader never sees half a checkpoint."""
+    path = Path(path)
+    path.parent.mkdir(parents=True, exist_ok=True)
+    ckpt = {"epoch": int(epoch), "global_step": int(global_step),
+            "state_dict": {PREFIX + k: v.detach().cpu() for k, v in encoder.state_dict().items()},
+            "optimizer_states": [] if optimizer_state is None else [optimizer_state],
+            "lr_schedulers": [] if lr_scheduler_state is None else [lr_scheduler_state]}
+    if rng_state is not None:
+        ckpt["rng_state"] = rng_state
+    tmp = path.with_name(path.name + ".tmp")
+    torch.save(ckpt, tmp)
+    tmp.replace(path)
+    return path
