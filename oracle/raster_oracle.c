@@ -26,6 +26,7 @@
  *   orc_preprocess        SURVEY A.1 + A.4   (upstream forward.cu preprocessCUDA)
  *   orc_bin               SURVEY A.2         (duplicateWithKeys + radix sort + identifyTileRanges)
  *   orc_composite_fwd     SURVEY A.3         (upstream forward.cu renderCUDA)
+ *   orc_composite_margins per pixel, how close the forward's walk came to taking another branch
  *   orc_composite_bwd     SURVEY A.5         (upstream backward.cu renderCUDA)
  *   orc_preprocess_bwd    SURVEY A.5         (computeCov2DCUDA + preprocessCUDA backward)
  */
@@ -361,6 +362,60 @@ void orc_composite_fwd(int W, int H, const uint32_t *ranges, const uint32_t *val
             final_T[pix] = T;
             n_contrib[pix] = last;
             for (int ch = 0; ch < 3; ++ch) out_color[ch * H * W + pix] = C[ch] + T * bg[ch];
+        }
+}
+
+/*
+ * orc_composite_margins: how close each pixel's walk came to taking another branch.  Walks the list exactly as
+ * orc_composite_fwd does, up to and including the entry at which it breaks, and writes per pixel [H, W] the
+ * smallest distance of each decision value from its threshold over the entries it looked at:
+ *   m_alpha  min |alpha / (1/255) - 1|   (alpha after min(0.99, .), over entries that reach the alpha test)
+ *   m_T      min |test_T / 1e-4 - 1|     (over entries that reach the T test, the breaking one included)
+ *   m_power  min |power|                 (over entries whose sign test can matter: power > 0, or power within
+ *            ORC_POWER_REL of zero relative to the products it is a difference of, |co| dx^2 ...; that is as far
+ *            as a float32 evaluation in another order or with FMAs can move it across 0.  The margin itself is
+ *            absolute, because the threshold is 0 and an implementation may place its test a fixed distance
+ *            above 0 to keep such rounding from dropping a pixel that sits on a Gaussian's centre: the
+ *            warp-task compositor rejects at log2-power > 1e-4.  A positive power of a positive-definite conic
+ *            is a rounding artefact, so every positive value counts.  dx = dy = 0 does not: every product is
+ *            then exactly 0 and so is the power, whatever the order.)
+ * A margin no entry contributed to is ORC_NO_MARGIN.
+ */
+#define ORC_POWER_REL 1.0e-5
+#define ORC_NO_MARGIN 1.0e30
+void orc_composite_margins(int W, int H, const uint32_t *ranges, const uint32_t *values, const real *xy,
+                           const real *conic_opacity, real *m_alpha, real *m_T, real *m_power) {
+    int gx = (W + TILE - 1) / TILE;
+    for (int py = 0; py < H; ++py)
+        for (int px = 0; px < W; ++px) {
+            int tile = (py / TILE) * gx + (px / TILE);
+            uint32_t s = ranges[2 * tile], e = ranges[2 * tile + 1];
+            real T = K(1), ma = K(ORC_NO_MARGIN), mt = K(ORC_NO_MARGIN), mp = K(ORC_NO_MARGIN);
+            real pxf = (real)px, pyf = (real)py;
+            for (uint32_t i = s; i < e; ++i) {
+                uint32_t g = values[i];
+                real dx = xy[2 * g] - pxf, dy = xy[2 * g + 1] - pyf;
+                const real *co = conic_opacity + 4 * g;
+                real power = K(-0.5) * (co[0] * dx * dx + co[2] * dy * dy) - co[1] * dx * dy;
+                real ax = co[0] * dx * dx, ay = co[2] * dy * dy, ab = co[1] * dx * dy;
+                real terms = K(0.5) * ((ax < K(0) ? -ax : ax) + (ay < K(0) ? -ay : ay)) + (ab < K(0) ? -ab : ab);
+                if (power > K(0) || (terms > K(0) && power >= K(-ORC_POWER_REL) * terms))
+                    mp = rmin(mp, power < K(0) ? -power : power);
+                if (power > K(0)) continue;
+                real alpha = rmin(K(0.99), co[3] * R_EXP(power));
+                real da = alpha / K(1.0 / 255.0) - K(1);
+                ma = rmin(ma, da < K(0) ? -da : da);
+                if (alpha < K(1.0 / 255.0)) continue;
+                real test_T = T * (K(1) - alpha);
+                real dt = test_T / K(0.0001) - K(1);
+                mt = rmin(mt, dt < K(0) ? -dt : dt);
+                if (test_T < K(0.0001)) break;
+                T = test_T;
+            }
+            int pix = py * W + px;
+            m_alpha[pix] = ma;
+            m_T[pix] = mt;
+            m_power[pix] = mp;
         }
 }
 

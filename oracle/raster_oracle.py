@@ -214,6 +214,61 @@ def backward(fwd: Forward, dL_dcolor_img, means, cov6, sh, viewmatrix, projmatri
     return Backward(d_means, d_cov6, d_sh, cl, c(d_opac), m2, cn)
 
 
+@dataclass
+class Margins:
+    """Per pixel [H, W]: the smallest distance of a decision value from its threshold over the entries the forward
+    looked at (orc_composite_margins).  `alpha` and `T` are relative to the threshold (1/255, 1e-4).  `power` is
+    |power| of the entries whose sign test could go either way (positive, or zero to within rounding of the products
+    it is a difference of); it is absolute because its threshold is 0 and an implementation may test a fixed
+    distance above 0 instead, as the warp-task compositor does.  NO_MARGIN where no entry reached the decision."""
+    alpha: np.ndarray
+    T: np.ndarray
+    power: np.ndarray
+
+
+NO_MARGIN = 1.0e30
+POWER_DELTA = 1.0e-4     # absolute; covers the warp-task compositor's `log2-power > 1e-4` form of `power > 0`
+
+
+def decision_margins(fwd: Forward, W, H) -> Margins:
+    """The decision margins of `fwd`'s composite, in fwd's precision, from its per-Gaussian records and list."""
+    dtype = fwd.color.dtype
+    m = Margins(*(np.zeros((H, W), dtype) for _ in range(3)))
+    values = fwd.binned.values if fwd.binned.values.size else np.zeros(1, np.uint32)
+    _lib(dtype).orc_composite_margins(int(W), int(H), _p(fwd.binned.ranges), _p(values), _p(fwd.pre.xy),
+                                      _p(fwd.pre.conic_opacity), _p(m.alpha), _p(m.T), _p(m.power))
+    return m
+
+
+def unsettled_kinds(m: Margins, delta: float, power_delta: float = POWER_DELTA) -> dict:
+    """{"alpha", "T", "power"} -> bool [H, W]: the pixels with a decision of that kind within the margin."""
+    return dict(alpha=m.alpha <= delta, T=m.T <= delta, power=m.power <= power_delta)
+
+
+def settled_mask(m: Margins, delta: float, power_delta: float = POWER_DELTA) -> np.ndarray:
+    """bool [H, W]: every decision the pixel's walk took is further than `delta` (relative; `power_delta`
+    absolute for `power > 0`) from its threshold, so an implementation whose decision values agree with the
+    oracle's to within that takes the same branches and must agree on n_contrib and, to rounding, on the rest."""
+    k = unsettled_kinds(m, delta, power_delta)
+    return ~(k["alpha"] | k["T"] | k["power"])
+
+
+def composite64_on_records(fwd: Forward, bg, W, H) -> Forward:
+    """The float64 composite on `fwd`'s (float32) per-Gaussian records and binned list, widened: a high-precision
+    reference of the composite alone that shares every front-end decision (radii, tile rectangles, list order,
+    colour clamps) with whatever produced those records."""
+    w = lambda a: np.ascontiguousarray(a, np.float64)
+    p = fwd.pre
+    pre = Preprocessed(w(p.depth), p.radii, w(p.xy), w(p.conic_opacity), w(p.rgb), p.clamped, p.rect,
+                       p.tiles_touched)
+    color, final_T, n_contrib = np.zeros((3, H, W)), np.zeros((H, W)), np.zeros((H, W), np.uint32)
+    values = fwd.binned.values if fwd.binned.values.size else np.zeros(1, np.uint32)
+    _lib(np.float64).orc_composite_fwd(int(W), int(H), _p(fwd.binned.ranges), _p(values), _p(pre.xy),
+                                       _p(pre.conic_opacity), _p(pre.rgb), _p(w(bg).reshape(3)), _p(color),
+                                       _p(final_T), _p(n_contrib))
+    return Forward(pre, fwd.binned, color, final_T, n_contrib)
+
+
 def upstream_key_list(binned: Binned):
     """(keys, values) exactly as upstream's sorted binning buffers hold them."""
     return binned.keys, binned.values
