@@ -380,7 +380,9 @@ PS_API int ps_epipolar_attention_forward(const ps_epipolar_desc *desc, const ps_
                                          float *z, float *e, float *mass, float *lse, void *stream);
 
 /* d_row [N,heads] = dz.z + de.e (+ dmass.mass).  dfeatures [b,v,grid_h,grid_w,128] must be
- * zero-initialised by the caller; the kernel accumulates into it atomically. */
+ * zero-initialised by the caller; the kernel accumulates into it atomically.  Like the forward, it returns
+ * PS_ERR_INVALID_ARGUMENT for a NULL required pointer, in->q_pe included when pe_dim > 0, before anything is
+ * enqueued. */
 PS_API int ps_epipolar_attention_backward(const ps_epipolar_desc *desc, const ps_epipolar_inputs *in,
                                           const float *lse, const float *dz, const float *de,
                                           const float *dmass, const float *d_row, float *dq_feat,

@@ -16,6 +16,8 @@
 // stay GEMMs.  One warp per query; lane l owns channels 4l..4l+3 for the gather and sample l
 // for the soft-max / PE.  C = 128, S <= 32.
 #include <cstdlib>
+#include <initializer_list>
+#include <type_traits>
 
 #include "ps_common.cuh"
 
@@ -44,13 +46,14 @@ struct Taps {
     float w[4];
 };
 
-__device__ __forceinline__ Taps make_taps(float x, float y, int h, int w) {
+// (x0, y0) receives the cell's top-left tap, which may lie outside the map.
+__device__ __forceinline__ Taps make_taps(float x, float y, int h, int w, int &x0, int &y0) {
     const float ix = x * (float)w - 0.5f, iy = y * (float)h - 0.5f;
     const float fx0 = floorf(ix), fy0 = floorf(iy);
     const float ax = ix - fx0, ay = iy - fy0;
     // clamp before the int cast so wild coordinates cannot overflow; they are outside anyway
-    const int x0 = (int)fminf(fmaxf(fx0, -2.0f), (float)w + 1.0f);
-    const int y0 = (int)fminf(fmaxf(fy0, -2.0f), (float)h + 1.0f);
+    x0 = (int)fminf(fmaxf(fx0, -2.0f), (float)w + 1.0f);
+    y0 = (int)fminf(fmaxf(fy0, -2.0f), (float)h + 1.0f);
     Taps t;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
@@ -60,32 +63,6 @@ __device__ __forceinline__ Taps make_taps(float x, float y, int h, int w) {
         t.w[k] = ((k & 1) ? ax : 1.0f - ax) * ((k >> 1) ? ay : 1.0f - ay);
     }
     return t;
-}
-
-// Sum over the 32 lanes of 32 per-lane values v[0..31]; lane l receives sum_lanes v[l].
-__device__ __forceinline__ float transpose_reduce32(float (&v)[32], int lane) {
-#pragma unroll
-    for (int half = 16; half >= 1; half >>= 1) {
-        const bool up = (lane & half) != 0;
-#pragma unroll
-        for (int i = 0; i < half; ++i) {
-            const float keep = up ? v[i + half] : v[i];
-            const float send = up ? v[i] : v[i + half];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, half);
-        }
-    }
-    return v[0];
-}
-
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-    return v;
-}
-__device__ __forceinline__ float warp_add(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
 }
 
 // PE(rd)[2k] = sin(f_k rd), [2k+1] = sin(f_k rd + pi/2), layout "(d f p)"
@@ -164,6 +141,134 @@ struct __align__(16) EpiWarpSmem {
     float aux[4][kMaxPE];    // backward: d_e
 };
 
+// ---- Shared by both kernels.  The backward recomputes the forward's probabilities as exp(score - lse), so both
+// must form the query, the samples and their scores with the same code.
+
+// Query n = (b V + v) R + r of the warp.
+struct EpiQuery {
+    int r, bv, v, b;         // bv = b V + v
+};
+
+// Decodes query n and loads its qt (lane = channels 4 lane .. 4 lane + 3) and its pq (into sm.pq; the caller's
+// __syncwarp publishes it).  The backward loads its own per-query rows in the same two loops: per_head(hd) after
+// qt_hd, per_pe(i) after entry i of the [HEADS, npe] pq row.
+template <int HEADS, class PerHead, class PerPe>
+__device__ __forceinline__ EpiQuery epi_query(const EpiParams &P, int n, int lane, EpiWarpSmem &sm,
+                                              float (&qt)[HEADS][4], PerHead &&per_head, PerPe &&per_pe) {
+    const int R = P.h * P.w;
+    EpiQuery q;
+    q.r = n % R; q.bv = n / R;
+    q.v = q.bv % P.V; q.b = q.bv / P.V;
+#pragma unroll
+    for (int hd = 0; hd < HEADS; ++hd) {
+        const float4 t = ldg4(P.qt + ((size_t)n * HEADS + hd) * kEpiC + 4 * lane);
+        qt[hd][0] = t.x; qt[hd][1] = t.y; qt[hd][2] = t.z; qt[hd][3] = t.w;
+        per_head(hd);
+    }
+    for (int i = lane; i < HEADS * P.npe; i += 32) {
+        sm.pq[i / P.npe][i % P.npe] = P.pq[(size_t)n * HEADS * P.npe + i];
+        per_pe(i);
+    }
+    return q;
+}
+
+// The query's ray in other view ov, which is view ov < v ? ov : ov + 1.
+struct EpiRay {
+    size_t ray;              // (bv OV + ov) R + r: the row of seg, valid and rd
+    float4 seg;
+    bool ok;                 // valid[ray]
+    int map;                 // b V + the other view: its feature map
+    size_t map_base;         // element offset of the lane's channels in that map
+};
+
+__device__ __forceinline__ EpiRay epi_ray(const EpiParams &P, const EpiQuery &q, int ov, int lane) {
+    const int R = P.h * P.w;
+    EpiRay y;
+    const int o_view = ov < q.v ? ov : ov + 1;
+    y.ray = ((size_t)(q.bv * P.OV + ov)) * R + q.r;
+    y.seg = ldg4(P.seg + 4 * y.ray);
+    y.ok = P.valid[y.ray] != 0;
+    y.map = q.b * P.V + o_view;
+    y.map_base = (size_t)y.map * R * kEpiC + 4 * lane;
+    return y;
+}
+
+// Lane = sample s = lane of the ray.  taps: its bilinear taps, none (offset -1, weight 0) past S or on an invalid
+// ray.  (bx, by): the top-left tap of its bilinear cell, (-2, -2) -- a cell that touches no texel -- where there are
+// no taps.  PE(rd_s) goes into pe and sm.pe[s] (zero past S), and the PE half of its scores plus the bias into
+// sm.scpe[s] (-inf past S).
+template <int HEADS>
+__device__ __forceinline__ void epi_sample(const EpiParams &P, const EpiRay &ray, int n, int ov, int lane,
+                                           EpiWarpSmem &sm, Taps &taps, int &bx, int &by, float (&pe)[kMaxPE]) {
+    const bool has_sample = lane < P.S;
+    if (has_sample && ray.ok) {
+        const float u = ((float)lane + 0.5f) / (float)P.S;
+        const float sx = ray.seg.x + u * (ray.seg.z - ray.seg.x), sy = ray.seg.y + u * (ray.seg.w - ray.seg.y);
+        taps = make_taps(sx, sy, P.h, P.w, bx, by);
+    } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) { taps.off[k] = -1; taps.w[k] = 0.0f; }
+        bx = by = -2;
+    }
+    positional_encoding(has_sample ? P.rd[ray.ray * P.S + lane] : 0.0f, P.npe, pe);
+#pragma unroll
+    for (int j = 0; j < kMaxPE; ++j)
+        if (j < P.npe) sm.pe[lane][j] = has_sample ? pe[j] : 0.0f;
+#pragma unroll
+    for (int hd = 0; hd < HEADS; ++hd) {
+        float sc = 0.0f;
+#pragma unroll
+        for (int j = 0; j < kMaxPE; ++j)
+            if (j < P.npe) sc += sm.pq[hd][j] * pe[j];
+        if (P.bias) sc += P.bias[((size_t)n * HEADS + hd) * P.OV + ov];
+        sm.scpe[lane][hd] = has_sample ? sc : -INFINITY;
+    }
+}
+
+// f[i] = channels 4 lane .. 4 lane + 3 of sample sub SUB + i, gathered from the map at fmap.
+template <int SUB>
+__device__ __forceinline__ void epi_gather(const float *fmap, const Taps &my_taps, int sub, float (&f)[SUB][4]) {
+#pragma unroll
+    for (int i = 0; i < SUB; ++i) {
+        const int s = sub * SUB + i;
+        f[i][0] = f[i][1] = f[i][2] = f[i][3] = 0.0f;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            // the taps of sample s were formed once, by lane s (every lane needs the same four)
+            const int off = __shfl_sync(0xffffffffu, my_taps.off[k], s);
+            const float wk = __shfl_sync(0xffffffffu, my_taps.w[k], s);
+            if (off >= 0) {
+                const float4 a = ldg4(fmap + off);
+                f[i][0] += wk * a.x; f[i][1] += wk * a.y;
+                f[i][2] += wk * a.z; f[i][3] += wk * a.w;
+            }
+        }
+    }
+}
+
+// For the lane's sample s_mine = sub SUB + (lane & (SUB - 1)) of a sub-chunk: x . f over the 128 channels plus
+// pe_half[s_mine][hd].  With qt_hd and sm.scpe this is the sample's score (-inf past S); the backward forms d a
+// from dz_hd and sm.dape the same way.
+template <int SUB>
+__device__ __forceinline__ float epi_sub_dot(const float (&x)[4], const float (&f)[SUB][4],
+                                             const float (&pe_half)[32][4], int s_mine, int hd, int lane) {
+    float part[SUB];
+#pragma unroll
+    for (int i = 0; i < SUB; ++i) part[i] = x[0] * f[i][0] + x[1] * f[i][1] + x[2] * f[i][2] + x[3] * f[i][3];
+    return transpose_reduce_sub<SUB>(part, lane) + pe_half[s_mine][hd];
+}
+
+// The lane's entries of a query's [HEADS, npe] row (e, dpq; HEADS npe <= 96): fn(i, o, head, pe index) for each
+// o = lane + 32 i < HEADS npe.
+template <int HEADS, class Fn>
+__device__ __forceinline__ void for_lane_pe_entries(int npe, int lane, Fn &&fn) {
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        const int o = lane + 32 * i;
+        if (o < HEADS * npe) fn(i, o, o / npe, o % npe);
+    }
+}
+
 template <int HEADS, int SUB>
 __global__ void __launch_bounds__(kEpiWarps * 32, 4)
 k_epi_attn_fwd(EpiParams P, int n_queries, float *__restrict__ z_out, float *__restrict__ e_out,
@@ -173,18 +278,8 @@ k_epi_attn_fwd(EpiParams P, int n_queries, float *__restrict__ z_out, float *__r
     EpiWarpSmem &sm = sm_all[warp];
     const int n = blockIdx.x * kEpiWarps + warp;
     if (n >= n_queries) return;
-    const int R = P.h * P.w;
-    const int r = n % R, bv = n / R;
-    const int v = bv % P.V, b = bv / P.V;
-
     float qt[HEADS][4];
-#pragma unroll
-    for (int hd = 0; hd < HEADS; ++hd) {
-        const float4 q = ldg4(P.qt + ((size_t)n * HEADS + hd) * kEpiC + 4 * lane);
-        qt[hd][0] = q.x; qt[hd][1] = q.y; qt[hd][2] = q.z; qt[hd][3] = q.w;
-    }
-    for (int i = lane; i < HEADS * P.npe; i += 32)
-        sm.pq[i / P.npe][i % P.npe] = P.pq[(size_t)n * HEADS * P.npe + i];
+    const EpiQuery q = epi_query<HEADS>(P, n, lane, sm, qt, [](int) {}, [](int) {});
     __syncwarp();
 
     float m_run[HEADS], l_run[HEADS], z[HEADS][4], e_acc[3];   // e_acc: outputs lane, lane+32, lane+64
@@ -196,78 +291,24 @@ k_epi_attn_fwd(EpiParams P, int n_queries, float *__restrict__ z_out, float *__r
     }
     e_acc[0] = e_acc[1] = e_acc[2] = 0.0f;
     const int nsub = (P.S + SUB - 1) / SUB;
-    const int total_e = HEADS * P.npe;
 
     for (int ov = 0; ov < P.OV; ++ov) {
-        const int o_view = ov < v ? ov : ov + 1;
-        const size_t ray = ((size_t)(bv * P.OV + ov)) * R + r;
-        const float4 sg = ldg4(P.seg + 4 * ray);
-        const bool ok = P.valid[ray] != 0;
-        const float *fmap = P.feat + (size_t)(b * P.V + o_view) * R * kEpiC + 4 * lane;
-
-        // ---- PE half of the scores and the bilinear taps, lane = sample
+        const EpiRay ray = epi_ray(P, q, ov, lane);
         Taps my_taps;
-        int my_cell = -0x7ffffffe;
-        {
-            float pe[kMaxPE];
-            const bool has_sample = lane < P.S;
-            if (has_sample && ok) {
-                const float u = ((float)lane + 0.5f) / (float)P.S;
-                const float sx = sg.x + u * (sg.z - sg.x), sy = sg.y + u * (sg.w - sg.y);
-                my_taps = make_taps(sx, sy, P.h, P.w);
-                const float ix = sx * (float)P.w - 0.5f, iy = sy * (float)P.h - 0.5f;
-                const int bx = (int)fminf(fmaxf(floorf(ix), -2.0f), (float)P.w + 1.0f);
-                const int by = (int)fminf(fmaxf(floorf(iy), -2.0f), (float)P.h + 1.0f);
-                my_cell = by * (P.w + 4) + bx;            // the bilinear cell (backward merges samples that share it)
-            } else {
-#pragma unroll
-                for (int k = 0; k < 4; ++k) { my_taps.off[k] = -1; my_taps.w[k] = 0.0f; }
-            }
-            positional_encoding(has_sample ? P.rd[ray * P.S + lane] : 0.0f, P.npe, pe);
-#pragma unroll
-            for (int j = 0; j < kMaxPE; ++j)
-                if (j < P.npe) sm.pe[lane][j] = has_sample ? pe[j] : 0.0f;
-#pragma unroll
-            for (int hd = 0; hd < HEADS; ++hd) {
-                float sc = 0.0f;
-#pragma unroll
-                for (int j = 0; j < kMaxPE; ++j)
-                    if (j < P.npe) sc += sm.pq[hd][j] * pe[j];
-                if (P.bias) sc += P.bias[((size_t)n * HEADS + hd) * P.OV + ov];
-                sm.scpe[lane][hd] = has_sample ? sc : -INFINITY;
-            }
-        }
+        int bx, by;
+        float pe[kMaxPE];
+        epi_sample<HEADS>(P, ray, n, ov, lane, sm, my_taps, bx, by, pe);
         __syncwarp();
 
         for (int sub = 0; sub < nsub; ++sub) {
-            // ---- gather SUB samples (channels 4*lane..4*lane+3 of each)
             float f[SUB][4];
-#pragma unroll
-            for (int i = 0; i < SUB; ++i) {
-                const int s = sub * SUB + i;
-                f[i][0] = f[i][1] = f[i][2] = f[i][3] = 0.0f;
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    // the taps of sample s were formed once, by lane s (every lane needs the same four)
-                    const int off = __shfl_sync(0xffffffffu, my_taps.off[k], s);
-                    const float wk = __shfl_sync(0xffffffffu, my_taps.w[k], s);
-                    if (off >= 0) {
-                        const float4 a = ldg4(fmap + off);
-                        f[i][0] += wk * a.x; f[i][1] += wk * a.y;
-                        f[i][2] += wk * a.z; f[i][3] += wk * a.w;
-                    }
-                }
-            }
+            epi_gather<SUB>(P.feat + ray.map_base, my_taps, sub, f);
             // ---- scores: every lane ends up with the score of sample sub*SUB + (lane & (SUB-1))
             const int s_mine = sub * SUB + (lane & (SUB - 1));
             float scale_old[HEADS];
 #pragma unroll
             for (int hd = 0; hd < HEADS; ++hd) {
-                float part[SUB];
-#pragma unroll
-                for (int i = 0; i < SUB; ++i)
-                    part[i] = qt[hd][0] * f[i][0] + qt[hd][1] * f[i][1] + qt[hd][2] * f[i][2] + qt[hd][3] * f[i][3];
-                const float sc = transpose_reduce_sub<SUB>(part, lane) + sm.scpe[s_mine][hd];   // -inf beyond S
+                const float sc = epi_sub_dot<SUB>(qt[hd], f, sm.scpe, s_mine, hd, lane);   // -inf beyond S
                 const float m_new = fmaxf(m_run[hd], group_max<SUB>(sc));     // >= one finite score per sub-chunk
                 scale_old[hd] = __expf(m_run[hd] - m_new);                     // exp(-inf) = 0 on the first one
                 const float pnum = __expf(sc - m_new);                         // exp(-inf) = 0 beyond S
@@ -294,21 +335,16 @@ k_epi_attn_fwd(EpiParams P, int n_queries, float *__restrict__ z_out, float *__r
                     z[hd][2] += pw[hd] * f[i][2]; z[hd][3] += pw[hd] * f[i][3];
                 }
             }
-            // e[h][j] = sum_s p[s][h] * pe[s][j]; output index o = lane + 32*i -> (h, j) = (o / npe, o % npe)
+            // e[h][j] = sum_s p[s][h] * pe[s][j]
+            for_lane_pe_entries<HEADS>(P.npe, lane, [&](int i3, int, int hd, int j) {
+                float acc = 0.0f;
 #pragma unroll
-            for (int i3 = 0; i3 < 3; ++i3) {
-                const int o = lane + 32 * i3;
-                if (o < total_e) {
-                    const int hd = o / P.npe, j = o % P.npe;
-                    float acc = 0.0f;
+                for (int i = 0; i < SUB; ++i) acc += sm.p[i][hd] * sm.pe[sub * SUB + i][j];
+                float so = 0.0f;
 #pragma unroll
-                    for (int i = 0; i < SUB; ++i) acc += sm.p[i][hd] * sm.pe[sub * SUB + i][j];
-                    float so = 0.0f;
-#pragma unroll
-                    for (int q = 0; q < HEADS; ++q) so = (q == hd) ? scale_old[q] : so;
-                    e_acc[i3] = e_acc[i3] * so + acc;
-                }
-            }
+                for (int k = 0; k < HEADS; ++k) so = (k == hd) ? scale_old[k] : so;
+                e_acc[i3] = e_acc[i3] * so + acc;
+            });
             __syncwarp();
         }
     }
@@ -322,17 +358,12 @@ k_epi_attn_fwd(EpiParams P, int n_queries, float *__restrict__ z_out, float *__r
         if (lane == 0) lse_out[(size_t)n * HEADS + hd] = m_run[hd] + __logf(l_run[hd]);
         if (mass_out && lane < P.OV) mass_out[((size_t)n * HEADS + hd) * P.OV + lane] = mass_acc[hd] * inv;
     }
+    for_lane_pe_entries<HEADS>(P.npe, lane, [&](int i3, int o, int hd, int) {
+        float lr = 1.0f;
 #pragma unroll
-    for (int i3 = 0; i3 < 3; ++i3) {
-        const int o = lane + 32 * i3;
-        if (o < total_e) {
-            const int hd = o / P.npe;
-            float lr = 1.0f;
-#pragma unroll
-            for (int q = 0; q < HEADS; ++q) lr = (q == hd) ? l_run[q] : lr;
-            e_out[(size_t)n * total_e + o] = e_acc[i3] / lr;
-        }
-    }
+        for (int k = 0; k < HEADS; ++k) lr = (k == hd) ? l_run[k] : lr;
+        e_out[(size_t)n * (HEADS * P.npe) + o] = e_acc[i3] / lr;
+    });
 }
 
 // Slot records of the fixed-order d(feature map) (ps_epipolar_attention_backward_deterministic).  Slot
@@ -367,82 +398,44 @@ k_epi_attn_bwd(EpiParams P, int n_queries, const float *__restrict__ lse, const 
     EpiWarpSmem &sm = sm_all[warp];
     const int n = blockIdx.x * kEpiWarps + warp;
     if (n >= n_queries) return;
-    const int R = P.h * P.w;
-    const int r = n % R, bv = n / R;
-    const int v = bv % P.V, b = bv / P.V;
-
     float qt[HEADS][4], gz[HEADS][4], dq[HEADS][4], lse_h[HEADS], D_h[HEADS];
-#pragma unroll
-    for (int hd = 0; hd < HEADS; ++hd) {
-        const size_t o = ((size_t)n * HEADS + hd) * kEpiC + 4 * lane;
-        const float4 q = ldg4(P.qt + o), g = ldg4(dz + o);
-        qt[hd][0] = q.x; qt[hd][1] = q.y; qt[hd][2] = q.z; qt[hd][3] = q.w;
+    const EpiQuery q = epi_query<HEADS>(P, n, lane, sm, qt, [&](int hd) {
+        const float4 g = ldg4(dz + ((size_t)n * HEADS + hd) * kEpiC + 4 * lane);
         gz[hd][0] = g.x; gz[hd][1] = g.y; gz[hd][2] = g.z; gz[hd][3] = g.w;
         dq[hd][0] = dq[hd][1] = dq[hd][2] = dq[hd][3] = 0.0f;
         lse_h[hd] = lse[(size_t)n * HEADS + hd];
         D_h[hd] = Drow[(size_t)n * HEADS + hd];
-    }
-    for (int i = lane; i < HEADS * P.npe; i += 32) {
-        sm.pq[i / P.npe][i % P.npe] = P.pq[(size_t)n * HEADS * P.npe + i];
-        sm.aux[i / P.npe][i % P.npe] = de[(size_t)n * HEADS * P.npe + i];
-    }
+    }, [&](int i) { sm.aux[i / P.npe][i % P.npe] = de[(size_t)n * HEADS * P.npe + i]; });
     __syncwarp();
     float dpq_acc[3] = {0.0f, 0.0f, 0.0f};
     const int nsub = (P.S + SUB - 1) / SUB;
 
     for (int ov = 0; ov < P.OV; ++ov) {
-        const int o_view = ov < v ? ov : ov + 1;
-        const size_t ray = ((size_t)(bv * P.OV + ov)) * R + r;
-        const float4 sg = ldg4(P.seg + 4 * ray);
-        const bool ok = P.valid[ray] != 0;
-        const size_t map_base = (size_t)(b * P.V + o_view) * R * kEpiC + 4 * lane;
-        const float *fmap = P.feat + map_base;
-
-        // ---- PE halves of the score and of d a, and the bilinear taps, lane = sample
+        const EpiRay ray = epi_ray(P, q, ov, lane);
         Taps my_taps;
-        int my_cell = -0x7ffffffe;
-        unsigned my_key = det.n_cells;                    // DET only: the sentinel unless the cell touches the map
-        {
-            float pe[kMaxPE];
-            const bool has_sample = lane < P.S;
-            if (has_sample && ok) {
-                const float u = ((float)lane + 0.5f) / (float)P.S;
-                const float sx = sg.x + u * (sg.z - sg.x), sy = sg.y + u * (sg.w - sg.y);
-                my_taps = make_taps(sx, sy, P.h, P.w);
-                const float ix = sx * (float)P.w - 0.5f, iy = sy * (float)P.h - 0.5f;
-                const int bx = (int)fminf(fmaxf(floorf(ix), -2.0f), (float)P.w + 1.0f);
-                const int by = (int)fminf(fmaxf(floorf(iy), -2.0f), (float)P.h + 1.0f);
-                my_cell = by * (P.w + 4) + bx;            // the bilinear cell (backward merges samples that share it)
-                if constexpr (DET) {
-                    if (bx >= -1 && bx < P.w && by >= -1 && by < P.h)
-                        my_key = (unsigned)(((b * P.V + o_view) * (P.h + 1) + by + 1) * (P.w + 1) + bx + 1);
-                }
-            } else {
+        int bx, by;
+        float pe[kMaxPE];
+        epi_sample<HEADS>(P, ray, n, ov, lane, sm, my_taps, bx, by, pe);
+        // ---- PE half of d a (+ dmass), beside the score's
 #pragma unroll
-                for (int k = 0; k < 4; ++k) { my_taps.off[k] = -1; my_taps.w[k] = 0.0f; }
-            }
-            if constexpr (DET) {
-                if (has_sample) {
-                    const size_t t = ((size_t)n * P.OV + ov) * P.S + lane;
-                    det.key[t] = my_key;
-                    if (my_key != det.n_cells) det.w[t] = make_float4(my_taps.w[0], my_taps.w[1], my_taps.w[2], my_taps.w[3]);
-                }
-            }
-            positional_encoding(has_sample ? P.rd[ray * P.S + lane] : 0.0f, P.npe, pe);
+        for (int hd = 0; hd < HEADS; ++hd) {
+            float da = 0.0f;
 #pragma unroll
             for (int j = 0; j < kMaxPE; ++j)
-                if (j < P.npe) sm.pe[lane][j] = has_sample ? pe[j] : 0.0f;
-#pragma unroll
-            for (int hd = 0; hd < HEADS; ++hd) {
-                float sc = 0.0f, da = 0.0f;
-#pragma unroll
-                for (int j = 0; j < kMaxPE; ++j)
-                    if (j < P.npe) { sc += sm.pq[hd][j] * pe[j]; da += sm.aux[hd][j] * pe[j]; }
-                if (P.bias) sc += P.bias[((size_t)n * HEADS + hd) * P.OV + ov];
-                if (dmass) da += dmass[((size_t)n * HEADS + hd) * P.OV + ov];
-                sm.scpe[lane][hd] = has_sample ? sc : -INFINITY;
-                sm.dape[lane][hd] = da;
-                sm.ds_all[lane][hd] = 0.0f;
+                if (j < P.npe) da += sm.aux[hd][j] * pe[j];
+            if (dmass) da += dmass[((size_t)n * HEADS + hd) * P.OV + ov];
+            sm.dape[lane][hd] = da;
+            sm.ds_all[lane][hd] = 0.0f;
+        }
+        const int my_cell = by * (P.w + 4) + bx;          // the bilinear cell (samples that share it are merged)
+        unsigned my_key = det.n_cells;                    // DET only: the sentinel unless the cell touches the map
+        if constexpr (DET) {
+            if (bx >= -1 && bx < P.w && by >= -1 && by < P.h)
+                my_key = (unsigned)((ray.map * (P.h + 1) + by + 1) * (P.w + 1) + bx + 1);
+            if (lane < P.S) {
+                const size_t t = ((size_t)n * P.OV + ov) * P.S + lane;
+                det.key[t] = my_key;
+                if (my_key != det.n_cells) det.w[t] = make_float4(my_taps.w[0], my_taps.w[1], my_taps.w[2], my_taps.w[3]);
             }
         }
         __syncwarp();
@@ -459,7 +452,7 @@ k_epi_attn_bwd(EpiParams P, int n_queries, const float *__restrict__ lse, const 
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 if (tap_off[k] >= 0)
-                    atomicAdd(reinterpret_cast<float4 *>(dfeat + map_base + tap_off[k]),
+                    atomicAdd(reinterpret_cast<float4 *>(dfeat + ray.map_base + tap_off[k]),
                               make_float4(tap_acc[k][0], tap_acc[k][1], tap_acc[k][2], tap_acc[k][3]));
                 tap_acc[k][0] = tap_acc[k][1] = tap_acc[k][2] = tap_acc[k][3] = 0.0f;
             }
@@ -467,34 +460,12 @@ k_epi_attn_bwd(EpiParams P, int n_queries, const float *__restrict__ lse, const 
 
         for (int sub = 0; sub < nsub; ++sub) {
             float f[SUB][4];
-#pragma unroll
-            for (int i = 0; i < SUB; ++i) {
-                const int s = sub * SUB + i;
-                f[i][0] = f[i][1] = f[i][2] = f[i][3] = 0.0f;
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    // the taps of sample s were formed once, by lane s (every lane needs the same four)
-                    const int off = __shfl_sync(0xffffffffu, my_taps.off[k], s);
-                    const float wk = __shfl_sync(0xffffffffu, my_taps.w[k], s);
-                    if (off >= 0) {
-                        const float4 a = ldg4(fmap + off);
-                        f[i][0] += wk * a.x; f[i][1] += wk * a.y;
-                        f[i][2] += wk * a.z; f[i][3] += wk * a.w;
-                    }
-                }
-            }
+            epi_gather<SUB>(P.feat + ray.map_base, my_taps, sub, f);
             const int s_mine = sub * SUB + (lane & (SUB - 1));
 #pragma unroll
             for (int hd = 0; hd < HEADS; ++hd) {
-                float part[SUB];
-#pragma unroll
-                for (int i = 0; i < SUB; ++i)
-                    part[i] = qt[hd][0] * f[i][0] + qt[hd][1] * f[i][1] + qt[hd][2] * f[i][2] + qt[hd][3] * f[i][3];
-                const float sc = transpose_reduce_sub<SUB>(part, lane) + sm.scpe[s_mine][hd];
-#pragma unroll
-                for (int i = 0; i < SUB; ++i)
-                    part[i] = gz[hd][0] * f[i][0] + gz[hd][1] * f[i][1] + gz[hd][2] * f[i][2] + gz[hd][3] * f[i][3];
-                const float da = transpose_reduce_sub<SUB>(part, lane) + sm.dape[s_mine][hd];
+                const float sc = epi_sub_dot<SUB>(qt[hd], f, sm.scpe, s_mine, hd, lane);
+                const float da = epi_sub_dot<SUB>(gz[hd], f, sm.dape, s_mine, hd, lane);
                 const float a = __expf(sc - lse_h[hd]);                 // 0 beyond S (score -inf)
                 const float dsc = a * (da - D_h[hd]);
                 if (lane < SUB) {
@@ -523,12 +494,12 @@ k_epi_attn_bwd(EpiParams P, int n_queries, const float *__restrict__ lse, const 
                     }
                 }
                 if constexpr (DET) {
-                    if (s < P.S && ok) {
+                    if (s < P.S && ray.ok) {
                         if (__shfl_sync(0xffffffffu, my_key, s) != det.n_cells)
                             *reinterpret_cast<float4 *>(det.df + (((size_t)n * P.OV + ov) * P.S + s) * kEpiC + 4 * lane) =
                                 make_float4(df[0], df[1], df[2], df[3]);
                     }
-                } else if (s < P.S && ok) {
+                } else if (s < P.S && ray.ok) {
                     Taps t;
 #pragma unroll
                     for (int k = 0; k < 4; ++k) {
@@ -558,56 +529,66 @@ k_epi_attn_bwd(EpiParams P, int n_queries, const float *__restrict__ lse, const 
             for (int hd = 0; hd < HEADS; ++hd) dbias_out[((size_t)n * HEADS + hd) * P.OV + ov] = dbias_acc[hd];
         }
         // dpq[h][j] += sum_s ds[s][h] pe[s][j]
-        {
-            const int total = HEADS * P.npe;
-#pragma unroll
-            for (int i = 0; i < 3; ++i) {
-                const int o = lane + 32 * i;
-                if (o < total) {
-                    const int hd = o / P.npe, j = o % P.npe;
-                    float acc = 0.0f;
-                    for (int s = 0; s < 32; ++s) acc += sm.ds_all[s][hd] * sm.pe[s][j];
-                    dpq_acc[i] += acc;
-                }
-            }
-        }
+        for_lane_pe_entries<HEADS>(P.npe, lane, [&](int i, int, int hd, int j) {
+            float acc = 0.0f;
+            for (int s = 0; s < 32; ++s) acc += sm.ds_all[s][hd] * sm.pe[s][j];
+            dpq_acc[i] += acc;
+        });
         __syncwarp();
     }
 #pragma unroll
     for (int hd = 0; hd < HEADS; ++hd)
         *reinterpret_cast<float4 *>(dqt_out + ((size_t)n * HEADS + hd) * kEpiC + 4 * lane) =
             make_float4(dq[hd][0], dq[hd][1], dq[hd][2], dq[hd][3]);
-    {
-        const int total = HEADS * P.npe;
-#pragma unroll
-        for (int i = 0; i < 3; ++i) {
-            const int o = lane + 32 * i;
-            if (o < total) dpq_out[(size_t)n * total + o] = dpq_acc[i];
-        }
-    }
+    for_lane_pe_entries<HEADS>(P.npe, lane,
+                               [&](int i, int o, int, int) { dpq_out[(size_t)n * (HEADS * P.npe) + o] = dpq_acc[i]; });
 }
 
 constexpr int kEpiSubFwd = 8, kEpiSubBwd = 4;
 
-template <int HEADS>
-static int launch_epi(bool backward, const EpiParams &P, int n, float *z, float *e, float *mass, float *lse_out,
-                      const float *lse, const float *dz, const float *de, const float *dmass, const float *Drow,
-                      float *dqt, float *dpq, float *dbias, float *dfeat, cudaStream_t st) {
-    const int blocks = (n + kEpiWarps - 1) / kEpiWarps;
-    if (!backward) {
-        static int sub_fwd = 0;                       // PIXELSPLAT_B200_EPI_SUB_FWD = 4 | 8 (A/B runs)
-        if (sub_fwd == 0) {
-            const char *e = getenv("PIXELSPLAT_B200_EPI_SUB_FWD");
-            sub_fwd = (e && e[0] == '4') ? 4 : kEpiSubFwd;
-        }
-        if (sub_fwd == 4) k_epi_attn_fwd<HEADS, 4><<<blocks, kEpiWarps * 32, 0, st>>>(P, n, z, e, mass, lse_out);
-        else k_epi_attn_fwd<HEADS, kEpiSubFwd><<<blocks, kEpiWarps * 32, 0, st>>>(P, n, z, e, mass, lse_out);
-        PS_LAUNCH_CHECK("k_epi_attn_fwd");
-    } else {
-        k_epi_attn_bwd<HEADS, kEpiSubBwd><<<blocks, kEpiWarps * 32, 0, st>>>(P, n, lse, dz, de, dmass, Drow, dqt, dpq, dbias, dfeat,
-                                                                             EpiDetRecords{});
-        PS_LAUNCH_CHECK("k_epi_attn_bwd");
+// fn(std::integral_constant<int, heads>()) for heads in [1, 4] (epi_check has checked the range).
+template <class Fn>
+static void with_heads(int heads, Fn &&fn) {
+    switch (heads) {
+        case 1: fn(std::integral_constant<int, 1>()); break;
+        case 2: fn(std::integral_constant<int, 2>()); break;
+        case 3: fn(std::integral_constant<int, 3>()); break;
+        default: fn(std::integral_constant<int, 4>()); break;
     }
+}
+
+static int launch_epi_fwd(const EpiParams &P, int heads, int n, float *z, float *e, float *mass, float *lse,
+                          cudaStream_t st) {
+    static int sub_fwd = 0;                           // PIXELSPLAT_B200_EPI_SUB_FWD = 4 | 8 (A/B runs)
+    if (sub_fwd == 0) {
+        const char *env = getenv("PIXELSPLAT_B200_EPI_SUB_FWD");
+        sub_fwd = (env && env[0] == '4') ? 4 : kEpiSubFwd;
+    }
+    const int blocks = (n + kEpiWarps - 1) / kEpiWarps;
+    with_heads(heads, [&](auto H) {
+        constexpr int HEADS = decltype(H)::value;
+        if (sub_fwd == 4) k_epi_attn_fwd<HEADS, 4><<<blocks, kEpiWarps * 32, 0, st>>>(P, n, z, e, mass, lse);
+        else k_epi_attn_fwd<HEADS, kEpiSubFwd><<<blocks, kEpiWarps * 32, 0, st>>>(P, n, z, e, mass, lse);
+    });
+    PS_LAUNCH_CHECK("k_epi_attn_fwd");
+    return PS_OK;
+}
+
+// The backward's cotangents and gradients, as its entry points take them.
+struct EpiGrads {
+    const float *lse, *dz, *de, *dmass, *d_row;
+    float *dq_feat, *dq_pe, *dbias, *dfeatures;
+};
+
+// DET: the slot records go to `det`, and dfeatures is left to the fixed-order sum that follows.
+template <bool DET>
+static int launch_epi_bwd(const EpiParams &P, int heads, int n, const EpiGrads &g, const EpiDetRecords &det,
+                          cudaStream_t st) {
+    with_heads(heads, [&](auto H) {
+        k_epi_attn_bwd<decltype(H)::value, kEpiSubBwd, DET><<<(n + kEpiWarps - 1) / kEpiWarps, kEpiWarps * 32, 0, st>>>(
+            P, n, g.lse, g.dz, g.de, g.dmass, g.d_row, g.dq_feat, g.dq_pe, g.dbias, DET ? nullptr : g.dfeatures, det);
+    });
+    PS_LAUNCH_CHECK(DET ? "k_epi_attn_bwd<DET>" : "k_epi_attn_bwd");
     return PS_OK;
 }
 
@@ -808,18 +789,15 @@ static int epi_det_layout(const ps_epipolar_desc *d, EpiDetLayout *L) {
     return PS_OK;
 }
 
-template <int HEADS>
-static int launch_epi_bwd_det(const EpiParams &P, int n, const EpiDetLayout &L, char *ws, const float *lse,
-                              const float *dz, const float *de, const float *dmass, const float *Drow, float *dqt,
-                              float *dpq, float *dbias, float *dfeat, cudaStream_t st) {
+static int launch_epi_bwd_det(const EpiParams &P, int heads, int n, const EpiDetLayout &L, char *ws,
+                              const EpiGrads &g, cudaStream_t st) {
     EpiDetRecords rec;
     rec.df = reinterpret_cast<float *>(ws + L.df);
     rec.w = reinterpret_cast<float4 *>(ws + L.w);
     rec.key = reinterpret_cast<unsigned *>(ws + L.key[0]);
     rec.n_cells = L.n_cells;
-    k_epi_attn_bwd<HEADS, kEpiSubBwd, true><<<(n + kEpiWarps - 1) / kEpiWarps, kEpiWarps * 32, 0, st>>>(
-        P, n, lse, dz, de, dmass, Drow, dqt, dpq, dbias, nullptr, rec);
-    PS_LAUNCH_CHECK("k_epi_attn_bwd<DET>");
+    const int rc = launch_epi_bwd<true>(P, heads, n, g, rec, st);
+    if (rc) return rc;
 
     const int T = (int)L.T;
     unsigned *hist = reinterpret_cast<unsigned *>(ws + L.hist);
@@ -847,7 +825,7 @@ static int launch_epi_bwd_det(const EpiParams &P, int n, const EpiDetLayout &L, 
     PS_LAUNCH_CHECK("k_epi_cell_sums");
     const int texels = P.B * P.V * P.h * P.w;
     k_epi_texel_finish<<<(texels + kCellWarps - 1) / kCellWarps, kCellWarps * 32, 0, st>>>(cell_sum, texels, P.h, P.w,
-                                                                                            dfeat);
+                                                                                            g.dfeatures);
     PS_LAUNCH_CHECK("k_epi_texel_finish");
     return PS_OK;
 }
@@ -868,6 +846,21 @@ static int epi_check(const ps_epipolar_desc *d) {
     return PS_OK;
 }
 
+// Argument check of the attention entry points, before anything is enqueued: the descriptor, `in` and the inputs
+// every call reads, then the entry point's own pointers -- `always` must be non-NULL, `with_pe` too when pe_dim > 0.
+static int epi_check_call(const char *who, const ps_epipolar_desc *d, const ps_epipolar_inputs *in,
+                          std::initializer_list<const void *> always, std::initializer_list<const void *> with_pe) {
+    const int rc = epi_check(d);
+    if (rc) return rc;
+    bool ok = in && in->features && in->segments && in->valid && in->rel_disparity && in->q_feat &&
+              (d->pe_dim == 0 || in->q_pe);
+    for (const void *p : always) ok = ok && p;
+    if (d->pe_dim > 0)
+        for (const void *p : with_pe) ok = ok && p;
+    if (!ok) { set_error("%s: a required pointer is NULL", who); return PS_ERR_INVALID_ARGUMENT; }
+    return PS_OK;
+}
+
 static EpiParams epi_params(const ps_epipolar_desc *d, const ps_epipolar_inputs *in) {
     EpiParams P;
     P.B = d->batch; P.V = d->views; P.OV = d->views - 1; P.h = d->grid_h; P.w = d->grid_w; P.S = d->samples;
@@ -882,44 +875,22 @@ using namespace ps;
 
 extern "C" PS_API int ps_epipolar_attention_forward(const ps_epipolar_desc *d, const ps_epipolar_inputs *in,
                                                     float *z, float *e, float *mass, float *lse, void *stream) {
-    int rc = epi_check(d);
+    const int rc = epi_check_call("ps_epipolar_attention_forward", d, in, {z, lse}, {e});
     if (rc) return rc;
-    if (!in || !in->features || !in->segments || !in->valid || !in->rel_disparity || !in->q_feat ||
-        (d->pe_dim > 0 && (!in->q_pe || !e)) || !z || !lse) {
-        set_error("ps_epipolar_attention_forward: a required pointer is NULL");
-        return PS_ERR_INVALID_ARGUMENT;
-    }
-    const EpiParams P = epi_params(d, in);
-    const int n = d->batch * d->views * d->grid_h * d->grid_w;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    switch (d->heads) {
-        case 1: return launch_epi<1>(false, P, n, z, e, mass, lse, 0, 0, 0, 0, 0, 0, 0, 0, 0, st);
-        case 2: return launch_epi<2>(false, P, n, z, e, mass, lse, 0, 0, 0, 0, 0, 0, 0, 0, 0, st);
-        case 3: return launch_epi<3>(false, P, n, z, e, mass, lse, 0, 0, 0, 0, 0, 0, 0, 0, 0, st);
-        default: return launch_epi<4>(false, P, n, z, e, mass, lse, 0, 0, 0, 0, 0, 0, 0, 0, 0, st);
-    }
+    return launch_epi_fwd(epi_params(d, in), d->heads, d->batch * d->views * d->grid_h * d->grid_w, z, e, mass, lse,
+                          static_cast<cudaStream_t>(stream));
 }
 
 extern "C" PS_API int ps_epipolar_attention_backward(const ps_epipolar_desc *d, const ps_epipolar_inputs *in,
                                                      const float *lse, const float *dz, const float *de,
                                                      const float *dmass, const float *d_row, float *dq_feat,
                                                      float *dq_pe, float *dbias, float *dfeatures, void *stream) {
-    int rc = epi_check(d);
+    const int rc = epi_check_call("ps_epipolar_attention_backward", d, in, {lse, dz, d_row, dq_feat, dfeatures},
+                                  {de, dq_pe});
     if (rc) return rc;
-    if (!in || !in->features || !in->segments || !in->valid || !in->rel_disparity || !in->q_feat || !lse ||
-        !dz || (d->pe_dim > 0 && (!de || !dq_pe)) || !d_row || !dq_feat || !dfeatures) {
-        set_error("ps_epipolar_attention_backward: a required pointer is NULL");
-        return PS_ERR_INVALID_ARGUMENT;
-    }
-    const EpiParams P = epi_params(d, in);
-    const int n = d->batch * d->views * d->grid_h * d->grid_w;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    switch (d->heads) {
-        case 1: return launch_epi<1>(true, P, n, 0, 0, 0, 0, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
-        case 2: return launch_epi<2>(true, P, n, 0, 0, 0, 0, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
-        case 3: return launch_epi<3>(true, P, n, 0, 0, 0, 0, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
-        default: return launch_epi<4>(true, P, n, 0, 0, 0, 0, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
-    }
+    const EpiGrads g{lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures};
+    return launch_epi_bwd<false>(epi_params(d, in), d->heads, d->batch * d->views * d->grid_h * d->grid_w, g,
+                                 EpiDetRecords{}, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" PS_API int ps_epipolar_attention_backward_workspace_bytes(const ps_epipolar_desc *d, size_t *out) {
@@ -936,13 +907,9 @@ extern "C" PS_API int ps_epipolar_attention_backward_deterministic(
         const ps_epipolar_desc *d, const ps_epipolar_inputs *in, const float *lse, const float *dz, const float *de,
         const float *dmass, const float *d_row, float *dq_feat, float *dq_pe, float *dbias, float *dfeatures,
         void *workspace, size_t workspace_bytes, void *stream) {
-    int rc = epi_check(d);
+    int rc = epi_check_call("ps_epipolar_attention_backward_deterministic", d, in,
+                            {lse, dz, d_row, dq_feat, dfeatures, workspace}, {de, dq_pe});
     if (rc) return rc;
-    if (!in || !in->features || !in->segments || !in->valid || !in->rel_disparity || !in->q_feat || !lse ||
-        !dz || (d->pe_dim > 0 && (!in->q_pe || !de || !dq_pe)) || !d_row || !dq_feat || !dfeatures || !workspace) {
-        set_error("ps_epipolar_attention_backward_deterministic: a required pointer is NULL");
-        return PS_ERR_INVALID_ARGUMENT;
-    }
     EpiDetLayout L;
     if ((rc = epi_det_layout(d, &L))) return rc;
     if (workspace_bytes < L.total) {
@@ -950,14 +917,7 @@ extern "C" PS_API int ps_epipolar_attention_backward_deterministic(
                   L.total);
         return PS_ERR_INVALID_ARGUMENT;
     }
-    const EpiParams P = epi_params(d, in);
-    const int n = d->batch * d->views * d->grid_h * d->grid_w;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    char *ws = static_cast<char *>(workspace);
-    switch (d->heads) {
-        case 1: return launch_epi_bwd_det<1>(P, n, L, ws, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
-        case 2: return launch_epi_bwd_det<2>(P, n, L, ws, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
-        case 3: return launch_epi_bwd_det<3>(P, n, L, ws, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
-        default: return launch_epi_bwd_det<4>(P, n, L, ws, lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures, st);
-    }
+    const EpiGrads g{lse, dz, de, dmass, d_row, dq_feat, dq_pe, dbias, dfeatures};
+    return launch_epi_bwd_det(epi_params(d, in), d->heads, d->batch * d->views * d->grid_h * d->grid_w, L,
+                              static_cast<char *>(workspace), g, static_cast<cudaStream_t>(stream));
 }
