@@ -144,6 +144,61 @@ __device__ __forceinline__ void stage_rows_x4(const float *__restrict__ src, flo
     }
 }
 
+// Block prologue of both directions: the view's SH rotation and camera into shared memory, then the warp's 32
+// rays: rows_valid of them exist, the first at flat (view, ray) index vr0, their staged rows at float row0 of the
+// dynamic shared memory.  Returns false for a warp past n_rays, only after the barrier the whole block must reach.
+__device__ __forceinline__ bool adapter_prologue(const ps_adapter_desc &d, const ps_adapter_inputs &in, float *sD,
+                                                 AdapterView &sv, int row_stride, int &rows_valid, size_t &vr0,
+                                                 size_t &row0) {
+    const int view = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, n_sh = d.sh_coeffs;
+    load_rotation(in.sh_rotation + (size_t)view * n_sh * n_sh, in.sh_mask, n_sh, sD, tid, kAdThreads);
+    if (tid == 0) adapter_view_setup(in.extrinsics + 16 * view, in.intrinsics + 9 * view, d.image_w, d.image_h, sv);
+    __syncthreads();
+    const int ray0 = (blockIdx.x * kAdWarps + warp) * 32;
+    if (ray0 >= d.n_rays) return false;
+    rows_valid = min(32, d.n_rays - ray0);
+    vr0 = (size_t)view * d.n_rays + ray0;
+    row0 = (size_t)warp * 32 * row_stride;
+    return true;
+}
+
+// Everything a ray's Gaussians share.  The backward differentiates the function the forward evaluates only
+// because both build this frame here; it also keeps sg, qr, dh and inv_n, which the forward does not use.
+struct RayFrame {
+    float sg[3], sigma[3];   // sigmoid of the scale logits, the range-mapped scales
+    float qr[4];             // the raw quaternion
+    QuatFrame qf;
+    float A[9];              // C * Rq
+    float dh[3], inv_n;      // unit camera-space ray direction, 1 / |K^-1 (x, y, 1)|
+    float dw[3];             // world-space ray direction
+};
+
+__device__ __forceinline__ void ray_frame(const float *raw7, const float *coordinates, size_t vr, const AdapterView &sv,
+                                          const ps_adapter_desc &d, RayFrame &f) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        f.sg[k] = sigmoidf(raw7[k]);
+        f.sigma[k] = d.scale_min + (d.scale_max - d.scale_min) * f.sg[k];
+    }
+#pragma unroll
+    for (int a = 0; a < 4; ++a) f.qr[a] = raw7[3 + a];
+    quat_forward(f.qr, d.eps, f.qf);
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+            f.A[3 * r + c] = sv.C[3 * r] * f.qf.R[c] + sv.C[3 * r + 1] * f.qf.R[3 + c] + sv.C[3 * r + 2] * f.qf.R[6 + c];
+    const float x = coordinates[2 * vr], y = coordinates[2 * vr + 1];
+    float dc[3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) dc[r] = sv.Ki[3 * r] * x + sv.Ki[3 * r + 1] * y + sv.Ki[3 * r + 2];
+    f.inv_n = 1.0f / sqrtf(dc[0] * dc[0] + dc[1] * dc[1] + dc[2] * dc[2]);
+#pragma unroll
+    for (int r = 0; r < 3; ++r) f.dh[r] = dc[r] * f.inv_n;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) f.dw[r] = sv.C[3 * r] * f.dh[0] + sv.C[3 * r + 1] * f.dh[1] + sv.C[3 * r + 2] * f.dh[2];
+}
+
 __global__ void __launch_bounds__(kAdThreads)
 k_gaussian_adapter_fwd(ps_adapter_desc d, ps_adapter_inputs in, float *__restrict__ means, float *__restrict__ cov,
                        float *__restrict__ harmonics, float *__restrict__ scales, float *__restrict__ rotations,
@@ -151,16 +206,11 @@ k_gaussian_adapter_fwd(ps_adapter_desc d, ps_adapter_inputs in, float *__restric
     extern __shared__ float s_rows[];                 // [warps][32][row_stride]
     __shared__ float sD[165];
     __shared__ AdapterView sv;
-    const int view = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int n_sh = d.sh_coeffs, raw_n = 7 + 3 * n_sh, ns = d.n_samples;
-    load_rotation(in.sh_rotation + (size_t)view * n_sh * n_sh, in.sh_mask, n_sh, sD, tid, kAdThreads);
-    if (tid == 0) adapter_view_setup(in.extrinsics + 16 * view, in.intrinsics + 9 * view, d.image_w, d.image_h, sv);
-    __syncthreads();
-    const int ray0 = (blockIdx.x * kAdWarps + warp) * 32;
-    if (ray0 >= d.n_rays) return;
-    const int rows_valid = min(32, d.n_rays - ray0);
-    const size_t vr0 = (size_t)view * d.n_rays + ray0;
-    float *wrows = s_rows + (size_t)warp * 32 * row_stride;
+    const int lane = threadIdx.x & 31, n_sh = d.sh_coeffs, raw_n = 7 + 3 * n_sh, ns = d.n_samples;
+    int rows_valid;
+    size_t vr0, row0;
+    if (!adapter_prologue(d, in, sD, sv, row_stride, rows_valid, vr0, row0)) return;
+    float *wrows = s_rows + row0;
     stage_rows_x4(in.raw + vr0 * raw_n, wrows, rows_valid, raw_n, row_stride, lane);
     __syncwarp();
     const bool live = lane < rows_valid;
@@ -168,30 +218,11 @@ k_gaussian_adapter_fwd(ps_adapter_desc d, ps_adapter_inputs in, float *__restric
     if (live) {
         const size_t vr = vr0 + lane;
         sh_rotate_row<false>(row + 7, sD, n_sh);
-        // ---- shared per-ray quantities
-        float sigma[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) sigma[k] = d.scale_min + (d.scale_max - d.scale_min) * sigmoidf(row[k]);
-        QuatFrame qf;
-        quat_forward(row + 3, d.eps, qf);
-        float A[9];                                                   // C * Rq
-#pragma unroll
-        for (int r = 0; r < 3; ++r)
-#pragma unroll
-            for (int c = 0; c < 3; ++c)
-                A[3 * r + c] = sv.C[3 * r] * qf.R[c] + sv.C[3 * r + 1] * qf.R[3 + c] + sv.C[3 * r + 2] * qf.R[6 + c];
-        const float x = in.coordinates[2 * vr], y = in.coordinates[2 * vr + 1];
-        float dc[3], dw[3];
-#pragma unroll
-        for (int r = 0; r < 3; ++r) dc[r] = sv.Ki[3 * r] * x + sv.Ki[3 * r + 1] * y + sv.Ki[3 * r + 2];
-        const float inv_n = 1.0f / sqrtf(dc[0] * dc[0] + dc[1] * dc[1] + dc[2] * dc[2]);
-#pragma unroll
-        for (int r = 0; r < 3; ++r) dc[r] *= inv_n;
-#pragma unroll
-        for (int r = 0; r < 3; ++r) dw[r] = sv.C[3 * r] * dc[0] + sv.C[3 * r + 1] * dc[1] + sv.C[3 * r + 2] * dc[2];
+        RayFrame f;
+        ray_frame(row, in.coordinates, vr, sv, d, f);
         if (rotations) {
 #pragma unroll
-            for (int a = 0; a < 4; ++a) rotations[4 * vr + a] = qf.q[a];
+            for (int a = 0; a < 4; ++a) rotations[4 * vr + a] = f.qf.q[a];
         }
         for (int j = 0; j < ns; ++j) {
             const size_t g = vr * ns + j;
@@ -199,18 +230,18 @@ k_gaussian_adapter_fwd(ps_adapter_desc d, ps_adapter_inputs in, float *__restric
             float sc2[3];
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
-                const float sc = sigma[k] * dep * sv.mult;
+                const float sc = f.sigma[k] * dep * sv.mult;
                 if (scales) scales[3 * g + k] = sc;
                 sc2[k] = sc * sc;
             }
 #pragma unroll
-            for (int r = 0; r < 3; ++r) means[3 * g + r] = sv.o[r] + dw[r] * dep;
+            for (int r = 0; r < 3; ++r) means[3 * g + r] = sv.o[r] + f.dw[r] * dep;
 #pragma unroll
             for (int r = 0; r < 3; ++r)
 #pragma unroll
                 for (int c = 0; c < 3; ++c)
-                    cov[9 * g + 3 * r + c] = sc2[0] * A[3 * r] * A[3 * c] + sc2[1] * A[3 * r + 1] * A[3 * c + 1] +
-                                             sc2[2] * A[3 * r + 2] * A[3 * c + 2];
+                    cov[9 * g + 3 * r + c] = sc2[0] * f.A[3 * r] * f.A[3 * c] + sc2[1] * f.A[3 * r + 1] * f.A[3 * c + 1] +
+                                             sc2[2] * f.A[3 * r + 2] * f.A[3 * c + 2];
         }
     }
     __syncwarp();
@@ -240,16 +271,11 @@ k_gaussian_adapter_bwd(ps_adapter_desc d, ps_adapter_inputs in, const float *__r
     extern __shared__ float s_rows[];                 // [warps][32][row_stride] gradient rows
     __shared__ float sD[165];
     __shared__ AdapterView sv;
-    const int view = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int n_sh = d.sh_coeffs, raw_n = 7 + 3 * n_sh, ns = d.n_samples, sh_n = 3 * n_sh;
-    load_rotation(in.sh_rotation + (size_t)view * n_sh * n_sh, in.sh_mask, n_sh, sD, tid, kAdThreads);
-    if (tid == 0) adapter_view_setup(in.extrinsics + 16 * view, in.intrinsics + 9 * view, d.image_w, d.image_h, sv);
-    __syncthreads();
-    const int ray0 = (blockIdx.x * kAdWarps + warp) * 32;
-    if (ray0 >= d.n_rays) return;
-    const int rows_valid = min(32, d.n_rays - ray0);
-    const size_t vr0 = (size_t)view * d.n_rays + ray0;
-    float *wrows = s_rows + (size_t)warp * 32 * row_stride;
+    const int lane = threadIdx.x & 31, n_sh = d.sh_coeffs, raw_n = 7 + 3 * n_sh, ns = d.n_samples, sh_n = 3 * n_sh;
+    int rows_valid;
+    size_t vr0, row0;
+    if (!adapter_prologue(d, in, sD, sv, row_stride, rows_valid, vr0, row0)) return;
+    float *wrows = s_rows + row0;
     // ---- dL/d(harmonics), summed over the ray's samples, coalesced into the gradient rows
     {
         const bool has0 = lane < sh_n, has1 = lane + 32 < sh_n, has2 = lane + 64 < sh_n;
@@ -273,33 +299,8 @@ k_gaussian_adapter_bwd(ps_adapter_desc d, ps_adapter_inputs in, const float *__r
     if (live) {
         const size_t vr = vr0 + lane;
         sh_rotate_row<true>(row + 7, sD, n_sh);
-        // ---- recompute the forward's per-ray quantities
-        const float *raw = in.raw + vr * raw_n;
-        float sg[3], sigma[3], qr[4];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            sg[k] = sigmoidf(raw[k]);
-            sigma[k] = d.scale_min + (d.scale_max - d.scale_min) * sg[k];
-        }
-#pragma unroll
-        for (int a = 0; a < 4; ++a) qr[a] = raw[3 + a];
-        QuatFrame qf;
-        quat_forward(qr, d.eps, qf);
-        float A[9];
-#pragma unroll
-        for (int r = 0; r < 3; ++r)
-#pragma unroll
-            for (int c = 0; c < 3; ++c)
-                A[3 * r + c] = sv.C[3 * r] * qf.R[c] + sv.C[3 * r + 1] * qf.R[3 + c] + sv.C[3 * r + 2] * qf.R[6 + c];
-        const float x = in.coordinates[2 * vr], y = in.coordinates[2 * vr + 1];
-        float dc[3], dh[3], dw[3];
-#pragma unroll
-        for (int r = 0; r < 3; ++r) dc[r] = sv.Ki[3 * r] * x + sv.Ki[3 * r + 1] * y + sv.Ki[3 * r + 2];
-        const float inv_n = 1.0f / sqrtf(dc[0] * dc[0] + dc[1] * dc[1] + dc[2] * dc[2]);
-#pragma unroll
-        for (int r = 0; r < 3; ++r) dh[r] = dc[r] * inv_n;
-#pragma unroll
-        for (int r = 0; r < 3; ++r) dw[r] = sv.C[3 * r] * dh[0] + sv.C[3 * r + 1] * dh[1] + sv.C[3 * r + 2] * dh[2];
+        RayFrame f;
+        ray_frame(in.raw + vr * raw_n, in.coordinates, vr, sv, d, f);
         // ---- accumulate over the ray's samples
         float g_dw[3] = {0.0f, 0.0f, 0.0f}, g_sigma[3] = {0.0f, 0.0f, 0.0f};
         float gA[9] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
@@ -311,20 +312,20 @@ k_gaussian_adapter_bwd(ps_adapter_desc d, ps_adapter_inputs in, const float *__r
             for (int r = 0; r < 3; ++r) gm[r] = d_means[3 * g + r];
 #pragma unroll
             for (int e = 0; e < 9; ++e) G[e] = d_cov[9 * g + e];
-            float g_dep = gm[0] * dw[0] + gm[1] * dw[1] + gm[2] * dw[2];
+            float g_dep = gm[0] * f.dw[0] + gm[1] * f.dw[1] + gm[2] * f.dw[2];
 #pragma unroll
             for (int r = 0; r < 3; ++r) g_dw[r] += gm[r] * dep;
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
-                const float a0 = A[k], a1 = A[3 + k], a2 = A[6 + k];          // column k of A
+                const float a0 = f.A[k], a1 = f.A[3 + k], a2 = f.A[6 + k];    // column k of A
                 // (G + G^T) a_k
                 const float u0 = 2.0f * G[0] * a0 + (G[1] + G[3]) * a1 + (G[2] + G[6]) * a2;
                 const float u1 = (G[3] + G[1]) * a0 + 2.0f * G[4] * a1 + (G[5] + G[7]) * a2;
                 const float u2 = (G[6] + G[2]) * a0 + (G[7] + G[5]) * a1 + 2.0f * G[8] * a2;
                 const float quad = 0.5f * (a0 * u0 + a1 * u1 + a2 * u2);      // a_k^T G a_k
-                const float sc = sigma[k] * dep * sv.mult;
+                const float sc = f.sigma[k] * dep * sv.mult;
                 const float g_sc = 2.0f * sc * quad + (d_scales ? d_scales[3 * g + k] : 0.0f);
-                g_dep += g_sc * sigma[k] * sv.mult;
+                g_dep += g_sc * f.sigma[k] * sv.mult;
                 g_sigma[k] += g_sc * dep * sv.mult;
                 const float s2 = sc * sc;
                 gA[k] += s2 * u0; gA[3 + k] += s2 * u1; gA[6 + k] += s2 * u2;
@@ -333,7 +334,7 @@ k_gaussian_adapter_bwd(ps_adapter_desc d, ps_adapter_inputs in, const float *__r
         }
         // ---- scale logits
 #pragma unroll
-        for (int k = 0; k < 3; ++k) row[k] = g_sigma[k] * (d.scale_max - d.scale_min) * sg[k] * (1.0f - sg[k]);
+        for (int k = 0; k < 3; ++k) row[k] = g_sigma[k] * (d.scale_max - d.scale_min) * f.sg[k] * (1.0f - f.sg[k]);
         // ---- rotation: dL/dRq = C^T dL/dA, then through quaternion_to_matrix and the normalisation
         float gR[9];
 #pragma unroll
@@ -341,7 +342,7 @@ k_gaussian_adapter_bwd(ps_adapter_desc d, ps_adapter_inputs in, const float *__r
 #pragma unroll
             for (int c = 0; c < 3; ++c)
                 gR[3 * r + c] = sv.C[r] * gA[c] + sv.C[3 + r] * gA[3 + c] + sv.C[6 + r] * gA[6 + c];
-        const float i = qf.q[0], j = qf.q[1], k = qf.q[2], r = qf.q[3], ts = qf.ts;
+        const float i = f.qf.q[0], j = f.qf.q[1], k = f.qf.q[2], r = f.qf.q[3], ts = f.qf.ts;
         const float g_ts = -gR[0] * (j * j + k * k) + gR[1] * (i * j - k * r) + gR[2] * (i * k + j * r) +
                            gR[3] * (i * j + k * r) - gR[4] * (i * i + k * k) + gR[5] * (j * k - i * r) +
                            gR[6] * (i * k - j * r) + gR[7] * (j * k + i * r) - gR[8] * (i * i + j * j);
@@ -352,19 +353,19 @@ k_gaussian_adapter_bwd(ps_adapter_desc d, ps_adapter_inputs in, const float *__r
         gq[3] = ts * (-gR[1] * k + gR[2] * j + gR[3] * k - gR[5] * i - gR[6] * j + gR[7] * i);
         const float g_s2 = -0.5f * ts * ts * g_ts;                             // d ts / d (q.q)
 #pragma unroll
-        for (int a = 0; a < 4; ++a) gq[a] += 2.0f * g_s2 * qf.q[a] + (d_rot ? d_rot[4 * vr + a] : 0.0f);
-        const float den = qf.nq + d.eps;
-        const float dotq = qr[0] * gq[0] + qr[1] * gq[1] + qr[2] * gq[2] + qr[3] * gq[3];
-        const float corr = qf.nq > 0.0f ? dotq / (qf.nq * den * den) : 0.0f;
+        for (int a = 0; a < 4; ++a) gq[a] += 2.0f * g_s2 * f.qf.q[a] + (d_rot ? d_rot[4 * vr + a] : 0.0f);
+        const float den = f.qf.nq + d.eps;
+        const float dotq = f.qr[0] * gq[0] + f.qr[1] * gq[1] + f.qr[2] * gq[2] + f.qr[3] * gq[3];
+        const float corr = f.qf.nq > 0.0f ? dotq / (f.qf.nq * den * den) : 0.0f;
 #pragma unroll
-        for (int a = 0; a < 4; ++a) row[3 + a] = gq[a] / den - qr[a] * corr;
+        for (int a = 0; a < 4; ++a) row[3 + a] = gq[a] / den - f.qr[a] * corr;
         // ---- pixel coordinates: through C, the normalisation and K^-1
         float g_dh[3], g_dc[3];
 #pragma unroll
         for (int c = 0; c < 3; ++c) g_dh[c] = sv.C[c] * g_dw[0] + sv.C[3 + c] * g_dw[1] + sv.C[6 + c] * g_dw[2];
-        const float proj = dh[0] * g_dh[0] + dh[1] * g_dh[1] + dh[2] * g_dh[2];
+        const float proj = f.dh[0] * g_dh[0] + f.dh[1] * g_dh[1] + f.dh[2] * g_dh[2];
 #pragma unroll
-        for (int c = 0; c < 3; ++c) g_dc[c] = (g_dh[c] - dh[c] * proj) * inv_n;
+        for (int c = 0; c < 3; ++c) g_dc[c] = (g_dh[c] - f.dh[c] * proj) * f.inv_n;
         d_coord[2 * vr] = sv.Ki[0] * g_dc[0] + sv.Ki[3] * g_dc[1] + sv.Ki[6] * g_dc[2];
         d_coord[2 * vr + 1] = sv.Ki[1] * g_dc[0] + sv.Ki[4] * g_dc[1] + sv.Ki[7] * g_dc[2];
     }
@@ -447,6 +448,20 @@ static int adapter_check(const ps_adapter_desc *d, const ps_adapter_inputs *in, 
     return PS_OK;
 }
 
+// Runs launch(grid, smem, row_stride) for either kernel: kAdThreads rays per block, rows at an odd shared stride.
+template <class Launch>
+static int launch_adapter(const ps_adapter_desc &d, const char *kernel, Launch launch) {
+    static unsigned long long attr_devices = 0;
+    if (first_use_on_device(attr_devices)) {
+        PS_CUDA_CHECK(cudaFuncSetAttribute(k_gaussian_adapter_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+        PS_CUDA_CHECK(cudaFuncSetAttribute(k_gaussian_adapter_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+    }
+    const int row_stride = (7 + 3 * d.sh_coeffs) | 1;
+    launch(dim3((d.n_rays + kAdThreads - 1) / kAdThreads, d.n_views), sizeof(float) * kAdThreads * row_stride, row_stride);
+    PS_LAUNCH_CHECK(kernel);
+    return PS_OK;
+}
+
 }  // namespace ps
 
 extern "C" PS_API int ps_gaussian_adapter_forward(const ps_adapter_desc *desc, const ps_adapter_inputs *in,
@@ -456,18 +471,10 @@ extern "C" PS_API int ps_gaussian_adapter_forward(const ps_adapter_desc *desc, c
     const int rc = adapter_check(desc, in, "ps_gaussian_adapter_forward");
     if (rc != PS_OK) return rc;
     if (!means || !covariances || !harmonics) { set_error("ps_gaussian_adapter_forward: null output pointer"); return PS_ERR_INVALID_ARGUMENT; }
-    const int raw_n = 7 + 3 * desc->sh_coeffs, row_stride = raw_n | 1;
-    const size_t smem = sizeof(float) * kAdThreads * row_stride;
-    static unsigned long long attr_devices = 0;
-    if (first_use_on_device(attr_devices)) {
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_gaussian_adapter_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_gaussian_adapter_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-    }
-    dim3 grid((desc->n_rays + kAdThreads - 1) / kAdThreads, desc->n_views);
-    k_gaussian_adapter_fwd<<<grid, kAdThreads, smem, static_cast<cudaStream_t>(stream)>>>(
-        *desc, *in, means, covariances, harmonics, scales, rotations, row_stride);
-    PS_LAUNCH_CHECK("k_gaussian_adapter_fwd");
-    return PS_OK;
+    return launch_adapter(*desc, "k_gaussian_adapter_fwd", [&](dim3 grid, size_t smem, int row_stride) {
+        k_gaussian_adapter_fwd<<<grid, kAdThreads, smem, static_cast<cudaStream_t>(stream)>>>(
+            *desc, *in, means, covariances, harmonics, scales, rotations, row_stride);
+    });
 }
 
 extern "C" PS_API int ps_gaussian_adapter_backward(const ps_adapter_desc *desc, const ps_adapter_inputs *in,
@@ -482,19 +489,11 @@ extern "C" PS_API int ps_gaussian_adapter_backward(const ps_adapter_desc *desc, 
         set_error("ps_gaussian_adapter_backward: null gradient pointer");
         return PS_ERR_INVALID_ARGUMENT;
     }
-    const int raw_n = 7 + 3 * desc->sh_coeffs, row_stride = raw_n | 1;
-    const size_t smem = sizeof(float) * kAdThreads * row_stride;
-    static unsigned long long attr_devices = 0;
-    if (first_use_on_device(attr_devices)) {
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_gaussian_adapter_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_gaussian_adapter_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-    }
-    dim3 grid((desc->n_rays + kAdThreads - 1) / kAdThreads, desc->n_views);
-    k_gaussian_adapter_bwd<<<grid, kAdThreads, smem, static_cast<cudaStream_t>(stream)>>>(
-        *desc, *in, d_means, d_covariances, d_harmonics, d_scales, d_rotations, d_coordinates, d_depths, d_raw,
-        row_stride);
-    PS_LAUNCH_CHECK("k_gaussian_adapter_bwd");
-    return PS_OK;
+    return launch_adapter(*desc, "k_gaussian_adapter_bwd", [&](dim3 grid, size_t smem, int row_stride) {
+        k_gaussian_adapter_bwd<<<grid, kAdThreads, smem, static_cast<cudaStream_t>(stream)>>>(
+            *desc, *in, d_means, d_covariances, d_harmonics, d_scales, d_rotations, d_coordinates, d_depths, d_raw,
+            row_stride);
+    });
 }
 
 extern "C" PS_API int ps_sh_rotation_matrices(int32_t n_views, int32_t sh_coeffs, int32_t n_dirs, int32_t convention,
