@@ -96,16 +96,24 @@ class _GaussianAdapterFn(torch.autograd.Function):
         _lib.check(rc, "ps_gaussian_adapter_forward")
         ctx.save_for_backward(*tensors)
         ctx.desc = desc
+        ctx.out_shapes = (means.shape, cov.shape, harm.shape)
+        # training reads scales and rotations only for a visualisation dump: their cotangents stay None and reach
+        # the kernel as NULL instead of as zero tensors it would read for nothing
+        ctx.set_materialize_grads(False)
         return means, cov, harm, scales, rot
 
     @staticmethod
     def backward(ctx, d_means, d_cov, d_harm, d_scales, d_rot):
+        if all(g is None for g in (d_means, d_cov, d_harm, d_scales, d_rot)):
+            return (None,) * 11
         tensors = ctx.saved_tensors
         desc = ctx.desc
         dev = tensors[-1].device
         inputs = _lib.AdapterInputs(*[t.data_ptr() for t in tensors])
         f = lambda t: t.contiguous().float()
-        d_means, d_cov, d_harm = f(d_means), f(d_cov), f(d_harm)
+        # the kernel requires these three; d_scales / d_rot may be NULL
+        d_means, d_cov, d_harm = [f(t) if t is not None else torch.zeros(s, dtype=torch.float32, device=dev)
+                                  for t, s in zip((d_means, d_cov, d_harm), ctx.out_shapes)]
         d_scales = f(d_scales) if d_scales is not None else None
         d_rot = f(d_rot) if d_rot is not None else None
         d_coord = torch.empty_like(tensors[4])
