@@ -428,7 +428,7 @@ PS_API int ps_self_attention_forward(int32_t n_images, int32_t tokens, int32_t h
 PS_API int ps_self_attention_forward_stats(int32_t n_images, int32_t tokens, int32_t heads, int32_t dim_head,
                                            const float *qkv, float scale, float *out, float *stats, void *stream);
 
-/* Backward (wgmma, TF32 operands, FP32 accumulate; csrc/self_attention_tc_bwd.cu): autograd of the forward
+/* Backward (wgmma, TF32 operands, FP32 accumulate; csrc/self_attention_tc.cu): autograd of the forward
  * above.  out / d_out [n_images, 256, heads * 128]; d_qkv has qkv's layout and is fully written. */
 PS_API int ps_self_attention_backward(int32_t n_images, int32_t tokens, int32_t heads, int32_t dim_head,
                                       const float *qkv, const float *out, const float *d_out, const float *stats,

@@ -35,7 +35,6 @@ constexpr uint32_t kLbo64 = 64 * 16;  // bytes between 16-byte K chunks of a 64-
 constexpr uint32_t kLbo128 = 128 * 16;
 constexpr int kTileBytes = kVaTile * kVaD * 4;   // 16 KB
 constexpr int kRowsBytes = kVaRows * kVaD * 4;   // 32 KB
-constexpr float kLog2e = 1.4426950408889634f;
 
 __device__ __forceinline__ void cp_async16(void *dst, const void *src, bool valid) {
     const int n = valid ? 16 : 0;                                  // 0: zero-fill, nothing is read
@@ -44,17 +43,6 @@ __device__ __forceinline__ void cp_async16(void *dst, const void *src, bool vali
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
-__device__ __forceinline__ void sync_before_mma() {
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic -> async proxy (smem operands)
-    __syncthreads();
-}
-
-template <int N>
-__device__ __forceinline__ void zero(float (&d)[N]) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) d[i] = 0.0f;
-}
 
 // ROWS x 64 fp32 rows `src` (row stride in floats) -> canonical K-major no-swizzle layout: 16-byte chunk c of row r
 // at c * ROWS * 16 + r * 16.  Rows >= rows_valid are zero-filled without touching global memory.
@@ -97,6 +85,54 @@ __device__ __forceinline__ void round_and_transpose(unsigned char *nat, unsigned
     }
 }
 
+// Double-buffered stream of the 64-row tiles of two [L, 64] operands a and b (row strides in floats), each through
+// two kTileBytes buffers: tile j of a lands at tile_a(j).
+struct TileStream {
+    unsigned char *sa, *sb;
+    const float *a, *b;
+    size_t rs_a, rs_b;
+    int L, n_tiles;
+    __device__ __forceinline__ unsigned char *tile_a(int j) const { return sa + (j & 1) * kTileBytes; }
+    __device__ __forceinline__ unsigned char *tile_b(int j) const { return sb + (j & 1) * kTileBytes; }
+    // Rows r0 .. r0 + 63 of a and b into buffer pair `buf` (0 or 1).
+    __device__ __forceinline__ void load(int buf, int r0, int tid) const {
+        load_async<kVaTile>(sa + buf * kTileBytes, a + (size_t)r0 * rs_a, rs_a, L - r0, tid);
+        load_async<kVaTile>(sb + buf * kTileBytes, b + (size_t)r0 * rs_b, rs_b, L - r0, tid);
+    }
+    // Prefetches tile j + 1, waits for tile j (tile 0 is loaded in the kernel's first commit group), syncs the CTA.
+    __device__ __forceinline__ void wait(int j, int tid) const {
+        if (j + 1 < n_tiles) {
+            load((j + 1) & 1, j * kVaTile + kVaTile, tid);
+            cp_async_commit();
+            cp_async_wait<1>();
+        } else {
+            cp_async_wait<0>();
+        }
+        __syncthreads();
+    }
+};
+
+// This CTA's (image, head) slice: its q, k, v columns in qkv-shaped tensors (rows rs3 floats apart, k and v at
+// + inner and + 2 inner), its columns in [n, L, H * 64] tensors (rows rs1 apart), its row of [n, H, L] tensors.
+struct HeadSlice {
+    int inner;
+    size_t rs3, rs1, qkv, rows, hl;
+    __device__ __forceinline__ HeadSlice(int L, int n_heads) {
+        const int head = blockIdx.y, img = blockIdx.z;
+        inner = n_heads * kVaD;
+        rs3 = 3 * (size_t)inner;
+        rs1 = (size_t)inner;
+        qkv = (size_t)img * L * rs3 + (size_t)head * kVaD;
+        rows = (size_t)img * L * rs1 + (size_t)head * kVaD;
+        hl = ((size_t)img * n_heads + head) * L;
+    }
+};
+
+// The backward's rebuild of the forward's probability P = exp(s scale - lse) of logit s, lse in log2 units, and
+// of dS = P o (dP - D) scale, rounded as the next MMA sees it.
+__device__ __forceinline__ float prob(float s, float scale_log2e, float lse2) { return exp2f(s * scale_log2e - lse2); }
+__device__ __forceinline__ float dscore(float p, float dp, float D, float scale) { return to_tf32(p * (dp - D) * scale); }
+
 }  // namespace
 
 __global__ void __launch_bounds__(kVaThreads, 1)
@@ -107,38 +143,27 @@ k_vit_attn_fwd(const float *__restrict__ qkv, float *__restrict__ out, float *__
     unsigned char *sK = sQ + kRowsBytes;                             // 2 x (64 x 64)
     unsigned char *sV = sK + 2 * kTileBytes;                         // 2 x (64 x 64), natural
     unsigned char *sVt = sV + 2 * kTileBytes;                        // V^T of the current tile
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
-    const int t = lane & 3;
-    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);         // first of this thread's rows (+8)
+    const int tid = threadIdx.x;
+    const Frag f;
+    const int t = f.t, row = f.row;                                  // rows `row` and `row + 8`
     const int q0 = blockIdx.x * kVaRows, head = blockIdx.y, img = blockIdx.z;
-    const int inner = n_heads * kVaD;
-    const size_t rs3 = 3 * (size_t)inner;
-    const float *q_img = qkv + (size_t)img * L * rs3 + (size_t)head * kVaD;
-    const float *k_img = q_img + inner, *v_img = q_img + 2 * inner;
-    const int n_tiles = (L + kVaTile - 1) / kVaTile;
+    const HeadSlice hs(L, n_heads);
+    const int inner = hs.inner;
+    const float *q_img = qkv + hs.qkv;
+    const TileStream kv{sK, sV, q_img + inner, q_img + 2 * inner, hs.rs3, hs.rs3, L, (L + kVaTile - 1) / kVaTile};
 
-    load_async<kVaRows>(sQ, q_img + (size_t)q0 * rs3, rs3, L - q0, tid);
-    load_async<kVaTile>(sK, k_img, rs3, L, tid);
-    load_async<kVaTile>(sV, v_img, rs3, L, tid);
+    load_async<kVaRows>(sQ, q_img + (size_t)q0 * hs.rs3, hs.rs3, L - q0, tid);
+    kv.load(0, 0, tid);
     cp_async_commit();
 
     float o[32];
     zero(o);
     float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.0f, l1 = 0.0f;     // running max (log2 units), partial row sums
 #pragma unroll 1
-    for (int j = 0; j < n_tiles; ++j) {
+    for (int j = 0; j < kv.n_tiles; ++j) {
         const int k0 = j * kVaTile;
-        unsigned char *bK = sK + (j & 1) * kTileBytes, *bV = sV + (j & 1) * kTileBytes;
-        if (j + 1 < n_tiles) {
-            const int k1 = k0 + kVaTile;
-            load_async<kVaTile>(sK + ((j + 1) & 1) * kTileBytes, k_img + (size_t)k1 * rs3, rs3, L - k1, tid);
-            load_async<kVaTile>(sV + ((j + 1) & 1) * kTileBytes, v_img + (size_t)k1 * rs3, rs3, L - k1, tid);
-            cp_async_commit();
-            cp_async_wait<1>();
-        } else {
-            cp_async_wait<0>();
-        }
-        __syncthreads();
+        unsigned char *bK = kv.tile_a(j), *bV = kv.tile_b(j);
+        kv.wait(j, tid);
         if (j == 0) round_tile<kVaRows>(sQ, tid);
         round_tile<kVaTile>(bK, tid);
         round_and_transpose(bV, sVt, tid);
@@ -146,20 +171,13 @@ k_vit_attn_fwd(const float *__restrict__ qkv, float *__restrict__ out, float *__
 
         float s[32];
         zero(s);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < kVaD / 8; ++k)
-            wgmma_ss_n64(s, gmma_desc(smem_u32(sQ) + k * 2 * kLbo128 + wg * 64 * 16, kLbo128, 128),
-                         gmma_desc(smem_u32(bK) + k * 2 * kLbo64, kLbo64, 128), k > 0);
-        wgmma_commit();
-        wgmma_wait_all();
-        fence_operands(s);
+        mma_ss<kVaD / 8, kVaD / 8>(s, {smem_u32(sQ) + f.a_row(), kLbo128}, {smem_u32(bK), kLbo64});
 
         // online soft-max over this tile's keys of rows `row` (s[4 x + 0 / 1]) and `row + 8` (s[4 x + 2 / 3])
         float mx0 = m0, mx1 = m1;
 #pragma unroll
         for (int x = 0; x < 32; ++x) {
-            const bool valid = k0 + 8 * (x >> 2) + 2 * t + (x & 1) < L;
+            const bool valid = k0 + f.col(x) < L;
             s[x] = valid ? s[x] * scale_log2e : -INFINITY;
             if (x & 2) mx1 = fmaxf(mx1, s[x]);
             else mx0 = fmaxf(mx0, s[x]);
@@ -184,16 +202,7 @@ k_vit_attn_fwd(const float *__restrict__ qkv, float *__restrict__ out, float *__
         l0 = l0 * a0 + sum0;
         l1 = l1 * a1 + sum1;
 
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < kVaTile / 8; ++kk) {
-            uint32_t a[4];
-            acc_to_a(s, kk, a);
-            wgmma_rs_n64(o, a, gmma_desc(smem_u32(sVt) + kk * 2 * kLbo64, kLbo64, 128), 1);
-        }
-        wgmma_commit();
-        wgmma_wait_all();
-        fence_operands(o);
+        mma_rs<kVaTile / 8>(o, s, {smem_u32(sVt), kLbo64}, true);
         __syncthreads();                                             // buffers of tile j are free for tile j + 2
     }
 
@@ -207,15 +216,13 @@ k_vit_attn_fwd(const float *__restrict__ qkv, float *__restrict__ out, float *__
     float *dst = out + ((size_t)img * L + i0) * inner + (size_t)head * kVaD + 2 * t;
     if (i0 < L) {
 #pragma unroll
-        for (int x = 0; x < 8; ++x)
-            *reinterpret_cast<float2 *>(dst + 8 * x) = make_float2(o[4 * x] * inv0, o[4 * x + 1] * inv0);
-        if (t == 0) lse[((size_t)img * n_heads + head) * L + i0] = (m0 + log2f(l0)) * 0.6931471805599453f;
+        for (int x = 0; x < 8; ++x) store_cols(dst + 8 * x, o, x, 0, inv0);
+        if (t == 0) lse[hs.hl + i0] = (m0 + log2f(l0)) * 0.6931471805599453f;
     }
     if (i1 < L) {
 #pragma unroll
-        for (int x = 0; x < 8; ++x)
-            *reinterpret_cast<float2 *>(dst + 8 * (size_t)inner + 8 * x) = make_float2(o[4 * x + 2] * inv1, o[4 * x + 3] * inv1);
-        if (t == 0) lse[((size_t)img * n_heads + head) * L + i1] = (m1 + log2f(l1)) * 0.6931471805599453f;
+        for (int x = 0; x < 8; ++x) store_cols(dst + 8 * (size_t)inner + 8 * x, o, x, 1, inv1);
+        if (t == 0) lse[hs.hl + i1] = (m1 + log2f(l1)) * 0.6931471805599453f;
     }
 }
 
@@ -255,43 +262,33 @@ k_vit_attn_bwd_dkdv(const float *__restrict__ qkv, const float *__restrict__ d_o
     unsigned char *sOt = sQt + kTileBytes;                           // dO_C^T
     float *s_lse = reinterpret_cast<float *>(sOt + kTileBytes);      // [64] lse * log2 e of the chunk's queries
     float *s_D = s_lse + kVaTile;                                    // [64]
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
-    const int t = lane & 3;
-    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int tid = threadIdx.x;
+    const Frag f;
+    const int t = f.t, row = f.row;
     const int j0 = blockIdx.x * kVaRows, head = blockIdx.y, img = blockIdx.z;
-    const int inner = n_heads * kVaD;
-    const size_t rs3 = 3 * (size_t)inner, rs1 = (size_t)inner;
-    const float *q_img = qkv + (size_t)img * L * rs3 + (size_t)head * kVaD;
+    const HeadSlice hs(L, n_heads);
+    const int inner = hs.inner;
+    const size_t rs3 = hs.rs3, rs1 = hs.rs1;
+    const float *q_img = qkv + hs.qkv;
     const float *k_img = q_img + inner, *v_img = q_img + 2 * inner;
-    const float *do_img = d_out + (size_t)img * L * rs1 + (size_t)head * kVaD;
-    const float *lse_h = lse + ((size_t)img * n_heads + head) * L;
-    const float *D_h = Dws + ((size_t)img * n_heads + head) * L;
-    const int n_tiles = (L + kVaTile - 1) / kVaTile;
-    const uint32_t a_row = (uint32_t)wg * 64 * 16;
+    const float *do_img = d_out + hs.rows;
+    const float *lse_h = lse + hs.hl, *D_h = Dws + hs.hl;
+    const TileStream qo{sQ, sO, q_img, do_img, rs3, rs1, L, (L + kVaTile - 1) / kVaTile};
+    const uint32_t a_row = f.a_row();
 
     load_async<kVaRows>(sK, k_img + (size_t)j0 * rs3, rs3, L - j0, tid);
     load_async<kVaRows>(sV, v_img + (size_t)j0 * rs3, rs3, L - j0, tid);
-    load_async<kVaTile>(sQ, q_img, rs3, L, tid);
-    load_async<kVaTile>(sO, do_img, rs1, L, tid);
+    qo.load(0, 0, tid);
     cp_async_commit();
 
     float dv[32], dk[32];
     zero(dv);
     zero(dk);
 #pragma unroll 1
-    for (int c = 0; c < n_tiles; ++c) {
+    for (int c = 0; c < qo.n_tiles; ++c) {
         const int i0 = c * kVaTile;
-        unsigned char *bQ = sQ + (c & 1) * kTileBytes, *bO = sO + (c & 1) * kTileBytes;
-        if (c + 1 < n_tiles) {
-            const int i1 = i0 + kVaTile;
-            load_async<kVaTile>(sQ + ((c + 1) & 1) * kTileBytes, q_img + (size_t)i1 * rs3, rs3, L - i1, tid);
-            load_async<kVaTile>(sO + ((c + 1) & 1) * kTileBytes, do_img + (size_t)i1 * rs1, rs1, L - i1, tid);
-            cp_async_commit();
-            cp_async_wait<1>();
-        } else {
-            cp_async_wait<0>();
-        }
-        __syncthreads();
+        unsigned char *bQ = qo.tile_a(c), *bO = qo.tile_b(c);
+        qo.wait(c, tid);
         if (c == 0) {
             round_tile<kVaRows>(sK, tid);
             round_tile<kVaRows>(sV, tid);
@@ -309,43 +306,17 @@ k_vit_attn_bwd_dkdv(const float *__restrict__ qkv, const float *__restrict__ d_o
         float st[32], dpt[32];
         zero(st);
         zero(dpt);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < kVaD / 8; ++k) {
-            wgmma_ss_n64(st, gmma_desc(smem_u32(sK) + k * 2 * kLbo128 + a_row, kLbo128, 128),
-                         gmma_desc(smem_u32(bQ) + k * 2 * kLbo64, kLbo64, 128), k > 0);
-            wgmma_ss_n64(dpt, gmma_desc(smem_u32(sV) + k * 2 * kLbo128 + a_row, kLbo128, 128),
-                         gmma_desc(smem_u32(bO) + k * 2 * kLbo64, kLbo64, 128), k > 0);
-        }
-        wgmma_commit();
-        wgmma_wait_all();
-        fence_operands(st);
-        fence_operands(dpt);
-        // thread = key row: S^T -> P^T, dP^T -> dS^T in place; query i0 + q, q = column 8 (x >> 2) + 2 t + (x & 1)
+        mma_ss<kVaD / 8, kVaD / 8>(st, {smem_u32(sK) + a_row, kLbo128}, {smem_u32(bQ), kLbo64},
+                                   dpt, {smem_u32(sV) + a_row, kLbo128}, {smem_u32(bO), kLbo64});
+        // thread = key row: S^T -> P^T, dP^T -> dS^T in place; query i0 + column
 #pragma unroll
         for (int x = 0; x < 32; ++x) {
-            const int q = 8 * (x >> 2) + 2 * t + (x & 1);
-            const float p = exp2f(st[x] * scale_log2e - s_lse[q]);
+            const int q = f.col(x);
+            const float p = prob(st[x], scale_log2e, s_lse[q]);
             st[x] = to_tf32(p);
-            dpt[x] = to_tf32(p * (dpt[x] - s_D[q]) * scale);
+            dpt[x] = dscore(p, dpt[x], s_D[q], scale);
         }
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < kVaTile / 8; ++kk) {
-            uint32_t a[4];
-            acc_to_a(st, kk, a);
-            wgmma_rs_n64(dv, a, gmma_desc(smem_u32(sOt) + kk * 2 * kLbo64, kLbo64, 128), 1);
-        }
-#pragma unroll
-        for (int kk = 0; kk < kVaTile / 8; ++kk) {
-            uint32_t a[4];
-            acc_to_a(dpt, kk, a);
-            wgmma_rs_n64(dk, a, gmma_desc(smem_u32(sQt) + kk * 2 * kLbo64, kLbo64, 128), 1);
-        }
-        wgmma_commit();
-        wgmma_wait_all();
-        fence_operands(dv);
-        fence_operands(dk);
+        mma_rs<kVaTile / 8>(dv, st, {smem_u32(sOt), kLbo64}, dk, dpt, {smem_u32(sQt), kLbo64});
         __syncthreads();
     }
     float *dk_img = d_qkv + (size_t)img * L * rs3 + inner + (size_t)head * kVaD;
@@ -357,8 +328,8 @@ k_vit_attn_bwd_dkdv(const float *__restrict__ qkv, const float *__restrict__ d_o
         float *dkp = dk_img + (size_t)j * rs3 + 2 * t, *dvp = dv_img + (size_t)j * rs3 + 2 * t;
 #pragma unroll
         for (int x = 0; x < 8; ++x) {
-            *reinterpret_cast<float2 *>(dkp + 8 * x) = make_float2(dk[4 * x + 2 * h], dk[4 * x + 2 * h + 1]);
-            *reinterpret_cast<float2 *>(dvp + 8 * x) = make_float2(dv[4 * x + 2 * h], dv[4 * x + 2 * h + 1]);
+            store_cols(dkp + 8 * x, dk, x, h);
+            store_cols(dvp + 8 * x, dv, x, h);
         }
     }
 }
@@ -373,44 +344,31 @@ k_vit_attn_bwd_dq(const float *__restrict__ qkv, const float *__restrict__ d_out
     unsigned char *sK = sO + kRowsBytes;                             // 2 x (64 x 64), natural
     unsigned char *sV = sK + 2 * kTileBytes;                         // 2 x (64 x 64), natural
     unsigned char *sKt = sV + 2 * kTileBytes;                        // K_j^T
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
-    const int t = lane & 3;
-    const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    const int q0 = blockIdx.x * kVaRows, head = blockIdx.y, img = blockIdx.z;
-    const int inner = n_heads * kVaD;
-    const size_t rs3 = 3 * (size_t)inner, rs1 = (size_t)inner;
-    const float *q_img = qkv + (size_t)img * L * rs3 + (size_t)head * kVaD;
-    const float *k_img = q_img + inner, *v_img = q_img + 2 * inner;
-    const float *do_img = d_out + (size_t)img * L * rs1 + (size_t)head * kVaD;
-    const size_t hL = ((size_t)img * n_heads + head) * L;
-    const int n_tiles = (L + kVaTile - 1) / kVaTile;
-    const uint32_t a_row = (uint32_t)wg * 64 * 16;
+    const int tid = threadIdx.x;
+    const Frag f;
+    const int q0 = blockIdx.x * kVaRows;
+    const HeadSlice hs(L, n_heads);
+    const size_t rs3 = hs.rs3, rs1 = hs.rs1, hL = hs.hl;
+    const float *q_img = qkv + hs.qkv;
+    const float *do_img = d_out + hs.rows;
+    const TileStream kv{sK, sV, q_img + hs.inner, q_img + 2 * hs.inner, rs3, rs3, L, (L + kVaTile - 1) / kVaTile};
+    const uint32_t a_row = f.a_row();
 
     load_async<kVaRows>(sQ, q_img + (size_t)q0 * rs3, rs3, L - q0, tid);
     load_async<kVaRows>(sO, do_img + (size_t)q0 * rs1, rs1, L - q0, tid);
-    load_async<kVaTile>(sK, k_img, rs3, L, tid);
-    load_async<kVaTile>(sV, v_img, rs3, L, tid);
+    kv.load(0, 0, tid);
     cp_async_commit();
 
-    const int i0 = q0 + row, i1 = i0 + 8;
+    const int i0 = q0 + f.row, i1 = i0 + 8;
     const float lse0 = i0 < L ? lse[hL + i0] * kLog2e : 0.0f, D0 = i0 < L ? Dws[hL + i0] : 0.0f;
     const float lse1 = i1 < L ? lse[hL + i1] * kLog2e : 0.0f, D1 = i1 < L ? Dws[hL + i1] : 0.0f;
     float dq[32];
     zero(dq);
 #pragma unroll 1
-    for (int j = 0; j < n_tiles; ++j) {
+    for (int j = 0; j < kv.n_tiles; ++j) {
         const int k0 = j * kVaTile;
-        unsigned char *bK = sK + (j & 1) * kTileBytes, *bV = sV + (j & 1) * kTileBytes;
-        if (j + 1 < n_tiles) {
-            const int k1 = k0 + kVaTile;
-            load_async<kVaTile>(sK + ((j + 1) & 1) * kTileBytes, k_img + (size_t)k1 * rs3, rs3, L - k1, tid);
-            load_async<kVaTile>(sV + ((j + 1) & 1) * kTileBytes, v_img + (size_t)k1 * rs3, rs3, L - k1, tid);
-            cp_async_commit();
-            cp_async_wait<1>();
-        } else {
-            cp_async_wait<0>();
-        }
-        __syncthreads();
+        unsigned char *bK = kv.tile_a(j), *bV = kv.tile_b(j);
+        kv.wait(j, tid);
         if (j == 0) {
             round_tile<kVaRows>(sQ, tid);
             round_tile<kVaRows>(sO, tid);
@@ -422,44 +380,25 @@ k_vit_attn_bwd_dq(const float *__restrict__ qkv, const float *__restrict__ d_out
         float s[32], dp[32];
         zero(s);
         zero(dp);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < kVaD / 8; ++k) {
-            wgmma_ss_n64(s, gmma_desc(smem_u32(sQ) + k * 2 * kLbo128 + a_row, kLbo128, 128),
-                         gmma_desc(smem_u32(bK) + k * 2 * kLbo64, kLbo64, 128), k > 0);
-            wgmma_ss_n64(dp, gmma_desc(smem_u32(sO) + k * 2 * kLbo128 + a_row, kLbo128, 128),
-                         gmma_desc(smem_u32(bV) + k * 2 * kLbo64, kLbo64, 128), k > 0);
-        }
-        wgmma_commit();
-        wgmma_wait_all();
-        fence_operands(s);
-        fence_operands(dp);
+        mma_ss<kVaD / 8, kVaD / 8>(s, {smem_u32(sQ) + a_row, kLbo128}, {smem_u32(bK), kLbo64},
+                                   dp, {smem_u32(sO) + a_row, kLbo128}, {smem_u32(bV), kLbo64});
+        // keys past L: P = dS = 0
 #pragma unroll
         for (int x = 0; x < 32; ++x) {
-            const bool valid = k0 + 8 * (x >> 2) + 2 * t + (x & 1) < L;
-            const float p = valid ? exp2f(s[x] * scale_log2e - ((x & 2) ? lse1 : lse0)) : 0.0f;
-            s[x] = to_tf32(p * (dp[x] - ((x & 2) ? D1 : D0)) * scale);
+            const bool valid = k0 + f.col(x) < L;
+            const float p = valid ? prob(s[x], scale_log2e, (x & 2) ? lse1 : lse0) : 0.0f;
+            s[x] = dscore(p, dp[x], (x & 2) ? D1 : D0, scale);
         }
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < kVaTile / 8; ++kk) {
-            uint32_t a[4];
-            acc_to_a(s, kk, a);
-            wgmma_rs_n64(dq, a, gmma_desc(smem_u32(sKt) + kk * 2 * kLbo64, kLbo64, 128), 1);
-        }
-        wgmma_commit();
-        wgmma_wait_all();
-        fence_operands(dq);
+        mma_rs<kVaTile / 8>(dq, s, {smem_u32(sKt), kLbo64}, true);
         __syncthreads();
     }
-    float *dq_img = d_qkv + (size_t)img * L * rs3 + (size_t)head * kVaD + 2 * t;
+    float *dq_img = d_qkv + hs.qkv + 2 * f.t;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int i = i0 + 8 * h;
         if (i >= L) continue;
 #pragma unroll
-        for (int x = 0; x < 8; ++x)
-            *reinterpret_cast<float2 *>(dq_img + (size_t)i * rs3 + 8 * x) = make_float2(dq[4 * x + 2 * h], dq[4 * x + 2 * h + 1]);
+        for (int x = 0; x < 8; ++x) store_cols(dq_img + (size_t)i * rs3 + 8 * x, dq, x, h);
     }
 }
 
@@ -492,6 +431,23 @@ bool misaligned(std::initializer_list<const void *> ps) {
     return (a & 15) != 0;
 }
 
+unsigned long long attr_devices = 0;
+
+// Launches one of the three tiled kernels over (128-row tile, head, image).  The first launch on a device raises the
+// dynamic shared-memory limit of all three.
+template <typename Kernel, typename... Args>
+int launch_tiled(Kernel kernel, size_t smem, const char *name, int32_t n_images, int32_t tokens, int32_t heads,
+                 cudaStream_t st, Args... args) {
+    if (first_use_on_device(attr_devices)) {
+        PS_CUDA_CHECK(cudaFuncSetAttribute(k_vit_attn_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFwdSmem));
+        PS_CUDA_CHECK(cudaFuncSetAttribute(k_vit_attn_bwd_dkdv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDkdvSmem));
+        PS_CUDA_CHECK(cudaFuncSetAttribute(k_vit_attn_bwd_dq, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDqSmem));
+    }
+    kernel<<<dim3((tokens + kVaRows - 1) / kVaRows, heads, n_images), kVaThreads, smem, st>>>(args...);
+    PS_LAUNCH_CHECK(name);
+    return PS_OK;
+}
+
 }  // namespace
 
 }  // namespace ps
@@ -506,14 +462,8 @@ extern "C" PS_API int ps_vit_attention_forward(int32_t n_images, int32_t tokens,
         set_error("ps_vit_attention_forward: qkv and out must be 16-byte aligned");
         return PS_ERR_INVALID_ARGUMENT;
     }
-    static unsigned long long attr_devices = 0;
-    if (first_use_on_device(attr_devices))
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_vit_attn_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFwdSmem));
-    const dim3 grid((tokens + kVaRows - 1) / kVaRows, heads, n_images);
-    k_vit_attn_fwd<<<grid, kVaThreads, kFwdSmem, static_cast<cudaStream_t>(stream)>>>(qkv, out, lse, tokens, heads,
-                                                                                      scale * kLog2e);
-    PS_LAUNCH_CHECK("k_vit_attn_fwd");
-    return PS_OK;
+    return launch_tiled(k_vit_attn_fwd, kFwdSmem, "k_vit_attn_fwd", n_images, tokens, heads,
+                        static_cast<cudaStream_t>(stream), qkv, out, lse, tokens, heads, scale * kLog2e);
 }
 
 extern "C" PS_API int ps_vit_attention_backward_workspace_bytes(int32_t n_images, int32_t tokens, int32_t heads,
@@ -546,20 +496,14 @@ extern "C" PS_API int ps_vit_attention_backward(int32_t n_images, int32_t tokens
         set_error("ps_vit_attention_backward: qkv, out, d_out and d_qkv must be 16-byte aligned");
         return PS_ERR_INVALID_ARGUMENT;
     }
-    static unsigned long long attr_devices = 0;
-    if (first_use_on_device(attr_devices)) {
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_vit_attn_bwd_dkdv, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDkdvSmem));
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_vit_attn_bwd_dq, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDqSmem));
-    }
     const cudaStream_t st = static_cast<cudaStream_t>(stream);
     float *D = static_cast<float *>(workspace);
     const long long n_rows = (long long)n_images * tokens * heads;
     k_vit_attn_bwd_d<<<(unsigned)(((size_t)n_rows * 16 + 255) / 256), 256, 0, st>>>(out, d_out, D, n_rows, tokens, heads);
     PS_LAUNCH_CHECK("k_vit_attn_bwd_d");
-    const dim3 grid((tokens + kVaRows - 1) / kVaRows, heads, n_images);
-    k_vit_attn_bwd_dkdv<<<grid, kVaThreads, kDkdvSmem, st>>>(qkv, d_out, lse, D, d_qkv, tokens, heads, scale, scale * kLog2e);
-    PS_LAUNCH_CHECK("k_vit_attn_bwd_dkdv");
-    k_vit_attn_bwd_dq<<<grid, kVaThreads, kDqSmem, st>>>(qkv, d_out, lse, D, d_qkv, tokens, heads, scale, scale * kLog2e);
-    PS_LAUNCH_CHECK("k_vit_attn_bwd_dq");
-    return PS_OK;
+    const int rc2 = launch_tiled(k_vit_attn_bwd_dkdv, kDkdvSmem, "k_vit_attn_bwd_dkdv", n_images, tokens, heads, st,
+                                 qkv, d_out, lse, D, d_qkv, tokens, heads, scale, scale * kLog2e);
+    if (rc2 != PS_OK) return rc2;
+    return launch_tiled(k_vit_attn_bwd_dq, kDqSmem, "k_vit_attn_bwd_dq", n_images, tokens, heads, st,
+                        qkv, d_out, lse, D, d_qkv, tokens, heads, scale, scale * kLog2e);
 }

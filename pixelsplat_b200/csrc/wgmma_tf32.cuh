@@ -1,13 +1,12 @@
-// wgmma (Hopper warpgroup MMA) helpers shared by the self-attention forward and backward kernels: TF32
-// operands in the canonical K-major no-swizzle shared-memory layout, FP32 accumulators in registers.
+// TF32 wgmma (Hopper warpgroup MMA) layer of the attention kernels (self_attention_tc.cu, vit_attention.cu):
+// operands in the canonical K-major no-swizzle shared-memory layout, FP32 accumulators in registers, CTAs of two
+// warpgroups.
 #pragma once
 #include "ps_common.cuh"
 
 namespace ps {
 
-constexpr int kSaL = 256;        // tokens per image
-constexpr int kSaD = 128;        // head dimension
-constexpr int kSaThreads = 256;  // two warpgroups; warpgroup w owns MMA rows 64 w .. 64 w + 63 of the CTA's 128
+constexpr float kLog2e = 1.4426950408889634f;
 
 // fp32 -> nearest TF32 (ties away), kept in an fp32 container: the tensor core ignores the low 13
 // mantissa bits, so rounding here instead of letting it truncate halves the operand error and removes its bias.
@@ -160,6 +159,134 @@ __device__ __forceinline__ void acc_to_a(const float (&d)[N], int kk, uint32_t (
     a[1] = __float_as_uint(d[4 * kk + 2]);
     a[2] = __float_as_uint(d[4 * kk + 1]);
     a[3] = __float_as_uint(d[4 * kk + 3]);
+}
+
+// Makes the CTA's generic-proxy shared-memory stores visible to the wgmma operand reads that follow.
+__device__ __forceinline__ void sync_before_mma() {
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+}
+
+template <int N>
+__device__ __forceinline__ void zero(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) d[i] = 0.0f;
+}
+
+// This thread's place in the accumulator fragments of a 256-thread CTA: warpgroup wg owns MMA rows
+// 64 wg .. 64 wg + 63, and the thread holds rows `row` and `row + 8`, element x of an accumulator at column col(x).
+struct Frag {
+    int wg, t, row;
+    __device__ __forceinline__ Frag() {
+        const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+        wg = warp >> 2;
+        t = lane & 3;
+        row = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    }
+    __device__ __forceinline__ int col(int x) const { return 8 * (x >> 2) + 2 * t + (x & 1); }
+    __device__ __forceinline__ uint32_t a_row() const { return (uint32_t)wg * 64 * 16; }  // its rows in an A tile
+};
+
+// A K-major no-swizzle operand tile in shared memory: `lbo` bytes between its 16-byte K chunks.
+struct SmemTile {
+    uint32_t addr, lbo;
+    __device__ __forceinline__ uint64_t desc(int k) const { return gmma_desc(addr + k * 2 * lbo, lbo, 128); }
+};
+
+// One k8 step, the instruction picked by the accumulator width (N registers = N / 2 columns).
+template <int N>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    static_assert(N == 32 || N == 64 || N == 128, "accumulator width");
+    if constexpr (N == 32) wgmma_ss_n64(d, a_desc, b_desc, accumulate);
+    else if constexpr (N == 64) wgmma_ss_n128(d, a_desc, b_desc, accumulate);
+    else wgmma_ss_n256(d, a_desc, b_desc, accumulate);
+}
+template <int N>
+__device__ __forceinline__ void wgmma_rs(float (&d)[N], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+    static_assert(N == 32 || N == 64, "accumulator width");
+    if constexpr (N == 32) wgmma_rs_n64(d, a, b_desc, accumulate);
+    else wgmma_rs_n128(d, a, b_desc, accumulate);
+}
+
+// D = A B^T over K k8 steps (the first step overwrites D), A and B from shared memory; returns once D is in
+// registers; UNROLL unrolls the k loop.  The two-accumulator form issues both products step by step in one commit
+// group.
+template <int K, int UNROLL, int N>
+__device__ __forceinline__ void mma_ss(float (&d)[N], SmemTile a, SmemTile b) {
+    wgmma_fence();
+#pragma unroll UNROLL
+    for (int k = 0; k < K; ++k) wgmma_ss(d, a.desc(k), b.desc(k), k > 0);
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_operands(d);
+}
+template <int K, int UNROLL, int N>
+__device__ __forceinline__ void mma_ss(float (&d0)[N], SmemTile a0, SmemTile b0, float (&d1)[N], SmemTile a1, SmemTile b1) {
+    wgmma_fence();
+#pragma unroll UNROLL
+    for (int k = 0; k < K; ++k) {
+        wgmma_ss(d0, a0.desc(k), b0.desc(k), k > 0);
+        wgmma_ss(d1, a1.desc(k), b1.desc(k), k > 0);
+    }
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_operands(d0);
+    fence_operands(d1);
+}
+
+// D (+)= P B^T over K k8 steps with A = P straight from an earlier accumulator (acc_to_a's order); the first step
+// overwrites D unless `accumulate`.  The two-accumulator form accumulates into both, D0's steps then D1's, in one
+// commit group.
+template <int K, int N, int M>
+__device__ __forceinline__ void mma_rs(float (&d)[N], const float (&p)[M], SmemTile b, bool accumulate) {
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < K; ++kk) {
+        uint32_t a[4];
+        acc_to_a(p, kk, a);
+        wgmma_rs(d, a, b.desc(kk), accumulate || kk > 0);
+    }
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_operands(d);
+}
+template <int K, int N, int M>
+__device__ __forceinline__ void mma_rs(float (&d0)[N], const float (&p0)[M], SmemTile b0, float (&d1)[N],
+                                       const float (&p1)[M], SmemTile b1) {
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < K; ++kk) {
+        uint32_t a[4];
+        acc_to_a(p0, kk, a);
+        wgmma_rs(d0, a, b0.desc(kk), 1);
+    }
+#pragma unroll
+    for (int kk = 0; kk < K; ++kk) {
+        uint32_t a[4];
+        acc_to_a(p1, kk, a);
+        wgmma_rs(d1, a, b1.desc(kk), 1);
+    }
+    wgmma_commit();
+    wgmma_wait_all();
+    fence_operands(d0);
+    fence_operands(d1);
+}
+
+// Epilogue: columns 8 j + 2 t and 8 j + 2 t + 1 of row `row + 8 h` of accumulator d, times f, as one float2 at dst.
+template <int N>
+__device__ __forceinline__ void store_cols(float *dst, const float (&d)[N], int j, int h, float f = 1.0f) {
+    *reinterpret_cast<float2 *>(dst) = make_float2(d[4 * j + 2 * h] * f, d[4 * j + 2 * h + 1] * f);
+}
+
+// Columns [0, 8 J) of both rows: `row` times f0 at dst, `row + 8` times f1 at dst + 8 stride.
+template <int J, int N>
+__device__ __forceinline__ void store_row_pair(float *dst, size_t stride, const float (&d)[N], float f0 = 1.0f,
+                                               float f1 = 1.0f) {
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+        store_cols(dst + 8 * j, d, j, 0, f0);
+        store_cols(dst + 8 * stride + 8 * j, d, j, 1, f1);
+    }
 }
 
 // ---- staging of fp32 global tiles into the K-major no-swizzle layout (rounded to the nearest TF32) ---------

@@ -2,10 +2,9 @@
 for ImageSelfAttention's ViT blocks, TF32 operands / FP32 accumulation on the tensor cores.
 
 Reference semantics: /root/reference/src/model/transformer/attention.py:54-70 (z = None).  Forward AND
-backward run on the tensor cores (csrc/self_attention_tc_bwd.cu, round 2): the forward saves each row's
-(max, 1 / sum) so that the backward rebuilds exactly the probabilities the forward used, TF32 roundings
-included, and differentiates the forward that actually ran.  PIXELSPLAT_B200_SELF_ATTENTION_BWD=torch keeps the
-round-1 backward (fp32 torch GEMMs on the unrounded operands) for A/B checks.
+backward run on the tensor cores: the forward saves each row's (max, 1 / sum) so that the backward rebuilds
+exactly the probabilities the forward used, TF32 roundings included, and differentiates the forward that
+actually ran.
 
 PIXELSPLAT_B200_SELF_ATTENTION=fp32 routes the module through torch's fp32 matmul/softmax instead
 (for A/B precision checks); the default is the tensor-core kernel whenever the shape is the one it
@@ -67,27 +66,16 @@ class _SelfAttentionTC(torch.autograd.Function):
         qkv, out, stats = ctx.saved_tensors
         n, L, _ = qkv.shape
         H = ctx.heads
-        if os.environ.get("PIXELSPLAT_B200_SELF_ATTENTION_BWD", "tc") != "torch":
-            dout = dout.contiguous().float()
-            d_qkv = torch.empty_like(qkv)
-            stream = torch.cuda.current_stream(qkv.device)
-            rc = _lib.on_device(qkv.device, _lib.lib.ps_self_attention_backward, n, L, H, qkv.shape[-1] // (3 * H),
-                                ctypes.c_void_p(qkv.data_ptr()), ctypes.c_void_p(out.data_ptr()),
-                                ctypes.c_void_p(dout.data_ptr()), ctypes.c_void_p(stats.data_ptr()),
-                                ctypes.c_float(ctx.scale), ctypes.c_void_p(d_qkv.data_ptr()),
-                                ctypes.c_void_p(stream.cuda_stream))
-            _lib.check(rc, "ps_self_attention_backward")
-            return d_qkv, None, None
-        q, k, v = (t.reshape(n, L, H, -1).transpose(1, 2) for t in qkv.chunk(3, dim=-1))     # [n, H, L, d]
-        do = dout.reshape(n, L, H, -1).transpose(1, 2)
-        p = torch.softmax(torch.matmul(q, k.transpose(-1, -2)) * ctx.scale, dim=-1)
-        dv = torch.matmul(p.transpose(-1, -2), do)
-        dp = torch.matmul(do, v.transpose(-1, -2))
-        ds = p * (dp - (dp * p).sum(-1, keepdim=True)) * ctx.scale
-        dq = torch.matmul(ds, k)
-        dk = torch.matmul(ds.transpose(-1, -2), q)
-        back = lambda t: t.transpose(1, 2).reshape(n, L, -1)
-        return torch.cat([back(dq), back(dk), back(dv)], dim=-1), None, None
+        dout = dout.contiguous().float()
+        d_qkv = torch.empty_like(qkv)
+        stream = torch.cuda.current_stream(qkv.device)
+        rc = _lib.on_device(qkv.device, _lib.lib.ps_self_attention_backward, n, L, H, qkv.shape[-1] // (3 * H),
+                            ctypes.c_void_p(qkv.data_ptr()), ctypes.c_void_p(out.data_ptr()),
+                            ctypes.c_void_p(dout.data_ptr()), ctypes.c_void_p(stats.data_ptr()),
+                            ctypes.c_float(ctx.scale), ctypes.c_void_p(d_qkv.data_ptr()),
+                            ctypes.c_void_p(stream.cuda_stream))
+        _lib.check(rc, "ps_self_attention_backward")
+        return d_qkv, None, None
 
 
 def self_attention_tc(qkv: Tensor, heads: int, scale: float) -> Tensor:
