@@ -56,14 +56,23 @@ class EncoderEpipolar(EncoderEpipolarTail):
         else:
             self.epipolar_transformer = None
 
-    def forward(self, context: dict, global_step: int, deterministic: bool = False,
-                visualization_dump: Optional[dict] = None) -> Gaussians:
+    def trunk(self, context: dict) -> tuple[Tensor, Optional[Any]]:
+        """The part of `forward` before the tail: backbone -> backbone_projection -> epipolar transformer.  Returns
+        the features the tail takes [b, v, d_feature, h, w] and the transformer's sampling (None without one).
+        Neither `global_step` nor `deterministic` reaches it, and with two context views it draws no random numbers
+        (with more, the transformer draws one permutation of its view embeddings), so one trunk can feed several
+        calls of the tail, `EncoderEpipolarTail.forward(encoder, features, context, ...)`."""
         features = self.backbone(context)                                           # [b, v, c, h, w]
         features = self.backbone_projection(features.permute(0, 1, 3, 4, 2)).permute(0, 1, 4, 2, 3)
         sampling = None
         if self.cfg.use_epipolar_transformer:
             features, sampling = self.epipolar_transformer(features, context["extrinsics"], context["intrinsics"],
                                                            context["near"], context["far"])
+        return features, sampling
+
+    def forward(self, context: dict, global_step: int, deterministic: bool = False,
+                visualization_dump: Optional[dict] = None) -> Gaussians:
+        features, sampling = self.trunk(context)
         gaussians = super().forward(features, context, global_step, deterministic, visualization_dump)
         if visualization_dump is not None and sampling is not None:
             visualization_dump["sampling"] = sampling

@@ -2,7 +2,8 @@
 dataset, here with the bounded view sampler):
 
     config/main.yaml                      seed 111123, optimizer lr 1.5e-4 / warm_up_steps 2000, gradient_clip_val
-                                          0.5, train loader 16 workers / seed 1234, checkpoint every 5000 steps
+                                          0.5, train loader 16 workers / seed 1234, checkpoint every 5000 steps,
+                                          val loader batch 1 / 1 worker / seed 3456, val_check_interval 250
     config/experiment/{re10k,acid}.yaml   batch 7, max_steps 300_001, losses [mse, lpips]
     config/experiment/re10k_depth_loss.yaml   max_steps 350_001, losses [mse, lpips, depth], depth sigma_image 12 and
                                           second derivative, train.depth_mode depth
@@ -23,6 +24,8 @@ from ..loss import (LossDepth, LossDepthCfg, LossDepthCfgWrapper, LossLpips, Los
 PRESETS = ("re10k", "acid", "re10k_depth_loss")
 SEED = ev.SEED                  # torch.manual_seed(SEED + rank)
 LOADER_SEED = 1234              # the train loader's generator: LOADER_SEED + rank
+VAL_SEED = 3456                 # the validation loader's generator and the validation step's RNG: VAL_SEED + rank
+VAL_EVERY = 250                 # the reference's trainer.val_check_interval
 
 
 @dataclass(frozen=True)
@@ -81,6 +84,14 @@ def make_train_dataset(cfg: DatasetRE10kCfg, step_tracker: StepTracker | None) -
     sampler = get_view_sampler(cfg.view_sampler, "train", cfg.overfit_to_scene is not None,
                                cfg.cameras_are_circular, step_tracker)
     return DatasetRE10k(cfg, "train", sampler)
+
+
+def make_val_dataset(cfg: DatasetRE10kCfg, step_tracker: StepTracker | None) -> DatasetRE10k:
+    """The reference's validation data: stage "val" reads the test split, shuffles chunks and examples, never flips,
+    and samples views with the training's bounded sampler and warm-up."""
+    sampler = get_view_sampler(cfg.view_sampler, "val", cfg.overfit_to_scene is not None,
+                               cfg.cameras_are_circular, step_tracker)
+    return DatasetRE10k(cfg, "val", sampler)
 
 
 def make_losses(preset: TrainPreset, lpips=None) -> list:
