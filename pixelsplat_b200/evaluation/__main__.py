@@ -13,6 +13,10 @@ peak_memory.json and metrics.json (the mean and each scene's metrics).
 
 is the reference's compute_metrics script: it scores saved frame directories of one or more methods.
 
+--preset names the experiment the checkpoint was trained with: re10k, acid, re10k_depth_loss, the paper's ablations
+re10k_ablation_no_epipolar_transformer / _no_probabilistic_sampling / _no_depth_encoding, or re10k_3_view (three
+context views: the index's two and the frame halfway between them).
+
 Nothing is downloaded: the checkpoint holds every encoder weight, and LPIPS reads torchvision's VGG16 file and the
 lpips package's lin weights from disk (--lpips-vgg / --lpips-lin, or where those packages keep them).
 """
@@ -35,9 +39,9 @@ def _common(p: argparse.ArgumentParser) -> None:
     p.add_argument("--lpips-lin", type=Path, default=None, help="the lpips package's weights/v0.1/vgg.pth")
 
 
-def _loader(args):
+def _loader(args, preset: str = "re10k"):
     from .presets import dataset_cfg, make_test_dataset
-    cfg = dataset_cfg(args.dataset_root, args.index)
+    cfg = dataset_cfg(args.dataset_root, args.index, preset=preset)
     return cfg, torch.utils.data.DataLoader(make_test_dataset(cfg), batch_size=1, num_workers=args.num_workers,
                                             pin_memory=True)
 
@@ -47,27 +51,42 @@ def _lpips(args, device):
     return Lpips.from_files(args.lpips_vgg, args.lpips_lin).to(device).eval()
 
 
-def evaluate(argv: list[str]) -> dict:
+def load_preset_checkpoint(path: Path, encoder, preset: str) -> int:
+    """`load_checkpoint`, with a hint when the checkpoint's weights do not fit the preset's encoder: a checkpoint of
+    an ablation or of the three-view model loads only into the model of its own preset."""
+    from .checkpoint import load_checkpoint
+    try:
+        return load_checkpoint(path, encoder)
+    except RuntimeError as e:
+        raise SystemExit(f"evaluation: {path} does not fit the encoder of --preset {preset}; check that --preset "
+                         f"names the experiment the checkpoint was trained with ({e})") from e
+
+
+def parse_evaluate(argv: list[str]) -> argparse.Namespace:
+    from .presets import PRESETS
     p = argparse.ArgumentParser(prog="python -m pixelsplat_b200.evaluation",
                                 description="Evaluate a pixelSplat checkpoint on the RE10k / ACID test split.")
     _common(p)
     p.add_argument("--checkpoint", type=Path, required=True, help="a pixelSplat Lightning checkpoint (.ckpt)")
-    p.add_argument("--preset", choices=("re10k", "acid"), default="re10k")
+    p.add_argument("--preset", choices=PRESETS, default="re10k",
+                   help="the experiment the checkpoint was trained with (default: re10k)")
     p.add_argument("--output", type=Path, default=None, help="where frames and the JSON files go")
     p.add_argument("--deterministic", action="store_true",
                    help="the encoder picks each ray's most likely depth instead of sampling one")
     p.add_argument("--no-frames", action="store_true", help="write no PNG (metrics and JSON files only)")
     p.add_argument("--global-step", type=int, default=0,
                    help="step given to the encoder (the presets' opacity mapping does not depend on it)")
-    args = p.parse_args(argv)
+    return p.parse_args(argv)
 
-    from .checkpoint import load_checkpoint
+
+def evaluate(argv: list[str]) -> dict:
+    args = parse_evaluate(argv)
     from .evaluator import Evaluator
     from .presets import SEED, build_model
     device = torch.device("cuda", torch.cuda.current_device())
-    cfg, loader = _loader(args)
+    cfg, loader = _loader(args, args.preset)
     encoder, decoder = build_model(args.preset, cfg)
-    step = load_checkpoint(args.checkpoint, encoder)
+    step = load_preset_checkpoint(args.checkpoint, encoder, args.preset)
     print(f"Loaded {args.checkpoint} (trained for {step} steps).")
     evaluator = Evaluator(encoder.to(device).eval(), decoder.to(device), args.output, _lpips(args, device),
                           deterministic=args.deterministic, global_step=args.global_step,

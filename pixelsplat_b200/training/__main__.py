@@ -45,7 +45,7 @@ def parse(argv: list[str]) -> argparse.Namespace:
     p.add_argument("--dataset-root", type=Path, required=True, help="dataset root holding train/index.json")
     p.add_argument("--preset", choices=PRESETS, default="re10k")
     p.add_argument("--output", type=Path, required=True, help="where checkpoints/ and log.jsonl go")
-    p.add_argument("--batch-size", type=int, default=None, help="scenes per GPU (default: the preset's 7)")
+    p.add_argument("--batch-size", type=int, default=None, help="scenes per GPU (default: the preset's batch size)")
     p.add_argument("--max-steps", type=int, default=None, help="default: the preset's")
     p.add_argument("--checkpoint-every", type=int, default=None, help="steps (default: the preset's 5000)")
     p.add_argument("--log-every", type=int, default=10)

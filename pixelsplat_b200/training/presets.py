@@ -7,6 +7,8 @@ dataset, here with the bounded view sampler):
     config/experiment/{re10k,acid}.yaml   batch 7, max_steps 300_001, losses [mse, lpips]
     config/experiment/re10k_depth_loss.yaml   max_steps 350_001, losses [mse, lpips, depth], depth sigma_image 12 and
                                           second derivative, train.depth_mode depth
+    config/experiment/re10k_ablation_*.yaml   as re10k, with the encoder of the evaluation preset of the same name
+    config/experiment/re10k_3_view.yaml   batch 3, 3 context views, context gap 50..90 -> 90..384 over 150_000 steps
     config/loss/{mse,lpips,depth}.yaml    weights 1.0 / 0.05 (apply_after_step 150_000) / 0.25
     config/dataset/view_sampler/bounded.yaml + view_sampler_dataset_specific_config/bounded_re10k.yaml
                                           2 context views, 4 targets, context gap 25 -> 45 over 150_000 steps
@@ -21,7 +23,8 @@ from ..evaluation import presets as ev
 from ..loss import (LossDepth, LossDepthCfg, LossDepthCfgWrapper, LossLpips, LossLpipsCfg, LossLpipsCfgWrapper, LossMse,
                     LossMseCfg, LossMseCfgWrapper)
 
-PRESETS = ("re10k", "acid", "re10k_depth_loss")
+PRESETS = ("re10k", "acid", "re10k_depth_loss", "re10k_ablation_no_epipolar_transformer",
+           "re10k_ablation_no_probabilistic_sampling", "re10k_ablation_no_depth_encoding", "re10k_3_view")
 SEED = ev.SEED                  # torch.manual_seed(SEED + rank)
 LOADER_SEED = 1234              # the train loader's generator: LOADER_SEED + rank
 VAL_SEED = 3456                 # the validation loader's generator and the validation step's RNG: VAL_SEED + rank
@@ -64,6 +67,14 @@ TRAIN_PRESETS = {
     "acid": replace(_RE10K, model="acid"),
     "re10k_depth_loss": replace(_RE10K, max_steps=350_001, losses=("mse", "lpips", "depth"), depth_sigma_image=12.0,
                                 depth_use_second_derivative=True, depth_mode="depth"),
+    **{name: replace(_RE10K, model=name) for name in ("re10k_ablation_no_epipolar_transformer",
+                                                        "re10k_ablation_no_probabilistic_sampling",
+                                                        "re10k_ablation_no_depth_encoding")},
+    # twice the context gap, with a third view in between
+    "re10k_3_view": replace(_RE10K, model="re10k_3_view", batch_size=3, view_sampler=replace(
+        _BOUNDED_RE10K, num_context_views=3, min_distance_between_context_views=90,
+        max_distance_between_context_views=384, initial_min_distance_between_context_views=50,
+        initial_max_distance_between_context_views=90)),
 }
 
 

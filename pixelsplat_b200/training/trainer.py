@@ -175,7 +175,8 @@ class Trainer:
     def validation_step(self, batch: dict) -> dict:
         """The reference's validation step on a device-resident batch of one scene (what `device_shim` returns): the
         data shim, then the encoder's trunk once and its tail twice, probabilistic and then deterministic (the
-        reference's order; the trunk draws no random numbers, so the draws are the ones two full encoder passes make),
+        reference's order; with two context views the trunk draws no random numbers, so the draws are the ones two
+        full encoder passes make; with three it draws the view embeddings' permutation once and both tails see it),
         each encoding rendered at the targets.  Runs without autograd, with the encoder, the losses and the LPIPS
         module in eval mode (BatchNorm reads its running statistics and does not update them), and restores their
         modes afterwards; inside `validation_rng`, so the training's generators do not move.
