@@ -367,7 +367,10 @@ typedef struct ps_epipolar_inputs {
     const float *bias;          /* [b*v*R, heads, v-1] or NULL (view-embedding score term)      */
 } ps_epipolar_inputs;
 
-/* segments/valid/rel_disparity as above; t_range [b, v, v-1, R, 2] (t_min, t_max) or NULL. */
+/* segments/valid/rel_disparity as above; t_range [b, v, v-1, R, 2] (t_min, t_max) or NULL.
+ * PS_ERR_INVALID_ARGUMENT for a count below its minimum (b, grid, samples >= 1, v >= 2) or a NULL required pointer,
+ * and PS_ERR_UNSUPPORTED when b * v * (v - 1) > 65535 or grid_h * grid_w >= 2^31, both before anything is
+ * enqueued. */
 PS_API int ps_epipolar_geometry(int32_t batch, int32_t views, int32_t grid_h, int32_t grid_w,
                                 int32_t samples, const float *extrinsics /* [b,v,4,4] c2w */,
                                 const float *intrinsics /* [b,v,3,3] */, const float *near_plane,

@@ -120,8 +120,8 @@ k_epipolar_geometry(int B, int V, int h, int w, int S, const float *__restrict__
     if (threadIdx.x == 32) load_cam(extr + 16 * (b * V + o_view), intr + 9 * (b * V + o_view), cam_o);
     __syncthreads();
     const int R = h * w;
+    if ((int64_t)blockIdx.x * blockDim.x + threadIdx.x >= R) return;
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= R) return;
     const double nearv = (double)near_[b * V + v], farv = (double)far_[b * V + v];
 
     // --- world ray through the centre of ray-grid cell r of view v
@@ -170,9 +170,10 @@ k_epipolar_geometry(int B, int V, int h, int w, int S, const float *__restrict__
     const double disp_near = 1.0 / (nearv + eps), disp_far = 1.0 / (farv + eps);
     for (int s = 0; s < S; ++s) {
         const double u = (s + 0.5) / S;
-        // the reference forms the sample in the tensors' dtype (fp32): keep its rounding of xy
-        const float fx = (float)x0 + (float)u * ((float)x1 - (float)x0);
-        const float fy = (float)y0 + (float)u * ((float)y1 - (float)y0);
+        // the reference forms the sample in the tensors' dtype (fp32) as a multiply and an add, each rounded: keep
+        // its rounding of xy (intrinsics, not operators, so FMA contraction cannot fuse the two)
+        const float fx = __fadd_rn((float)x0, __fmul_rn((float)u, (float)x1 - (float)x0));
+        const float fy = __fadd_rn((float)y0, __fmul_rn((float)u, (float)y1 - (float)y0));
         double d2c[3], d2[3], o2[3];
         for (int i = 0; i < 3; ++i)
             d2c[i] = cam_o.kinv[3 * i] * (double)fx + cam_o.kinv[3 * i + 1] * (double)fy + cam_o.kinv[3 * i + 2];
@@ -216,8 +217,13 @@ extern "C" PS_API int ps_epipolar_geometry(int32_t batch, int32_t views, int32_t
         ps::set_error("ps_epipolar_geometry: bad argument (views must be >= 2, pointers non-NULL)");
         return PS_ERR_INVALID_ARGUMENT;
     }
-    const int R = grid_h * grid_w;
-    dim3 grid((R + 127) / 128, batch * views * (views - 1));
+    // one block row per (batch, view, other view) on the grid's y axis, and a 32-bit ray index
+    const int64_t slices = (int64_t)batch * views * (views - 1), rays = (int64_t)grid_h * grid_w;
+    if (slices > 65535 || rays > INT32_MAX) {
+        ps::set_error("ps_epipolar_geometry: batch * views * (views - 1) must be <= 65535 and grid_h * grid_w < 2^31");
+        return PS_ERR_UNSUPPORTED;
+    }
+    dim3 grid((unsigned)((rays + 127) / 128), (unsigned)slices);
     ps::k_epipolar_geometry<<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
         batch, views, grid_h, grid_w, samples, extrinsics, intrinsics, near_plane, far_plane, segments, valid,
         rel_disparity, t_range);

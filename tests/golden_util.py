@@ -55,7 +55,17 @@ def camera_rig(b: int, v: int, case: str = "generic"):
       generic   views spread along x with small rotations (the re10k situation)
       parallel  identical orientation and identical position for two views (parallel rays -> 1e10)
       diverging cameras looking away from each other (most rays miss the other image: invalid)
+      epipole   the other cameras sit in front of view 0 along its optical axis, so each view's epipole lies inside
+                the other images and the near ends of many segments share a few cells
+      partial   cameras yawed apart, so each view's rays partly hit and partly miss every other image
+      facing    cameras in two rows facing each other, so each sees the others and the rays through the epipole
+                are anti-parallel to the other camera's rays through it
+      nearfar   the generic rig with near and far planes that differ per (batch, view)
+      aniso     the generic rig with anisotropic, off-centre intrinsics (fx != fy, principal point far from 0.5)
+    The generic, parallel and diverging rigs are pinned by committed fixtures: they must not change.
     """
+    if case in ("epipole", "partial", "facing", "nearfar", "aniso"):
+        return _derived_rig(b, v, case)
     ext = torch.eye(4, dtype=torch.float64).repeat(b, v, 1, 1)
     K = torch.eye(3, dtype=torch.float64).repeat(b, v, 1, 1)
     for bi in range(b):
@@ -75,6 +85,33 @@ def camera_rig(b: int, v: int, case: str = "generic"):
             K[bi, vi, 0, 2], K[bi, vi, 1, 2] = 0.5 + 0.01 * math.cos(s), 0.5 - 0.01 * math.sin(s)
     near = torch.full((b, v), 0.293, dtype=torch.float64) * (1 + 0.1 * torch.arange(v, dtype=torch.float64))
     far = torch.full((b, v), 450.6, dtype=torch.float64)
+    return ext, K, near, far
+
+
+def _derived_rig(b: int, v: int, case: str):
+    """The rigs camera_rig adds on top of the generic one (see there)."""
+    ext, K, near, far = camera_rig(b, v, "generic")
+    for bi in range(b):
+        for vi in range(v):
+            s = 0.37 * bi + 0.91 * vi
+            if case == "epipole":
+                ext[bi, vi] = torch.eye(4, dtype=torch.float64)
+                ext[bi, vi, :3, 3] = torch.tensor([0.02 * vi, -0.015 * vi, 0.8 * vi + 0.05 * bi], dtype=torch.float64)
+            elif case == "partial":
+                ext[bi, vi, :3, :3] = rotation(0.05 * math.sin(s), 0.45 * (vi - (v - 1) / 2) + 0.03 * bi, 0.0)
+                ext[bi, vi, :3, 3] = torch.tensor([0.6 * vi, 0.03 * math.sin(s), 0.1 * math.cos(s)],
+                                                  dtype=torch.float64)
+            elif case == "facing":
+                back = vi % 2
+                ext[bi, vi, :3, :3] = rotation(0.02 * math.sin(s), math.pi * back + 0.04 * math.cos(s), 0.01 * bi)
+                ext[bi, vi, :3, 3] = torch.tensor([0.15 * (vi // 2) + 0.01 * bi, 0.02 * math.sin(s), 2.0 * back],
+                                                  dtype=torch.float64)
+            elif case == "aniso":
+                K[bi, vi, 0, 0], K[bi, vi, 1, 1] = 1.3 + 0.05 * math.sin(s), 0.7 + 0.02 * math.cos(s)
+                K[bi, vi, 0, 2], K[bi, vi, 1, 2] = 0.82 + 0.02 * math.sin(s), 0.21 - 0.02 * math.cos(s)
+            if case == "nearfar":
+                near[bi, vi] = 0.15 + 0.2 * bi + 0.07 * vi
+                far[bi, vi] = 3.0 + 4.0 * bi + 1.5 * vi
     return ext, K, near, far
 
 

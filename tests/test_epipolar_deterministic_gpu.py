@@ -44,23 +44,10 @@ def det():
             os.environ["CUBLAS_WORKSPACE_CONFIG"] = cublas
 
 
-def _rig(b, v, case):
-    """golden_util.camera_rig, plus "epipole": the other cameras sit in front of view 0 along its optical axis, so each
-    view's epipole lies inside the other images and the near ends of many segments share a few cells."""
-    if case != "epipole":
-        return gu.camera_rig(b, v, case)
-    ext, K, near, far = gu.camera_rig(b, v, "generic")
-    for bi in range(b):
-        for vi in range(v):
-            ext[bi, vi] = torch.eye(4, dtype=torch.float64)
-            ext[bi, vi, :3, 3] = torch.tensor([0.02 * vi, -0.015 * vi, 0.8 * vi + 0.05 * bi], dtype=torch.float64)
-    return ext, K, near, far
-
-
 def _case(b, v, grid, S, heads, npe, rig, bias=True, seed=0):
     """Inputs of _EpipolarAttentionFn and the output cotangents (seeded)."""
     from pixelsplat_b200.encoder.attention_fused import epipolar_geometry
-    ext, K, near, far = [t.to(DEV, torch.float32) for t in _rig(b, v, rig)]
+    ext, K, near, far = [t.to(DEV, torch.float32) for t in gu.camera_rig(b, v, rig)]
     geom = epipolar_geometry(ext, K, near, far, grid, S)
     h, w = grid
     n, ov = b * v * h * w, v - 1
