@@ -419,8 +419,10 @@ PS_API int ps_epipolar_attention_backward_deterministic(const ps_epipolar_desc *
  * ImageSelfAttention (/root/reference/src/model/encoder/epipolar/image_self_attention.py:57-79):
  *   qkv  [n_images, tokens, 3 * heads * dim_head]   output of to_qkv ("b n (qkv h d)")
  *   out  [n_images, tokens, heads * dim_head]       softmax(q k^T * scale) v, "b n (h d)"
- * Supported shape: tokens == 256, dim_head == 128 (pixelSplat's ViT stage at 256x256), heads <= 16;
- * anything else returns PS_ERR_UNSUPPORTED.  debug_mode 1 writes the raw q k^T logits instead
+ * Supported shape: tokens == 256, dim_head == 128 (pixelSplat's ViT stage at 256x256), heads <= 16,
+ * n_images <= 65535; anything else returns PS_ERR_UNSUPPORTED before anything is enqueued.  scale must be finite
+ * and >= 0 (the row max is taken on the unscaled logits), else PS_ERR_INVALID_ARGUMENT, as for a NULL or not
+ * 16-byte aligned pointer; the backward checks the same.  debug_mode 1 writes the raw q k^T logits instead
  * (out is then [n_images, heads, 256, 256]); used by the tests only. */
 PS_API int ps_self_attention_forward(int32_t n_images, int32_t tokens, int32_t heads, int32_t dim_head,
                                      const float *qkv, float scale, float *out, int32_t debug_mode,

@@ -156,7 +156,9 @@ k_self_attention_tc_bwd(const float *__restrict__ qkv, const float *__restrict__
     float *dq_img = d_qkv + (size_t)img * kSaL * rs3 + (size_t)head * kSaD;
     float *dk_img = dq_img + inner, *dv_img = dq_img + 2 * inner;
 
-    // per-query constants of all 256 queries: (max, 1 / sum) saved by the forward, D = dO . O
+    // per-query constants of all 256 queries: (max, 1 / sum) saved by the forward, D = dO . O with dO rounded as
+    // the dPn = dO V^T MMA sees it, so that the TF32 error of dO cancels in dPn - D (with the fp32 dO it does not,
+    // and dQ, dK lose digits wherever dPn - D is small against dPn: values with a common offset, peaked rows)
     {
         const int i = tid;                                                  // kSaThreads == kSaL
         const float2 st = reinterpret_cast<const float2 *>(stats)[((size_t)img * n_heads + head) * kSaL + i];
@@ -167,7 +169,7 @@ k_self_attention_tc_bwd(const float *__restrict__ qkv, const float *__restrict__
         float acc = 0.0f;
 #pragma unroll 8
         for (int c = 0; c < kSaD / 4; ++c) {
-            const float4 x = __ldg(a + c), y = __ldg(b + c);
+            const float4 x = to_tf32(__ldg(a + c)), y = __ldg(b + c);
             acc += x.x * y.x + x.y * y.y + x.z * y.z + x.w * y.w;
         }
         s_D[i] = acc;
@@ -263,8 +265,10 @@ k_self_attention_tc_bwd(const float *__restrict__ qkv, const float *__restrict__
     }
 }
 
-// Shape, pointer and alignment checks of the three entry points: `ptrs` must be non-NULL and 16-byte aligned.
-static int sa_check(const char *who, int32_t n_images, int32_t tokens, int32_t heads, int32_t dim_head,
+// Shape, scale, pointer and alignment checks of the three entry points: `ptrs` must be non-NULL and 16-byte aligned.
+// The scale must be finite and >= 0: the forward takes the row max on the raw logits and scales afterwards, so a
+// negative scale would turn exp2 of (s - max) * scale into an overflow.  n_images is grid.z (<= 65535).
+static int sa_check(const char *who, int32_t n_images, int32_t tokens, int32_t heads, int32_t dim_head, float scale,
                     std::initializer_list<const void *> ptrs) {
     bool null = false;
     uintptr_t bits = 0;
@@ -280,6 +284,14 @@ static int sa_check(const char *who, int32_t n_images, int32_t tokens, int32_t h
         set_error("%s: only 256 tokens x 128-dim heads are supported (got %d x %d)", who, tokens, dim_head);
         return PS_ERR_UNSUPPORTED;
     }
+    if (n_images > 65535) {
+        set_error("%s: at most 65535 images per call are supported (got %d)", who, n_images);
+        return PS_ERR_UNSUPPORTED;
+    }
+    if (!(scale >= 0.0f && scale <= 3.402823466e38f)) {
+        set_error("%s: scale must be finite and >= 0 (got %g)", who, (double)scale);
+        return PS_ERR_INVALID_ARGUMENT;
+    }
     if (bits & 15) {
         set_error("%s: pointers must be 16-byte aligned", who);
         return PS_ERR_INVALID_ARGUMENT;
@@ -289,7 +301,7 @@ static int sa_check(const char *who, int32_t n_images, int32_t tokens, int32_t h
 
 static int sa_forward(int32_t n_images, int32_t tokens, int32_t heads, int32_t dim_head, const float *qkv, float scale,
                       float *out, float *stats, int32_t debug_mode, void *stream) {
-    const int rc = sa_check("ps_self_attention_forward", n_images, tokens, heads, dim_head, {qkv, out});
+    const int rc = sa_check("ps_self_attention_forward", n_images, tokens, heads, dim_head, scale, {qkv, out});
     if (rc != PS_OK) return rc;
     static unsigned long long attr_devices = 0;
     if (first_use_on_device(attr_devices))
@@ -319,7 +331,7 @@ extern "C" PS_API int ps_self_attention_backward(int32_t n_images, int32_t token
                                                  const float *qkv, const float *out, const float *d_out,
                                                  const float *stats, float scale, float *d_qkv, void *stream) {
     using namespace ps;
-    const int rc = sa_check("ps_self_attention_backward", n_images, tokens, heads, dim_head,
+    const int rc = sa_check("ps_self_attention_backward", n_images, tokens, heads, dim_head, scale,
                             {qkv, out, d_out, d_qkv, stats});
     if (rc != PS_OK) return rc;
     static unsigned long long attr_devices = 0;

@@ -13,6 +13,7 @@ is written for (256 tokens, 128-dim heads).
 from __future__ import annotations
 
 import ctypes
+import math
 import os
 
 import torch
@@ -23,9 +24,12 @@ from .. import _lib
 TOKENS, DIM_HEAD = 256, 128
 
 
-def supported(x: Tensor, heads: int, dim_head: int) -> bool:
+def supported(x: Tensor, heads: int, dim_head: int, scale: float) -> bool:
+    """Whether the kernel takes this call; a negative or non-finite scale is left to torch (the kernel takes the
+    row max on unscaled logits, which only a scale >= 0 preserves)."""
     return (x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.shape[1] == TOKENS
             and dim_head == DIM_HEAD and 1 <= heads <= 16
+            and 0.0 <= scale < math.inf
             and os.environ.get("PIXELSPLAT_B200_SELF_ATTENTION", "tf32") != "fp32")
 
 

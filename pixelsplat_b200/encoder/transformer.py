@@ -52,7 +52,7 @@ class Attention(nn.Module):
         if z is None:
             qkv = self.to_qkv(x)
             hooked = len(self.attend._forward_hooks) > 0 or len(self.attend._forward_pre_hooks) > 0
-            if not hooked and _satc.supported(qkv, self.heads, self.dim_head):
+            if not hooked and _satc.supported(qkv, self.heads, self.dim_head, self.scale):
                 # dense per-image self-attention on the tensor cores (csrc/self_attention_tc.cu)
                 return self.to_out(_satc.self_attention_tc(qkv, self.heads, self.scale))
             q, k, v = qkv.chunk(3, dim=-1)

@@ -13,13 +13,10 @@ import ctypes
 import pytest
 import torch
 
+from tests.attention_f64 import _tf32
+
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-
-def _tf32(t):
-    # cvt.rna.tf32.f32: nearest TF32, ties away from zero (sign-magnitude, so +0x1000 on the bits)
-    return ((t.contiguous().view(torch.int32) + 0x1000) & ~0x1FFF).view(torch.float32)
 
 
 def _split(qkv, heads):
