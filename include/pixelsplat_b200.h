@@ -705,6 +705,51 @@ PS_API int ps_clip_adam_workspace_bytes(const ps_clip_adam_desc *desc, size_t *o
 PS_API int ps_clip_adam_step(const ps_clip_adam_desc *desc, const ps_clip_adam_segment *segments,
                              const ps_clip_adam_state *state, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ---- PLY export: one scene's Gaussians as 3D Gaussian splatting vertex records (csrc/ply_export.cu) ---------------
+ * Writes desc->n_gaussians records of little-endian float32, one after the other, to `out` (the bytes that follow a
+ * PLY file's ASCII header).  With c = center[0..2] and s = scale[0] (device memory: the median of the means and the
+ * 0.95 quantile of the centred means' absolute values, so nothing is read back first) and M = desc->frame
+ * (row-major), every record starts x y z = M (mean - c) / s, nx ny nz = 0.
+ *   PS_PLY_REFERENCE  17 floats, the reference's export_ply: f_dc_0..2 = harmonics[g, :, 0], opacity = opacities[g]
+ *                     raw, scale_0..2 = log(scales[g] / s), rot_0..3 = wxyz of M R(q), q = rotations[g] (xyzw,
+ *                     normalised first).  `covariances` is not read; sh_degree must be 0.
+ *   PS_PLY_VIEWER     17 + 3 ((sh_degree + 1)^2 - 1) floats: f_dc_c, f_rest_{c ((d+1)^2 - 1) + k - 1} = (T h_c)_k with
+ *                     h_c = harmonics[g, c, :(d+1)^2] and T the block-diagonal sh_transform (blocks of degree 0..d,
+ *                     row-major, at float offsets 0, 1, 10, 35), opacity = logit(clamp(o, 1e-7, 1 - 1e-7)) in float64,
+ *                     and scale / rot from the eigendecomposition of M Sigma M^T / s^2 (cyclic Jacobi in float64 on
+ *                     the upper triangle of covariances[g], as the rasterizer reads it): scale_i = log sqrt(max(l_i,
+ *                     PS_PLY_MIN_EIGENVALUE)), rot = wxyz of the eigenvector matrix made proper (det +1), w >= 0.
+ *                     `scales` and `rotations` are not read.
+ * Both modes write rot with w >= 0.  Records are staged in shared memory and stored as 16-byte vectors; offsets are
+ * 64-bit.  No host synchronisation.  `harmonics` is [n, 3, sh_coeffs] with sh_coeffs >= (sh_degree + 1)^2, every
+ * other input is dense float32; `out` is 16-byte aligned.  Rejects a NULL desc, pointer or input the mode reads,
+ * an unknown mode, n_gaussians < 1, sh_degree outside [0, 3] (0 in reference mode), sh_coeffs < (sh_degree + 1)^2
+ * and a misaligned `out` with PS_ERR_INVALID_ARGUMENT before anything is enqueued. */
+#define PS_PLY_REFERENCE 0
+#define PS_PLY_VIEWER 1
+#define PS_PLY_SH_TRANSFORM_FLOATS 84   /* 1 + 9 + 25 + 49: degrees 0..3, the most the format holds */
+#define PS_PLY_MIN_EIGENVALUE 1e-20
+
+typedef struct {
+    int32_t mode;                       /* PS_PLY_* */
+    int32_t sh_degree;                  /* of the written record: 0..3 (viewer), 0 (reference) */
+    int32_t sh_coeffs;                  /* last dimension of harmonics */
+    int32_t reserved;
+    int64_t n_gaussians;
+    double frame[9];                    /* M, row-major */
+    float sh_transform[PS_PLY_SH_TRANSFORM_FLOATS];
+    const float *means;                 /* [n, 3] */
+    const float *covariances;           /* [n, 3, 3] (viewer) */
+    const float *scales;                /* [n, 3] (reference) */
+    const float *rotations;             /* [n, 4] xyzw (reference) */
+    const float *harmonics;             /* [n, 3, sh_coeffs] */
+    const float *opacities;             /* [n] */
+    const float *center;                /* [3] */
+    const float *scale;                 /* [1] */
+} ps_ply_desc;
+
+PS_API int ps_ply_pack(const ps_ply_desc *desc, float *out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -132,6 +132,18 @@ class ClipAdamState(ctypes.Structure):
     _fields_ = [("step", ctypes.c_void_p), ("grad_norm", ctypes.c_void_p)]
 
 
+PS_PLY_REFERENCE, PS_PLY_VIEWER = 0, 1
+PLY_SH_TRANSFORM_FLOATS = 84
+
+
+class PlyDesc(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("mode", "sh_degree", "sh_coeffs", "reserved")] + \
+        [("n_gaussians", ctypes.c_int64), ("frame", ctypes.c_double * 9),
+         ("sh_transform", ctypes.c_float * PLY_SH_TRANSFORM_FLOATS)] + \
+        [(n, ctypes.c_void_p) for n in ("means", "covariances", "scales", "rotations", "harmonics", "opacities",
+                                        "center", "scale")]
+
+
 class RasterCameraGrads(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in ("d_viewmatrix", "d_projmatrix", "d_campos", "d_tanfov", "workspace")] + \
         [("workspace_bytes", ctypes.c_size_t)]
@@ -155,7 +167,7 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_lpips_forward", "ps_lpips_backward", "ps_vit_attention_forward",
            "ps_vit_attention_backward_workspace_bytes", "ps_vit_attention_backward", "ps_image_resample",
            "ps_eval_images_workspace_bytes", "ps_eval_images", "ps_clip_adam_segment_chunks",
-           "ps_clip_adam_workspace_bytes", "ps_clip_adam_step")
+           "ps_clip_adam_workspace_bytes", "ps_clip_adam_step", "ps_ply_pack")
 
 
 class NativeLibraryMissing(ImportError):
@@ -263,6 +275,8 @@ def _load() -> ctypes.CDLL:
     lib.ps_clip_adam_step.argtypes = [P(ClipAdamDesc), ctypes.c_void_p, P(ClipAdamState), ctypes.c_void_p,
                                       ctypes.c_size_t, ctypes.c_void_p]
     lib.ps_clip_adam_step.restype = ctypes.c_int
+    lib.ps_ply_pack.argtypes = [P(PlyDesc), ctypes.c_void_p, ctypes.c_void_p]
+    lib.ps_ply_pack.restype = ctypes.c_int
     for f in ("ps_raster_sizes_query", "ps_raster_layout_query", "ps_raster_forward", "ps_raster_backward"):
         getattr(lib, f).restype = ctypes.c_int
     return lib
