@@ -377,6 +377,22 @@ PS_API int ps_epipolar_geometry(int32_t batch, int32_t views, int32_t grid_h, in
                                 const float *far_plane /* [b,v] */, float *segments, uint8_t *valid,
                                 float *rel_disparity, float *t_range, void *stream);
 
+/* View overlap of one step of the evaluation-index walk (EvaluationIndexGenerator.test_step,
+ * src/evaluation/evaluation_index_generator.py in the reference).  Over one scene's cameras (extrinsics [views,4,4]
+ * c2w, normalised intrinsics [views,3,3]) and the grid_h x grid_w ray grid at pixel centres, for each candidate
+ * frame k = first + i, i < count:
+ *   counts[i, 0] = rays of frame k whose unbounded projection (project_rays with near = far = None) overlaps the
+ *                  image of frame `context`;
+ *   counts[i, 1] = rays of frame `context` that overlap the image of frame k.
+ * counts [count, 2] int32 is overwritten (zeroed on the stream, then accumulated with one integer atomic per CTA,
+ * so the result does not depend on scheduling).  The geometry is ps_epipolar_geometry's, in float64.  One launch,
+ * graph-capturable, no host synchronisation.  PS_ERR_INVALID_ARGUMENT for a count below 1 (views, grid, count), a
+ * NULL pointer, or a context / candidate range outside [0, views); PS_ERR_UNSUPPORTED when count > 65535 or
+ * grid_h * grid_w >= 2^31; both before anything is enqueued. */
+PS_API int ps_view_overlap(int32_t views, int32_t grid_h, int32_t grid_w, const float *extrinsics,
+                           const float *intrinsics, int32_t context, int32_t first, int32_t count, int32_t *counts,
+                           void *stream);
+
 /* z [N,heads,128] = sum_s a_s f_s;  e [N,heads,pe_dim] = sum_s a_s PE(rd_s);
  * mass [N,heads,v-1] = per-other-view attention mass (or NULL);  lse [N,heads] log-sum-exp. */
 PS_API int ps_epipolar_attention_forward(const ps_epipolar_desc *desc, const ps_epipolar_inputs *in,

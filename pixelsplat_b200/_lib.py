@@ -167,7 +167,7 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_lpips_forward", "ps_lpips_backward", "ps_vit_attention_forward",
            "ps_vit_attention_backward_workspace_bytes", "ps_vit_attention_backward", "ps_image_resample",
            "ps_eval_images_workspace_bytes", "ps_eval_images", "ps_clip_adam_segment_chunks",
-           "ps_clip_adam_workspace_bytes", "ps_clip_adam_step", "ps_ply_pack")
+           "ps_clip_adam_workspace_bytes", "ps_clip_adam_step", "ps_ply_pack", "ps_view_overlap")
 
 
 class NativeLibraryMissing(ImportError):
@@ -214,6 +214,9 @@ def _load() -> ctypes.CDLL:
     lib.ps_timing_read.restype = ctypes.c_int
     lib.ps_epipolar_geometry.argtypes = [ctypes.c_int32] * 5 + [ctypes.c_void_p] * 9
     lib.ps_epipolar_geometry.restype = ctypes.c_int
+    lib.ps_view_overlap.argtypes = [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 2 + [ctypes.c_int32] * 3 + \
+        [ctypes.c_void_p] * 2
+    lib.ps_view_overlap.restype = ctypes.c_int
     lib.ps_epipolar_attention_forward.argtypes = [P(EpipolarDesc), P(EpipolarInputs)] + [ctypes.c_void_p] * 5
     lib.ps_epipolar_attention_forward.restype = ctypes.c_int
     lib.ps_epipolar_attention_backward.argtypes = [P(EpipolarDesc), P(EpipolarInputs)] + [ctypes.c_void_p] * 10

@@ -91,10 +91,10 @@ __device__ __forceinline__ double nan_to_num(double v, double pinf, double ninf)
     return v;
 }
 
-// Projection of the point o + t d (camera space) with the reference's guards.
-__device__ Proj point_proj(const double *k, const double *o, const double *d, double t) {
+// Projection of the camera-space point p, with the ray parameter t it stands for, with the reference's guards
+// (project_camera_space: p / (p_z + eps32), nan_to_num(+-1e8)).
+__device__ Proj project_point(const double *k, double px, double py, double pz, double t) {
     const double eps32 = 1.1920928955078125e-07;
-    const double px = o[0] + t * d[0], py = o[1] + t * d[1], pz = o[2] + t * d[2];
     const double den = pz + eps32;
     const double qx = nan_to_num(px / den, 1e8, -1e8), qy = nan_to_num(py / den, 1e8, -1e8),
                  qz = nan_to_num(pz / den, 1e8, -1e8);
@@ -104,6 +104,69 @@ __device__ Proj point_proj(const double *k, const double *o, const double *d, do
     p.y = k[3] * qx + k[4] * qy + k[5] * qz;
     p.valid = in_bounds(p.x, p.y) && (pz > -kEps) && (t > -kEps);
     return p;
+}
+
+// Projection of the point o + t d (camera space): project_rays' bounded near / far branch.
+__device__ Proj point_proj(const double *k, const double *o, const double *d, double t) {
+    return project_point(k, o[0] + t * d[0], o[1] + t * d[1], o[2] + t * d[2], t);
+}
+
+// project_rays' unbounded near branch, the projection at zero depth: an origin within kEps of the camera centre is
+// replaced by the direction; any other origin with z < kEps projects as invalid.
+__device__ Proj zero_depth_proj(const double *k, const double *o, const double *d) {
+    const bool at_camera = sqrt(o[0] * o[0] + o[1] * o[1] + o[2] * o[2]) < kEps;
+    const double *p = at_camera ? d : o;
+    Proj r = project_point(k, p[0], p[1], p[2], 0.0);
+    if (o[2] < kEps && !at_camera) r.valid = false;
+    return r;
+}
+
+// project_rays' unbounded far branch, the projection of the direction at infinity.
+__device__ Proj infinity_proj(const double *k, const double *d) {
+    return project_point(k, d[0], d[1], d[2], INFINITY);
+}
+
+// World ray (origin ow, unit direction dw) through the centre of cell r of an h x w grid of camera `cam`
+// (sample_image_grid + get_world_rays).
+__device__ __forceinline__ void world_ray(const EpiCam &cam, int r, int h, int w, double *ow, double *dw) {
+    const double x = ((r % w) + 0.5) / w, y = ((r / w) + 0.5) / h;
+    double dc[3];
+    for (int i = 0; i < 3; ++i) dc[i] = cam.kinv[3 * i] * x + cam.kinv[3 * i + 1] * y + cam.kinv[3 * i + 2];
+    const double dn = sqrt(dc[0] * dc[0] + dc[1] * dc[1] + dc[2] * dc[2]);
+    for (int i = 0; i < 3; ++i) dc[i] /= dn;
+    for (int i = 0; i < 3; ++i) {
+        dw[i] = cam.e[4 * i] * dc[0] + cam.e[4 * i + 1] * dc[1] + cam.e[4 * i + 2] * dc[2];
+        ow[i] = cam.e[4 * i + 3];
+    }
+}
+
+// A world ray in camera `cam`'s space.
+__device__ __forceinline__ void to_camera(const EpiCam &cam, const double *ow, const double *dw, double *oc,
+                                          double *dcam) {
+    for (int i = 0; i < 3; ++i) {
+        const double *m = cam.w2c + 4 * i;
+        oc[i] = m[0] * ow[0] + m[1] * ow[1] + m[2] * ow[2] + m[3];
+        dcam[i] = m[0] * dw[0] + m[1] * dw[1] + m[2] * dw[2];
+    }
+}
+
+// The ray's intersections with the four lines of the image frame: the first minimum (lo) and first maximum (hi) of
+// t over the valid ones, invalid ones ranked +inf / -inf (project_rays' _compare_projections); tmin / tmax are
+// those ranked values.
+__device__ __forceinline__ void frame_extremes(const double *k, const double *oc, const double *dcam, Proj &lo,
+                                               Proj &hi, double &tmin, double &tmax) {
+    Proj fr[4] = {frame_hit(k, oc, dcam, 0, 0.0), frame_hit(k, oc, dcam, 0, 1.0),
+                  frame_hit(k, oc, dcam, 1, 0.0), frame_hit(k, oc, dcam, 1, 1.0)};
+    lo = fr[0];
+    hi = fr[0];
+    tmin = fr[0].valid ? fr[0].t : INFINITY;
+    tmax = fr[0].valid ? fr[0].t : -INFINITY;
+#pragma unroll
+    for (int i = 1; i < 4; ++i) {
+        const double tlo = fr[i].valid ? fr[i].t : INFINITY, thi = fr[i].valid ? fr[i].t : -INFINITY;
+        if (tlo < tmin) { tmin = tlo; lo = fr[i]; }
+        if (thi > tmax) { tmax = thi; hi = fr[i]; }
+    }
 }
 
 __global__ void __launch_bounds__(128)
@@ -124,35 +187,15 @@ k_epipolar_geometry(int B, int V, int h, int w, int S, const float *__restrict__
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     const double nearv = (double)near_[b * V + v], farv = (double)far_[b * V + v];
 
-    // --- world ray through the centre of ray-grid cell r of view v
-    const double x = ((r % w) + 0.5) / w, y = ((r / w) + 0.5) / h;
-    double dc[3], dw[3], ow[3];
-    for (int i = 0; i < 3; ++i) dc[i] = cam_q.kinv[3 * i] * x + cam_q.kinv[3 * i + 1] * y + cam_q.kinv[3 * i + 2];
-    const double dn = sqrt(dc[0] * dc[0] + dc[1] * dc[1] + dc[2] * dc[2]);
-    for (int i = 0; i < 3; ++i) dc[i] /= dn;
-    for (int i = 0; i < 3; ++i) {
-        dw[i] = cam_q.e[4 * i] * dc[0] + cam_q.e[4 * i + 1] * dc[1] + cam_q.e[4 * i + 2] * dc[2];
-        ow[i] = cam_q.e[4 * i + 3];
-    }
-    // --- into the other camera's space
-    double oc[3], dcam[3];
-    for (int i = 0; i < 3; ++i) {
-        const double *m = cam_o.w2c + 4 * i;
-        oc[i] = m[0] * ow[0] + m[1] * ow[1] + m[2] * ow[2] + m[3];
-        dcam[i] = m[0] * dw[0] + m[1] * dw[1] + m[2] * dw[2];
-    }
-    // --- frame intersections: first-minimum / first-maximum of t over the valid ones
-    Proj fr[4] = {frame_hit(cam_o.k, oc, dcam, 0, 0.0), frame_hit(cam_o.k, oc, dcam, 0, 1.0),
-                  frame_hit(cam_o.k, oc, dcam, 1, 0.0), frame_hit(cam_o.k, oc, dcam, 1, 1.0)};
-    int imin = 0, imax = 0;
-    double tmin = fr[0].valid ? fr[0].t : INFINITY, tmax = fr[0].valid ? fr[0].t : -INFINITY;
-    for (int i = 1; i < 4; ++i) {
-        const double tlo = fr[i].valid ? fr[i].t : INFINITY, thi = fr[i].valid ? fr[i].t : -INFINITY;
-        if (tlo < tmin) { tmin = tlo; imin = i; }
-        if (thi > tmax) { tmax = thi; imax = i; }
-    }
+    // --- world ray through the centre of ray-grid cell r of view v, into the other camera's space
+    double dw[3], ow[3], oc[3], dcam[3];
+    world_ray(cam_q, r, h, w, ow, dw);
+    to_camera(cam_o, ow, dw, oc, dcam);
+    Proj frame_lo, frame_hi;
+    double tmin, tmax;
+    frame_extremes(cam_o.k, oc, dcam, frame_lo, frame_hi, tmin, tmax);
     const Proj pn = point_proj(cam_o.k, oc, dcam, nearv), pf = point_proj(cam_o.k, oc, dcam, farv);
-    Proj lo = pn.valid ? pn : fr[imin], hi = pf.valid ? pf : fr[imax];
+    Proj lo = pn.valid ? pn : frame_lo, hi = pf.valid ? pf : frame_hi;
     if (!pn.valid) lo.t = tmin;
     if (!pf.valid) hi.t = tmax;
     const bool overlaps = lo.valid && hi.valid;
@@ -228,5 +271,78 @@ extern "C" PS_API int ps_epipolar_geometry(int32_t batch, int32_t views, int32_t
         batch, views, grid_h, grid_w, samples, extrinsics, intrinsics, near_plane, far_plane, segments, valid,
         rel_disparity, t_range);
     PS_LAUNCH_CHECK("k_epipolar_geometry");
+    return PS_OK;
+}
+
+namespace ps {
+
+constexpr int kOverlapThreads = 128;
+constexpr int kOverlapRaysPerThread = 8;
+
+// View overlap of an evaluation-index walk (EvaluationIndexGenerator.test_step): for candidate frame k = first +
+// blockIdx.y and direction blockIdx.z, the number of rays of the source camera's h x w grid whose unbounded
+// projection (project_rays without near / far) overlaps the destination camera's image.  Direction 0 sends the
+// rays of k into camera `context`, direction 1 the rays of `context` into camera k.  Each thread counts up to
+// kOverlapRaysPerThread rays; the CTA's count is a warp reduction plus one integer atomic, so the result does not
+// depend on the order the CTAs run in.
+__global__ void __launch_bounds__(kOverlapThreads)
+k_view_overlap(int h, int w, int context, int first, const float *__restrict__ extr, const float *__restrict__ intr,
+               int *__restrict__ counts) {
+    __shared__ EpiCam cam_src, cam_dst;
+    __shared__ int warp_count[kOverlapThreads / 32];
+    const int k = first + blockIdx.y, dir = blockIdx.z;
+    const int src = dir == 0 ? k : context, dst = dir == 0 ? context : k;
+    if (threadIdx.x == 0) load_cam(extr + 16 * src, intr + 9 * src, cam_src);
+    if (threadIdx.x == 32) load_cam(extr + 16 * dst, intr + 9 * dst, cam_dst);
+    __syncthreads();
+    const int R = h * w;
+    int n = 0;
+    for (int r = blockIdx.x * kOverlapThreads + threadIdx.x; r < R; r += gridDim.x * kOverlapThreads) {
+        double ow[3], dw[3], oc[3], dcam[3];
+        world_ray(cam_src, r, h, w, ow, dw);
+        to_camera(cam_dst, ow, dw, oc, dcam);
+        Proj frame_lo, frame_hi;
+        double tmin, tmax;
+        frame_extremes(cam_dst.k, oc, dcam, frame_lo, frame_hi, tmin, tmax);
+        const bool lo = zero_depth_proj(cam_dst.k, oc, dcam).valid || frame_lo.valid;
+        const bool hi = infinity_proj(cam_dst.k, dcam).valid || frame_hi.valid;
+        n += lo && hi;
+    }
+    n = __reduce_add_sync(0xffffffffu, n);
+    if ((threadIdx.x & 31) == 0) warp_count[threadIdx.x >> 5] = n;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int total = 0;
+        for (int i = 0; i < kOverlapThreads / 32; ++i) total += warp_count[i];
+        atomicAdd(counts + 2 * blockIdx.y + dir, total);
+    }
+}
+
+}  // namespace ps
+
+extern "C" PS_API int ps_view_overlap(int32_t views, int32_t grid_h, int32_t grid_w, const float *extrinsics,
+                                      const float *intrinsics, int32_t context, int32_t first, int32_t count,
+                                      int32_t *counts, void *stream) {
+    if (views < 1 || grid_h < 1 || grid_w < 1 || count < 1 || !extrinsics || !intrinsics || !counts) {
+        ps::set_error("ps_view_overlap: bad argument (views, grid and count must be >= 1, pointers non-NULL)");
+        return PS_ERR_INVALID_ARGUMENT;
+    }
+    if (context < 0 || context >= views || first < 0 || first > views - count) {
+        ps::set_error("ps_view_overlap: the context frame and the candidate range must lie in [0, views)");
+        return PS_ERR_INVALID_ARGUMENT;
+    }
+    // one block row per candidate on the grid's y axis, and a 32-bit ray index
+    const int64_t rays = (int64_t)grid_h * grid_w;
+    if (count > 65535 || rays > INT32_MAX) {
+        ps::set_error("ps_view_overlap: count must be <= 65535 and grid_h * grid_w < 2^31");
+        return PS_ERR_UNSUPPORTED;
+    }
+    const cudaStream_t s = static_cast<cudaStream_t>(stream);
+    PS_CUDA_CHECK(cudaMemsetAsync(counts, 0, sizeof(int32_t) * 2 * (size_t)count, s));
+    const int64_t per_block = (int64_t)ps::kOverlapThreads * ps::kOverlapRaysPerThread;
+    dim3 grid((unsigned)((rays + per_block - 1) / per_block), (unsigned)count, 2);
+    ps::k_view_overlap<<<grid, ps::kOverlapThreads, 0, s>>>(grid_h, grid_w, context, first, extrinsics, intrinsics,
+                                                             counts);
+    PS_LAUNCH_CHECK("k_view_overlap");
     return PS_OK;
 }

@@ -141,6 +141,11 @@ def resample_u8(images: Tensor, scaled: tuple[int, int], crop: tuple[int, int, i
     return out
 
 
+def crop_shim_intrinsics(intrinsics: Tensor, in_shape: tuple[int, int], shape: tuple[int, int]) -> Tensor:
+    """The intrinsics apply_crop_shim gives views of in_shape (h, w) cropped to shape, without the images."""
+    return _crop_intrinsics(intrinsics, scaled_shape(*in_shape, shape), shape)
+
+
 def _crop_intrinsics(intrinsics: Tensor, scaled: tuple[int, int], shape: tuple[int, int]) -> Tensor:
     """center_crop's intrinsics update, with the rescaled size as its input size."""
     intrinsics = intrinsics.clone()

@@ -6,6 +6,10 @@ examples.  What it yields differs in one way: each view's image is the decoded u
 reference), uncropped, and a "flip" flag records the augmentation coin; the extrinsics are already reflected.
 `pixelsplat_b200.data.device_shim` then flips, resizes and crops the batch on the GPU, which gives the images
 and intrinsics the reference's loader gives, bit for bit.
+
+With `cameras_only=True` (the evaluation-index generator, which reads scenes through the reference's `all` view
+sampler) it decodes no frame: each example is every frame's cameras, the scene key and the frame count, after the
+same skips, with the image shape read from each JPEG header.
 """
 from __future__ import annotations
 
@@ -80,11 +84,13 @@ class DatasetRE10k(IterableDataset):
     near: float = 0.1
     far: float = 1000.0
 
-    def __init__(self, cfg: DatasetRE10kCfg, stage: Stage, view_sampler: ViewSampler) -> None:
+    def __init__(self, cfg: DatasetRE10kCfg, stage: Stage, view_sampler: ViewSampler | None,
+                 cameras_only: bool = False) -> None:
         super().__init__()
         self.cfg = cfg
         self.stage = stage
         self.view_sampler = view_sampler
+        self.cameras_only = cameras_only
         self.chunks = []
         for root in cfg.roots:
             root = Path(root) / self.data_stage
@@ -120,6 +126,8 @@ class DatasetRE10k(IterableDataset):
 
     def convert_example(self, example: dict) -> dict | None:
         """One chunk entry -> the yielded example, or None where the reference skips it."""
+        if self.cameras_only:
+            return self.convert_cameras(example)
         extrinsics, intrinsics = self.convert_poses(example["cameras"])
         scene = example["key"]
         try:
@@ -163,6 +171,29 @@ class DatasetRE10k(IterableDataset):
                 out[v]["extrinsics"] = reflect_extrinsics(out[v]["extrinsics"])
             out["flip"] = torch.tensor(True)
         return out
+
+    def convert_cameras(self, example: dict) -> dict | None:
+        """The `all` sampler's example without its images: {"extrinsics" [v, 4, 4], "intrinsics" [v, 3, 3] (as
+        stored, before the crop shim), "scene", "num_frames"}, or None where the reference skips it: a field of view
+        over max_fov, fewer images than cameras (its IndexError), a frame that would not decode to IMAGE_SHAPE, or
+        with exactly two frames, an insufficient baseline (the two-view rescale then applies)."""
+        extrinsics, intrinsics = self.convert_poses(example["cameras"])
+        scene, v = example["key"], extrinsics.shape[0]
+        if (get_fov(intrinsics).rad2deg() > self.cfg.max_fov).any() or len(example["images"]) < v:
+            return None
+        for i in range(v):
+            image = Image.open(BytesIO(example["images"][i].numpy().tobytes()))   # reads the header only
+            if (image.size[1], image.size[0], len(image.getbands())) != IMAGE_SHAPE:
+                log.info("Skipped bad example %s: an image is not %s.", scene, IMAGE_SHAPE)
+                return None
+        if v == 2 and self.cfg.make_baseline_1:
+            a, b = extrinsics[:, :3, 3]
+            scale = (a - b).norm()
+            if scale < self.cfg.baseline_epsilon:
+                log.info("Skipped %s because of insufficient baseline %.6f", scene, float(scale))
+                return None
+            extrinsics[:, :3, 3] /= scale
+        return {"extrinsics": extrinsics, "intrinsics": intrinsics, "scene": scene, "num_frames": v}
 
     def convert_poses(self, poses: Tensor) -> tuple[Tensor, Tensor]:
         """[b, 18] RE10k cameras -> (camera-to-world [b, 4, 4], normalised intrinsics [b, 3, 3])."""

@@ -20,6 +20,13 @@ is the reference's compute_metrics script: it scores saved frame directories of 
 encodes the test scenes as the test step does and writes each scene's Gaussians to <output>/<scene>.ply: by default
 in the viewer format (pixelsplat_b200.ply_export.export_gaussians_ply), or as the reference's export_ply writes them.
 
+    python -m pixelsplat_b200.evaluation generate-index --dataset-root datasets/re10k \
+        --output outputs/evaluation_index_re10k [--video]
+
+is the reference's generate_evaluation_index script: it writes <output>/evaluation_index.json (a context pair and
+target frames per test scene, or null), and with --video <output>/evaluation_index_video.json, where the targets are
+every frame between the pair.
+
 --preset names the experiment the checkpoint was trained with: re10k, acid, re10k_depth_loss, the paper's ablations
 re10k_ablation_no_epipolar_transformer / _no_probabilistic_sampling / _no_depth_encoding, or re10k_3_view (three
 context views: the index's two and the frame halfway between them).
@@ -194,9 +201,53 @@ def export_ply(argv: list[str]) -> list[Path]:
     return written
 
 
+def parse_generate_index(argv: list[str]) -> argparse.Namespace:
+    from .index_generator import EvaluationIndexGeneratorCfg
+    d = EvaluationIndexGeneratorCfg()
+    p = argparse.ArgumentParser(prog="python -m pixelsplat_b200.evaluation generate-index",
+                                description="Pick a context pair and target frames for every test scene.")
+    p.add_argument("--dataset-root", type=Path, required=True, help="dataset root holding test/index.json")
+    p.add_argument("--output", type=Path, required=True, help="directory of evaluation_index.json")
+    p.add_argument("--num-target-views", type=int, default=d.num_target_views, help="target frames per scene")
+    p.add_argument("--min-overlap", type=float, default=d.min_overlap, help="least overlap of a context pair")
+    p.add_argument("--max-overlap", type=float, default=d.max_overlap, help="largest overlap of a context pair")
+    p.add_argument("--min-distance", type=int, default=d.min_distance, help="least frame gap of a context pair")
+    p.add_argument("--max-distance", type=int, default=d.max_distance,
+                   help="frame gap past which a walk stops (the first frame past it is still a candidate)")
+    p.add_argument("--seed", type=int, default=d.seed, help="seed of the generator that draws every choice")
+    p.add_argument("--num-workers", type=int, default=8,
+                   help="DataLoader workers (the reference's: 8).  The scene order, and so the index, depends on it: "
+                        "keep 8 to reproduce the reference's index")
+    p.add_argument("--video", action="store_true",
+                   help="also write evaluation_index_video.json (every frame between the pair is a target)")
+    args = p.parse_args(argv)
+    if args.num_workers < 0:
+        p.error("--num-workers must be >= 0")
+    try:
+        args.cfg = EvaluationIndexGeneratorCfg(args.num_target_views, args.min_distance, args.max_distance,
+                                               args.min_overlap, args.max_overlap, args.output, args.seed)
+    except ValueError as e:
+        p.error(str(e))
+    return args
+
+
+def generate_index(argv: list[str]) -> list[Path]:
+    args = parse_generate_index(argv)
+    from . import index_generator as ig
+    from .presets import IMAGE_SHAPE
+    device = torch.device("cuda", torch.cuda.current_device())
+    index = ig.generate_index(ig.camera_loader(args.dataset_root, args.num_workers), *IMAGE_SHAPE, args.cfg, device)
+    written = ig.save_index(index, args.output, video=args.video)
+    found = sum(v is not None for v in index.values())
+    print(f"{len(index)} scenes, {found} with a context pair: wrote " + ", ".join(str(p) for p in written))
+    return written
+
+
 def main(argv: list[str] | None = None) -> None:
     argv = sys.argv[1:] if argv is None else argv
-    if argv and argv[0] == "compute-metrics":
+    if argv and argv[0] == "generate-index":
+        generate_index(argv[1:])
+    elif argv and argv[0] == "compute-metrics":
         compute_metrics(argv[1:])
     elif argv and argv[0] == "export-ply":
         export_ply(argv[1:])
