@@ -27,6 +27,14 @@ is the reference's generate_evaluation_index script: it writes <output>/evaluati
 target frames per test scene, or null), and with --video <output>/evaluation_index_video.json, where the targets are
 every frame between the pair.
 
+    python -m pixelsplat_b200.evaluation render-video --dataset-root datasets/re10k \
+        --index assets/evaluation_index_re10k.json --checkpoint checkpoints/re10k.ckpt --preset re10k \
+        --output outputs/video/re10k [--scene NAME ...] [--video rgb wobble interpolation_exagerrated]
+
+renders the reference's validation videos of the test scenes (pixelsplat_b200.video) and writes
+<output>/<scene>/<name>.mp4: by default rgb (context view 0 to view 1) and wobble; interpolation_exagerrated on
+request.  With three context views, rgb ends at the index's first target and the other two are skipped.
+
 --preset names the experiment the checkpoint was trained with: re10k, acid, re10k_depth_loss, the paper's ablations
 re10k_ablation_no_epipolar_transformer / _no_probabilistic_sampling / _no_depth_encoding, or re10k_3_view (three
 context views: the index's two and the frame halfway between them).
@@ -201,6 +209,67 @@ def export_ply(argv: list[str]) -> list[Path]:
     return written
 
 
+def parse_render_video(argv: list[str]) -> argparse.Namespace:
+    from ..video import VALIDATION_VIDEOS, VIDEOS
+    from .presets import PRESETS
+    p = argparse.ArgumentParser(prog="python -m pixelsplat_b200.evaluation render-video",
+                                description="Render the interpolation and wobble videos of test scenes as MP4.")
+    _data(p)
+    p.add_argument("--checkpoint", type=Path, required=True, help="a pixelSplat Lightning checkpoint (.ckpt)")
+    p.add_argument("--preset", choices=PRESETS, default="re10k",
+                   help="the experiment the checkpoint was trained with (default: re10k)")
+    p.add_argument("--output", type=Path, required=True, help="directory of the <scene>/<video>.mp4 files")
+    p.add_argument("--scene", action="append", default=None, metavar="NAME",
+                   help="render only this scene (repeatable; default: every test scene)")
+    p.add_argument("--video", nargs="+", choices=tuple(VIDEOS), default=list(VALIDATION_VIDEOS),
+                   help="videos to render (default: rgb wobble, the reference's validation videos)")
+    args = p.parse_args(argv)
+    args.video = list(dict.fromkeys(args.video))
+    return args
+
+
+def render_videos(argv: list[str]) -> list[Path]:
+    """The test step's data path; torch's generators seeded from --seed before each scene, so a scene's frames do
+    not depend on which scenes are rendered; one encoder trunk per scene and the videos in the order asked."""
+    args = parse_render_video(argv)
+    from ..data import device_shim
+    from ..video import render_video, write_mp4
+    from .presets import IMAGE_SHAPE, SEED, build_model
+    device = torch.device("cuda", torch.cuda.current_device())
+    cfg, loader = _loader(args, args.preset)
+    encoder, decoder = build_model(args.preset, cfg)
+    step = load_preset_checkpoint(args.checkpoint, encoder, args.preset)
+    print(f"Loaded {args.checkpoint} (trained for {step} steps).")
+    encoder, decoder = encoder.to(device).eval(), decoder.to(device)
+    data_shim = encoder.get_data_shim()
+    wanted = None if args.scene is None else set(args.scene)
+    seed = SEED if args.seed is None else args.seed
+    written: list[Path] = []
+    seen: set[str] = set()
+    with torch.no_grad():
+        for batch in loader:
+            (scene,) = batch["scene"]
+            if wanted is not None and scene not in wanted:
+                continue
+            seen.add(scene)
+            torch.manual_seed(seed)
+            batch = data_shim(device_shim(batch, IMAGE_SHAPE, device))
+            features, _ = encoder.trunk(batch["context"])
+            for name in args.video:
+                frames = render_video(encoder, decoder, batch["context"], batch["target"], name, 0, features)
+                if frames is None:
+                    print(f"{scene}: {name} needs two context views; skipped")
+                    continue
+                written.append(write_mp4(frames.numpy(), args.output / scene / f"{name}.mp4"))
+            if wanted is not None and not wanted - seen:
+                break
+    print(f"Wrote {len(written)} videos to {args.output}.")
+    missing = sorted(wanted - seen) if wanted is not None else []
+    if missing:
+        raise SystemExit(f"evaluation render-video: no test scene named {', '.join(missing)}")
+    return written
+
+
 def parse_generate_index(argv: list[str]) -> argparse.Namespace:
     from .index_generator import EvaluationIndexGeneratorCfg
     d = EvaluationIndexGeneratorCfg()
@@ -251,6 +320,8 @@ def main(argv: list[str] | None = None) -> None:
         compute_metrics(argv[1:])
     elif argv and argv[0] == "export-ply":
         export_ply(argv[1:])
+    elif argv and argv[0] == "render-video":
+        render_videos(argv[1:])
     else:
         evaluate(argv)
 

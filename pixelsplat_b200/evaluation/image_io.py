@@ -29,6 +29,28 @@ def quantise(image: Tensor) -> Tensor:
     return frames if batched else frames[0]
 
 
+def comparison_layout(*columns, gap: int = 8, border: int = 8) -> Tensor:
+    """The reference's comparison layout without its text labels, add_border(hcat(vcat(*a), vcat(*b), ...)): each
+    column a sequence of views [..., 3, h, w] (a tensor [v, ..., 3, h, w] or a tuple) stacked top to bottom with `gap`
+    rows between views, the columns side by side with `gap` columns between them and aligned to the top, all inside a
+    `border`.  Gaps, padding and border are white: 1.0, or 255 for uint8 views.  Leading dimensions (the frames of a
+    video) are laid out alike.  Returns [..., 3, H, W] in the views' dtype, on their device."""
+    first = columns[0][0]
+    height = max(len(c) * c[0].shape[-2] + (len(c) - 1) * gap for c in columns)
+    width = sum(c[0].shape[-1] for c in columns) + (len(columns) - 1) * gap
+    white = 255 if first.dtype == torch.uint8 else 1.0
+    out = torch.full((*first.shape[:-3], 3, height + 2 * border, width + 2 * border), white, dtype=first.dtype,
+                     device=first.device)
+    x = border
+    for column in columns:
+        h, w = column[0].shape[-2:]
+        for i, view in enumerate(column):
+            y = border + i * (h + gap)
+            out[..., y:y + h, x:x + w] = view
+        x += w + gap
+    return out
+
+
 def prep_image(image: Tensor) -> np.ndarray:
     """The reference's prep_image: [h, w], [c, h, w] or [b, c, h, w] (c = 1, 3 or 4; batches side by side) ->
     uint8 [h, w, c'] on the host, c' = 3 or 4."""

@@ -11,7 +11,8 @@ it): on rank 0, before the first step and after every 250th, one scene of the te
 and deterministically, scored with the float PSNR / SSIM / LPIPS of its renders (`<output>/validation.jsonl`) and
 drawn as context | ground truth | probabilistic | deterministic (`<output>/validation/comparison_{step:0>6}.png`).
 It needs `<dataset-root>/test/` and the LPIPS weights.  Validation draws from its own seeded generators, so the
-training's numbers are the same with it on or off.
+training's numbers are the same with it on or off.  `--val-videos` adds the reference's validation videos to each
+validation: `<output>/validation/video/rgb/{step:0>6}.mp4` and, with two context views, `.../wobble/...`.
 
 On several GPUs, one process per GPU:
 
@@ -53,6 +54,9 @@ def parse(argv: list[str]) -> argparse.Namespace:
                    help=f"validate on one scene of <dataset-root>/test before the first step and every N steps (the "
                         f"reference's val_check_interval is {VAL_EVERY}); writes <output>/validation.jsonl and "
                         f"<output>/validation/*.png.  0 (default): no validation")
+    p.add_argument("--val-videos", action="store_true",
+                   help="with --val-every: also render the rgb and wobble videos of each validation scene to "
+                        "<output>/validation/video/{rgb,wobble}/{step:0>6}.mp4")
     p.add_argument("--resume", type=Path, default=None, help="a checkpoint of this command or of the reference")
     p.add_argument("--backbone-weights", type=Path, nargs=2, default=None, metavar=("VIT", "RESNET"),
                    help="DINO's released ViT and ResNet-50 files")
@@ -64,7 +68,10 @@ def parse(argv: list[str]) -> argparse.Namespace:
                    help="torch.use_deterministic_algorithms(True, warn_only=True): every kernel of this package and "
                         "the optimiser sum in a fixed order; torch warns about the one op left without a "
                         "deterministic backward, the backbone's F.interpolate")
-    return p.parse_args(argv)
+    args = p.parse_args(argv)
+    if args.val_videos and args.val_every == 0:
+        p.error("--val-videos renders the videos of each validation; it needs --val-every N > 0")
+    return args
 
 
 def _worker_init_fn(worker_id: int) -> None:
@@ -141,7 +148,8 @@ def main(argv: list[str] | None = None) -> list[dict]:
     try:
         return trainer.fit(loader, preset.max_steps if args.max_steps is None else args.max_steps, args.output,
                            preset.checkpoint_every if args.checkpoint_every is None else args.checkpoint_every,
-                           args.log_every, log=say, validation=validation, val_every=args.val_every)
+                           args.log_every, log=say, validation=validation, val_every=args.val_every,
+                           val_videos=args.val_videos)
     finally:
         if args.deterministic:
             torch.use_deterministic_algorithms(False)

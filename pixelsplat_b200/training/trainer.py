@@ -33,10 +33,11 @@ from torch import Tensor, nn
 from ..data import StepTracker, device_shim
 from ..encoder.encoder_tail import EncoderEpipolarTail
 from ..evaluation.checkpoint import load_checkpoint, read_checkpoint, save_checkpoint
-from ..evaluation.image_io import save_image
+from ..evaluation.image_io import comparison_layout, save_image
 from ..loss import compute_psnr, compute_ssim, psnr_from_sse
 from ..optim import ClipAdam
 from ..parallel import GradientReducer, env_rank_world
+from ..video import VALIDATION_VIDEOS, render_video, write_mp4
 from .presets import VAL_SEED
 
 PHASES = ("forward", "backward", "allreduce", "optimizer")
@@ -57,24 +58,6 @@ def validation_rng(rank: int, global_step: int, device: torch.device | None = No
             with torch.cuda.device(device):
                 torch.cuda.manual_seed(seed)
         yield
-
-
-def comparison_layout(*columns: Tensor, gap: int = 8, border: int = 8) -> Tensor:
-    """The reference's comparison image without its text labels, add_border(hcat(vcat(*a), vcat(*b), ...)):
-    each column [v, 3, h, w] stacked top to bottom with `gap` rows between views, the columns side by side with `gap`
-    columns between them and aligned to the top, all inside a `border`.  Gaps, padding and border are 1.0 (white).
-    Returns float32 [3, H, W] on the columns' device."""
-    height = max(c.shape[0] * c.shape[2] + (c.shape[0] - 1) * gap for c in columns)
-    width = sum(c.shape[3] for c in columns) + (len(columns) - 1) * gap
-    out = torch.ones(3, height + 2 * border, width + 2 * border, dtype=torch.float32, device=columns[0].device)
-    x = border
-    for column in columns:
-        _, _, h, w = column.shape
-        for i, view in enumerate(column):
-            y = border + i * (h + gap)
-            out[:, y:y + h, x:x + w] = view
-        x += w + gap
-    return out
 
 
 def _module_modes(modules: Sequence[nn.Module]) -> list[tuple[nn.Module, bool]]:
@@ -172,7 +155,7 @@ class Trainer:
         return out
 
     # ---- validation -------------------------------------------------------------------------------------------
-    def validation_step(self, batch: dict) -> dict:
+    def validation_step(self, batch: dict, videos: Sequence[str] = ()) -> dict:
         """The reference's validation step on a device-resident batch of one scene (what `device_shim` returns): the
         data shim, then the encoder's trunk once and its tail twice, probabilistic and then deterministic (the
         reference's order; with two context views the trunk draws no random numbers, so the draws are the ones two
@@ -185,7 +168,11 @@ class Trainer:
         as the reference logs them, not of 8-bit frames as the evaluator scores them.  Returns `step`, `scene`,
         `context_index`, the six metrics (`psnr_probabilistic`, ..., `lpips_deterministic`) as host floats, `ms` and
         `phase_ms` (CUDA events), and `images`: the shimmed `context` and `target` views and the two renders, each
-        [v, 3, h, w] on the device."""
+        [v, 3, h, w] on the device.
+
+        `videos` names videos of `pixelsplat_b200.video` to render afterwards from the same trunk and in the same
+        generators, as the reference's validation step does: `videos` in the result maps each name to uint8 frames
+        [T, H, W, 3] on the host, leaving out those the number of context views rules out."""
         if self.lpips is None:
             raise ValueError("Trainer.validation_step: no Lpips module to score with; pass lpips= or train with "
                              "LossLpips")
@@ -219,6 +206,11 @@ class Trainer:
                                self.lpips(gt, color[tag], normalize=True)[:, 0, 0, 0].mean()]
                 ev[-1].record()
                 host = torch.stack([v.float() for v in values]).tolist()
+                rendered = {}
+                for name in videos:
+                    frames = render_video(self.encoder, self.decoder, ctx, tgt, name, self.global_step, features)
+                    if frames is not None:
+                        rendered[name] = frames
         finally:
             for m, mode in modes:
                 m.training = mode
@@ -227,6 +219,8 @@ class Trainer:
                **dict(zip(VAL_METRICS, host)), "ms": ev[0].elapsed_time(ev[-1]),
                "phase_ms": {p: ev[i].elapsed_time(ev[i + 1]) for i, p in enumerate(VAL_PHASES)}}
         out["images"] = {"context": ctx["image"][0], "target": gt, **color}
+        if videos:
+            out["videos"] = rendered
         return out
 
     # ---- checkpoints ------------------------------------------------------------------------------------------
@@ -260,7 +254,7 @@ class Trainer:
     # ---- the loop ---------------------------------------------------------------------------------------------
     def fit(self, batches: Iterable[dict], max_steps: int, output: Path | str | None = None,
             checkpoint_every: int = 5000, log_every: int = 10, log=print, validation: Iterable[dict] | None = None,
-            val_every: int = 0) -> list[dict]:
+            val_every: int = 0, val_videos: bool = False) -> list[dict]:
         """Steps over `batches` (a DataLoader over DatasetRE10k, or any iterable of its batches; it is restarted when
         exhausted, which counts an epoch) until `global_step == max_steps`.  Rank 0 writes a checkpoint every
         `checkpoint_every` steps and at the end, and one JSON line per `log_every` steps to `log` and
@@ -270,7 +264,9 @@ class Trainer:
         `val_every > 0`, rank 0 also runs `validation_step` before the first step (Lightning's sanity check) and after
         every step whose index is a multiple of `val_every`, after that step's checkpoint.  Each draws the next batch
         of one iterator over `validation`, restarted when exhausted, and writes one JSON line to
-        `<output>/validation.jsonl` and the comparison image to `<output>/validation/comparison_{step:0>6}.png`."""
+        `<output>/validation.jsonl` and the comparison image to `<output>/validation/comparison_{step:0>6}.png`.
+        With `val_videos`, each validation also renders the reference's validation videos (rgb, and wobble with two
+        context views) and writes `<output>/validation/video/{name}/{step:0>6}.mp4`."""
         output = None if output is None else Path(output)
         lines, log_file = [], None
         if output is not None and self.rank == 0:
@@ -288,8 +284,9 @@ class Trainer:
                     batch = next(val_iter, None)
             if batch is None:
                 raise ValueError("training: the validation loader yielded no batch")
-            result = self.validation_step(device_shim(batch, self.image_shape, self.device))
-            line = {k: v for k, v in result.items() if k not in ("images", "phase_ms")}
+            batch = device_shim(batch, self.image_shape, self.device)
+            result = self.validation_step(batch, VALIDATION_VIDEOS) if val_videos else self.validation_step(batch)
+            line = {k: v for k, v in result.items() if k not in ("images", "phase_ms", "videos")}
             if log is not None:
                 log(f"validation step {line['step']}; scene = {[line['scene']]}; context = {[line['context_index']]}")
                 log(json.dumps(line))
@@ -300,6 +297,8 @@ class Trainer:
                            output / "validation" / f"comparison_{line['step']:0>6}.png")
                 with (output / "validation.jsonl").open("a") as f:
                     f.write(json.dumps(line) + "\n")
+                for name, frames in result.get("videos", {}).items():
+                    write_mp4(frames.numpy(), output / "validation" / "video" / name / f"{line['step']:0>6}.mp4")
 
         try:
             if validating:
