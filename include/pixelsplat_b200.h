@@ -766,6 +766,54 @@ typedef struct {
 
 PS_API int ps_ply_pack(const ps_ply_desc *desc, float *out, void *stream);
 
+/* ---- PLY import: 3D Gaussian splatting vertex records as one scene's Gaussians (csrc/ply_import.cu) --------------
+ * Reads desc->n_gaussians records of n_props float32 each (a binary little-endian PLY body, uploaded unchanged) and
+ * writes the Gaussians layout.  Every column is given by index, so properties may come in any order and extra
+ * properties are ignored.  With the record's x, y, z = p, f_dc_c, f_rest_* (channel-major: f_rest_{c K + k - 1},
+ * K = (sh_degree + 1)^2 - 1), opacity o, scale_0..2 = l, rot_0..3 = q (wxyz), and the inverse frame (M = frame,
+ * row-major, s = scale, c = center):
+ *   means        [n, 3]            M^T p s + c
+ *   covariances  [n, 3, 3]         s^2 M^T R(q) diag(exp(2 l)) R(q)^T M, full and symmetric; q is normalised, and a
+ *                                  zero quaternion is the identity rotation
+ *   harmonics    [n, 3, sh_coeffs] per channel and degree l <= sh_degree, the block of sh_transform (degrees 0..3
+ *                                  at float offsets 0, 1, 10, 35, row-major) times the file's coefficients; zero
+ *                                  above sh_degree
+ *   opacities    [n]               sigmoid(o)
+ * All of it in float64, rounded once to float32.  Without a frame, pass M = I, s = 1, c = 0.  One thread per
+ * Gaussian, 64 per CTA; each CTA's records are staged in shared memory with 16-byte loads and its outputs stored as
+ * 16-byte vectors, every output entry once.  No host synchronisation.  Rejects a NULL desc or pointer,
+ * n_gaussians < 1, sh_degree outside [0, 3], sh_coeffs outside [(sh_degree + 1)^2, 25], n_props outside
+ * [1, PS_PLY_IMPORT_MAX_PROPERTIES], a column outside [0, n_props) and a pointer that is not 16-byte aligned with
+ * PS_ERR_INVALID_ARGUMENT before anything is enqueued. */
+#define PS_PLY_IMPORT_MAX_PROPERTIES 512
+#define PS_PLY_IMPORT_MAX_COEFFS 25
+
+typedef struct {
+    int32_t sh_degree;                  /* of the file: 0..3 */
+    int32_t sh_coeffs;                  /* last dimension of harmonics */
+    int32_t n_props;                    /* floats per record */
+    int32_t reserved;
+    int64_t n_gaussians;
+    int32_t col_xyz[3];                 /* column of each field in the record */
+    int32_t col_dc[3];
+    int32_t col_rest[45];               /* f_rest_0..; only the first 3 ((sh_degree + 1)^2 - 1) are read */
+    int32_t col_opacity;
+    int32_t col_scale[3];
+    int32_t col_rot[4];
+    int32_t reserved2;
+    double frame[9];                    /* M, row-major */
+    double center[3];                   /* c */
+    double scale;                       /* s */
+    float sh_transform[PS_PLY_SH_TRANSFORM_FLOATS];
+    const float *records;               /* [n, n_props] */
+    float *means;                       /* [n, 3] */
+    float *covariances;                 /* [n, 3, 3] */
+    float *harmonics;                   /* [n, 3, sh_coeffs] */
+    float *opacities;                   /* [n] */
+} ps_ply_import_desc;
+
+PS_API int ps_ply_unpack(const ps_ply_import_desc *desc, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

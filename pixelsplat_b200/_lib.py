@@ -144,6 +144,19 @@ class PlyDesc(ctypes.Structure):
                                         "center", "scale")]
 
 
+PLY_IMPORT_MAX_PROPERTIES, PLY_IMPORT_MAX_COEFFS = 512, 25
+
+
+class PlyImportDesc(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("sh_degree", "sh_coeffs", "n_props", "reserved")] + \
+        [("n_gaussians", ctypes.c_int64), ("col_xyz", ctypes.c_int32 * 3), ("col_dc", ctypes.c_int32 * 3),
+         ("col_rest", ctypes.c_int32 * 45), ("col_opacity", ctypes.c_int32), ("col_scale", ctypes.c_int32 * 3),
+         ("col_rot", ctypes.c_int32 * 4), ("reserved2", ctypes.c_int32), ("frame", ctypes.c_double * 9),
+         ("center", ctypes.c_double * 3), ("scale", ctypes.c_double),
+         ("sh_transform", ctypes.c_float * PLY_SH_TRANSFORM_FLOATS)] + \
+        [(n, ctypes.c_void_p) for n in ("records", "means", "covariances", "harmonics", "opacities")]
+
+
 class RasterCameraGrads(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in ("d_viewmatrix", "d_projmatrix", "d_campos", "d_tanfov", "workspace")] + \
         [("workspace_bytes", ctypes.c_size_t)]
@@ -167,7 +180,7 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_lpips_forward", "ps_lpips_backward", "ps_vit_attention_forward",
            "ps_vit_attention_backward_workspace_bytes", "ps_vit_attention_backward", "ps_image_resample",
            "ps_eval_images_workspace_bytes", "ps_eval_images", "ps_clip_adam_segment_chunks",
-           "ps_clip_adam_workspace_bytes", "ps_clip_adam_step", "ps_ply_pack", "ps_view_overlap")
+           "ps_clip_adam_workspace_bytes", "ps_clip_adam_step", "ps_ply_pack", "ps_ply_unpack", "ps_view_overlap")
 
 
 class NativeLibraryMissing(ImportError):
@@ -280,6 +293,8 @@ def _load() -> ctypes.CDLL:
     lib.ps_clip_adam_step.restype = ctypes.c_int
     lib.ps_ply_pack.argtypes = [P(PlyDesc), ctypes.c_void_p, ctypes.c_void_p]
     lib.ps_ply_pack.restype = ctypes.c_int
+    lib.ps_ply_unpack.argtypes = [P(PlyImportDesc), ctypes.c_void_p]
+    lib.ps_ply_unpack.restype = ctypes.c_int
     for f in ("ps_raster_sizes_query", "ps_raster_layout_query", "ps_raster_forward", "ps_raster_backward"):
         getattr(lib, f).restype = ctypes.c_int
     return lib

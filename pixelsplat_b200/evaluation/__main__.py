@@ -20,6 +20,19 @@ is the reference's compute_metrics script: it scores saved frame directories of 
 encodes the test scenes as the test step does and writes each scene's Gaussians to <output>/<scene>.ply: by default
 in the viewer format (pixelsplat_b200.ply_export.export_gaussians_ply), or as the reference's export_ply writes them.
 
+With --write-frame, each viewer-format file gets <output>/<scene>.frame.json: the export frame (centre, scale and
+rotation) that maps it back into the scene's world.
+
+    python -m pixelsplat_b200.evaluation render-ply --ply outputs/ply/re10k --dataset-root datasets/re10k \
+        --index assets/evaluation_index_re10k.json --output outputs/ply_render/re10k
+    python -m pixelsplat_b200.evaluation render-ply --ply outputs/ply/re10k/SCENE.ply --spin 120 \
+        --output outputs/spin.mp4 [--radius 2 --elevation 20 --resolution 256 256]
+
+renders 3D Gaussian splatting PLY files (pixelsplat_b200.ply_import).  Scene mode renders each index scene's target
+views from <ply>/<scene>.ply, put back into the scene's world by <scene>.frame.json, and writes the frames as the
+evaluator does (so compute-metrics can score them as a --method) with metrics.json.  Spin mode writes an orbit of
+one file about its +z axis as an mp4, colour beside turbo depth.
+
     python -m pixelsplat_b200.evaluation generate-index --dataset-root datasets/re10k \
         --output outputs/evaluation_index_re10k [--video]
 
@@ -163,7 +176,13 @@ def parse_export_ply(argv: list[str]) -> argparse.Namespace:
     p.add_argument("--format", choices=("viewer", "reference"), default="viewer",
                    help="viewer: what the rasterizer renders, with SH up to degree 3 (default); reference: the "
                         "reference's export_ply (DC only, camera-frame rotations, raw opacity)")
-    return p.parse_args(argv)
+    p.add_argument("--write-frame", action="store_true",
+                   help="also write <output>/<scene>.frame.json: the export frame's centre, scale and rotation, which "
+                        "render-ply needs to put the file back into the scene's world (viewer format only)")
+    args = p.parse_args(argv)
+    if args.write_frame and args.format != "viewer":
+        p.error("--write-frame needs --format viewer")
+    return args
 
 
 def export_ply(argv: list[str]) -> list[Path]:
@@ -172,7 +191,7 @@ def export_ply(argv: list[str]) -> list[Path]:
     ones the test step renders (the encoder samples depths from torch's generator)."""
     args = parse_export_ply(argv)
     from ..data import device_shim
-    from ..ply_export import export_gaussians_ply, export_ply as export_reference
+    from ..ply_export import export_frame, export_gaussians_ply, export_ply as export_reference, write_frame_json
     from .presets import IMAGE_SHAPE, SEED, build_model
     device = torch.device("cuda", torch.cuda.current_device())
     cfg, loader = _loader(args, args.preset)
@@ -198,6 +217,8 @@ def export_ply(argv: list[str]) -> list[Path]:
             extrinsics = batch["context"]["extrinsics"][0, 0]
             if args.format == "viewer":
                 export_gaussians_ply(gaussians, extrinsics, path)
+                if args.write_frame:
+                    write_frame_json(export_frame(gaussians.means[0], extrinsics), path.with_suffix(".frame.json"))
             else:
                 export_reference(extrinsics, gaussians.means[0], dump["scales"][0], dump["rotations"][0],
                                  gaussians.harmonics[0], gaussians.opacities[0], path)
@@ -270,6 +291,88 @@ def render_videos(argv: list[str]) -> list[Path]:
     return written
 
 
+def parse_render_ply(argv: list[str]) -> argparse.Namespace:
+    p = argparse.ArgumentParser(prog="python -m pixelsplat_b200.evaluation render-ply",
+                                description="Render 3D Gaussian splatting PLY files: the test scenes' target views "
+                                            "from exported files, or a spin around one file.")
+    p.add_argument("--ply", type=Path, required=True,
+                   help="directory of <scene>.ply and <scene>.frame.json (scene mode), or one .ply file (--spin)")
+    p.add_argument("--output", type=Path, required=True,
+                   help="directory of <scene>/color/<index>.png and metrics.json, or the .mp4 file (--spin)")
+    p.add_argument("--dataset-root", type=Path, default=None, help="dataset root holding test/index.json")
+    p.add_argument("--index", type=Path, default=None, help="evaluation index (scene -> context / target)")
+    p.add_argument("--num-workers", type=int, default=4, help="DataLoader workers (the reference's test loader: 4)")
+    p.add_argument("--lpips-vgg", type=Path, default=None, help="torchvision's vgg16-397923af.pth")
+    p.add_argument("--lpips-lin", type=Path, default=None, help="the lpips package's weights/v0.1/vgg.pth")
+    p.add_argument("--spin", type=int, default=None, metavar="FRAMES",
+                   help="render an orbit of FRAMES frames around the file's origin as an mp4 instead")
+    p.add_argument("--radius", type=float, default=2.0, help="orbit radius, in the file's units (default: 2)")
+    p.add_argument("--elevation", type=float, default=20.0, help="orbit elevation in degrees (default: 20)")
+    p.add_argument("--resolution", type=int, nargs=2, default=[256, 256], metavar=("H", "W"),
+                   help="spin frame size (default: 256 256)")
+    args = p.parse_args(argv)
+    if args.spin is None:
+        if args.dataset_root is None or args.index is None:
+            p.error("scene mode needs --dataset-root and --index (or --spin FRAMES for an orbit)")
+    elif args.spin < 1 or args.radius <= 0 or min(args.resolution) < 1:
+        p.error("--spin, --radius and --resolution must be positive")
+    return args
+
+
+def render_ply(argv: list[str]) -> dict:
+    """Scene mode: every index scene's target views rendered from <ply>/<scene>.ply, imported into the scene's world
+    through <scene>.frame.json, as the test step renders (chunks of CHUNK views, the 8-bit frame pass); frames in
+    the evaluator's layout and the evaluator's metrics.json.  Spin mode: one file's orbit as an mp4."""
+    args = parse_render_ply(argv)
+    from types import SimpleNamespace
+    from ..ply_import import load_gaussians_ply
+    from ..decoder import DecoderSplattingCUDA, DecoderSplattingCUDACfg
+    device = torch.device("cuda", torch.cuda.current_device())
+    if args.spin is not None:
+        from ..video import render_spin, write_mp4
+        decoder = DecoderSplattingCUDA(DecoderSplattingCUDACfg("splatting_cuda"),
+                                       SimpleNamespace(background_color=[0.0, 0.0, 0.0])).to(device)
+        frames = render_spin(decoder, load_gaussians_ply(args.ply, device), args.spin, args.radius,
+                             args.elevation, tuple(args.resolution))
+        path = write_mp4(frames.numpy(), args.output)
+        print(f"Wrote {len(frames)} frames to {path}.")
+        return {"frames": len(frames)}
+
+    from ..data import device_shim
+    from .evaluator import METRICS, mean_over_scenes
+    from .image_io import save_frame
+    from .metrics import CHUNK, frame_metrics_chunked
+    from .presets import IMAGE_SHAPE
+    cfg, loader = _loader(args)
+    decoder = DecoderSplattingCUDA(DecoderSplattingCUDACfg("splatting_cuda"), cfg).to(device)
+    lpips = _lpips(args, device)
+    scenes = {}
+    with torch.no_grad():
+        for batch in loader:
+            (scene,) = batch["scene"]
+            frame = args.ply / f"{scene}.frame.json"
+            if not frame.exists():
+                raise SystemExit(f"evaluation render-ply: {frame} is missing; export the scenes with "
+                                 "`export-ply --write-frame` to render them in their world")
+            gaussians = load_gaussians_ply(args.ply / f"{scene}.ply", device, frame=frame)
+            tgt = device_shim(batch, IMAGE_SHAPE, device)["target"]
+            v, (h, w) = tgt["image"].shape[1], tgt["image"].shape[-2:]
+            color = torch.cat([decoder.forward(gaussians, tgt["extrinsics"][:1, i:i + CHUNK],
+                                               tgt["intrinsics"][:1, i:i + CHUNK], tgt["near"][:1, i:i + CHUNK],
+                                               tgt["far"][:1, i:i + CHUNK], (h, w)).color
+                               for i in range(0, v, CHUNK)], dim=1)
+            per_view = frame_metrics_chunked(tgt["image"][0], color[0], lpips, return_frames=True)
+            frames = per_view.pop("frames").cpu().numpy()
+            for index, f in zip(tgt["index"][0].tolist(), frames):
+                save_frame(f, args.output / scene / "color" / f"{index:0>6}.png")
+            scenes[scene] = {k: float(per_view[k].mean()) for k in METRICS}
+    out = {"mean": mean_over_scenes(scenes.values()), "scenes": scenes}
+    print(f"{len(scenes)} scenes: " + ", ".join(f"{k} {v:.4f}" for k, v in out["mean"].items()))
+    args.output.mkdir(parents=True, exist_ok=True)
+    (args.output / "metrics.json").write_text(json.dumps(out))
+    return out
+
+
 def parse_generate_index(argv: list[str]) -> argparse.Namespace:
     from .index_generator import EvaluationIndexGeneratorCfg
     d = EvaluationIndexGeneratorCfg()
@@ -322,6 +425,8 @@ def main(argv: list[str] | None = None) -> None:
         export_ply(argv[1:])
     elif argv and argv[0] == "render-video":
         render_videos(argv[1:])
+    elif argv and argv[0] == "render-ply":
+        render_ply(argv[1:])
     else:
         evaluate(argv)
 

@@ -17,7 +17,9 @@ written in one call from a pinned host buffer.
 from __future__ import annotations
 
 import ctypes
+import json
 import math
+from dataclasses import dataclass
 from pathlib import Path
 from typing import Union
 
@@ -80,6 +82,35 @@ def normalisation(means: Tensor) -> tuple[Tensor, Tensor]:
     center = means.median(dim=0).values
     scale = (means - center).abs().quantile(0.95, dim=0).max().reshape(1)
     return center.contiguous(), scale
+
+
+@dataclass(frozen=True)
+class ExportFrame:
+    """The map from the world to a viewer-format file: x = M (p - c) / s.  `center` c (float32 [3]) and `scale` s
+    (float32 [1], a zero 0.95 quantile replaced by 1) stay on the means' device; `rotation` M is float64 [3, 3] on
+    the host."""
+    center: Tensor
+    scale: Tensor
+    rotation: Tensor
+
+    def to_json(self) -> dict:
+        """c, s and M as JSON numbers: the float32 values of c and s are exact in a double, so a reader gets the bits
+        the kernel used."""
+        return {"center": [float(v) for v in self.center.cpu()], "scale": float(self.scale.cpu()[0]),
+                "rotation": [[float(v) for v in row] for row in self.rotation]}
+
+
+def export_frame(means: Tensor, extrinsics: Tensor) -> ExportFrame:
+    """The frame `export_gaussians_ply` writes one scene's Gaussians in: the median of `means` [n, 3], s and
+    M = viewer_frame(extrinsics)."""
+    center, scale = normalisation(means)
+    return ExportFrame(center, torch.where(scale > 0, scale, torch.ones_like(scale)), viewer_frame(extrinsics))
+
+
+def write_frame_json(frame: ExportFrame, path: Union[Path, str]) -> None:
+    path = Path(path)
+    path.parent.mkdir(exist_ok=True, parents=True)
+    path.write_text(json.dumps(frame.to_json(), indent=1) + "\n")
 
 
 def _check(fn: str, name: str, t, shape: tuple, device=None) -> Tensor:
@@ -162,13 +193,12 @@ def pack_viewer(gaussians, extrinsics: Tensor, sh_degree: int = MAX_SH_DEGREE) -
     harmonics, have = _check_harmonics(fn, fields["harmonics"], n, dev)
     t = dict(means=means, covariances=_check(fn, "gaussians.covariances", fields["covariances"], (n, 3, 3), dev),
              harmonics=harmonics, opacities=_check(fn, "gaussians.opacities", fields["opacities"], (n,), dev))
-    center, scale = normalisation(means)
-    t["center"], t["scale"] = center, torch.where(scale > 0, scale, torch.ones_like(scale))
+    frame = export_frame(means, extrinsics)
+    t["center"], t["scale"] = frame.center, frame.scale
     degree = min(sh_degree, MAX_SH_DEGREE, have)
-    frame = viewer_frame(extrinsics)
-    transform = sh_transform(frame, degree, get_sh_basis())
+    transform = sh_transform(frame.rotation, degree, get_sh_basis())
     desc = _lib.PlyDesc(mode=_lib.PS_PLY_VIEWER, sh_degree=degree, sh_coeffs=harmonics.shape[-1])
-    desc.frame[:] = [float(v) for v in frame.reshape(-1)]
+    desc.frame[:] = [float(v) for v in frame.rotation.reshape(-1)]
     for l in range(degree + 1):
         block = transform[l * l:(l + 1) ** 2, l * l:(l + 1) ** 2].reshape(-1)
         desc.sh_transform[_BLOCK_OFFSETS[l]:_BLOCK_OFFSETS[l] + block.numel()] = [float(v) for v in block]

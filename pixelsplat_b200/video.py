@@ -168,6 +168,52 @@ def generate_wobble(extrinsics: Tensor, radius: Tensor, t: Tensor) -> Tensor:
     return extrinsics[..., None, :, :] @ generate_wobble_transformation(radius, t)
 
 
+# ---- spin: src/visualization/camera_trajectory/spin.py --------------------------------------------------------------
+
+def generate_spin(num_frames: int, device, elevation: float, radius: float) -> Tensor:
+    """The reference's generate_spin: float32 camera-to-world [num_frames, 4, 4] orbiting the origin about +y at
+    `radius`, raised by `elevation` degrees, each camera looking at the origin with its up vector (-Y) along +y at
+    zero elevation."""
+    tf_translation = torch.eye(4, dtype=torch.float32, device=device)
+    tf_translation[:2] *= -1
+    tf_translation[2, 3] = -radius
+    phi = 2 * np.pi * (np.arange(num_frames) / num_frames)
+    rotation_vectors = np.stack([np.zeros_like(phi), phi, np.zeros_like(phi)], axis=-1)
+    azimuth = torch.tensor(Rotation.from_rotvec(rotation_vectors).as_matrix(), dtype=torch.float32, device=device)
+    tf_azimuth = torch.eye(4, dtype=torch.float32, device=device).repeat(num_frames, 1, 1)
+    tf_azimuth[:, :3, :3] = azimuth
+    tilt = Rotation.from_rotvec(np.array([np.deg2rad(elevation), 0, 0], dtype=np.float32))
+    tf_elevation = torch.eye(4, dtype=torch.float32, device=device)
+    tf_elevation[:3, :3] = torch.tensor(tilt.as_matrix())
+    return tf_azimuth @ tf_elevation @ tf_translation
+
+
+# +y -> +z, +z -> -y: the reference's spin turned to orbit the up axis of the PLY export frame (+z)
+_Y_UP_TO_Z_UP = ((1.0, 0.0, 0.0, 0.0), (0.0, 0.0, -1.0, 0.0), (0.0, 1.0, 0.0, 0.0), (0.0, 0.0, 0.0, 1.0))
+
+
+def spin_trajectory(num_frames: int, radius: float, elevation: float) -> tuple[Tensor, Tensor, Tensor, Tensor]:
+    """Cameras orbiting the origin of a PLY export frame about its +z up axis: float32 extrinsics [T, 4, 4],
+    the intrinsics the reference's test_splatter script renders its spin with (fx = fy = 0.5, centred) [T, 3, 3],
+    near = radius / 100 and far = 2 radius [T], on the host."""
+    extrinsics = torch.tensor(_Y_UP_TO_Z_UP, dtype=torch.float32) @ generate_spin(num_frames, "cpu", elevation, radius)
+    k = torch.tensor([[0.5, 0.0, 0.5], [0.0, 0.5, 0.5], [0.0, 0.0, 1.0]], dtype=torch.float32)
+    near = torch.full((num_frames,), radius / 100, dtype=torch.float32)
+    far = torch.full((num_frames,), 2 * radius, dtype=torch.float32)
+    return extrinsics, k.expand(num_frames, 3, 3).contiguous(), near, far
+
+
+@torch.no_grad()
+def render_spin(decoder, gaussians, num_frames: int, radius: float, elevation: float, shape: tuple[int, int],
+                log: Optional[Callable[[str], None]] = print) -> Tensor:
+    """The spin of one scene's `gaussians` (batch 1, on the device): uint8 [T, h, 2 w, 3] on the host, colour on
+    the left and turbo depth on the right."""
+    device = gaussians.means.device
+    extrinsics, intrinsics, near, far = (t.to(device)[None] for t in spin_trajectory(num_frames, radius, elevation))
+    color, depth = _render_panels(decoder, gaussians, extrinsics, intrinsics, near, far, shape, log)
+    return torch.cat([color, depth], dim=-1).permute(0, 2, 3, 1).cpu()
+
+
 # ---- the three videos: ModelWrapper.render_video_* -----------------------------------------------------------------
 
 @dataclass(frozen=True)
