@@ -814,6 +814,50 @@ typedef struct {
 
 PS_API int ps_ply_unpack(const ps_ply_import_desc *desc, void *stream);
 
+/* ---- PLY refinement: one Adam step on a scene's vertex records (csrc/ply_import.cu) ---------------------------------
+ * One launch per optimisation step over the n = unpack.n_gaussians records [n, n_props] that unpack.records points
+ * at, given the gradients of a loss with respect to ps_ply_unpack's outputs for those records (d_means [n, 3],
+ * d_covariances [n, 3, 3], d_harmonics [n, 3, sh_coeffs], d_opacities [n]).  Per Gaussian, in float64:
+ *   backward   d_p = s M d_mean;  d_l_k = 2 var_k b_k^T dSigma b_k with var_k = s^2 exp(2 l_k) and b = R(q^)^T M (both
+ *              halves of an off-diagonal pair count: the unpack writes each twice);  d_q^ = dR/dq^ . (M db^T) with
+ *              db_k = 2 var_k (dSigma + dSigma^T)/2 b_k, then d_q = (d_q^ - q^ (q^ . d_q^)) / |q|, and 0 for a zero
+ *              quaternion (the unpack's identity rotation does not depend on q);  d_o = d_opacity sigmoid(o)
+ *              (1 - sigmoid(o));  f_dc / f_rest: T_l^T d_h per channel and degree l <= sh_degree (coefficients of
+ *              d_harmonics above the file's degree are not read).  Rounded once to float32: g.
+ *   Adam       torch.optim.Adam's float32 update (no weight decay, no amsgrad) of every column the unpack reads,
+ *              with lr[column]: m += (1 - beta1) (g - m), v = beta2 v + (1 - beta2) g^2, p -= lr / (1 - beta1^t)
+ *              * m / (sqrt(v) / sqrt(1 - beta2^t) + eps), t = step; the two corrections are formed on the host in
+ *              float64 and rounded to float32, as torch rounds its scalars.  Columns the unpack does not read
+ *              (normals, other pipelines' fields) have a gradient of exactly 0 and are not updated: the record and
+ *              both moments keep their bits.
+ *   unpack     the updated record through ps_ply_unpack's own per-record code into unpack.means, .covariances,
+ *              .harmonics, .opacities: bit-identical to ps_ply_unpack of records_out.
+ * records_out [n, n_props] receives the updated records and may be unpack.records itself (in place); exp_avg and
+ * exp_avg_sq [n, n_props] are updated in place; d_records [n, n_props], when not NULL, receives g (0 in the columns
+ * the unpack does not read).  Every output entry is written once, nothing past n is touched, there are no atomics
+ * (a Gaussian's outputs have one writer: equal inputs give equal bits) and no host synchronisation.  Staging and
+ * stores are ps_ply_unpack's.  Rejects what ps_ply_unpack rejects, n_props above PS_PLY_REFINE_MAX_PROPERTIES, a
+ * NULL or misaligned records_out, exp_avg, exp_avg_sq or gradient, a misaligned d_records, step < 1, a learning rate
+ * of a read column that is negative or not finite, and betas outside [0, 1) or eps < 0 with PS_ERR_INVALID_ARGUMENT
+ * before anything is enqueued. */
+#define PS_PLY_REFINE_MAX_PROPERTIES 256
+
+typedef struct {
+    ps_ply_import_desc unpack;          /* columns, frame, SH blocks, the records read and the Gaussians written */
+    int64_t step;                       /* t >= 1: the number of this step (bias corrections) */
+    double beta1, beta2, eps;
+    double lr[PS_PLY_REFINE_MAX_PROPERTIES];   /* per column; only the columns the unpack reads are used */
+    float *records_out;                 /* [n, n_props], may equal unpack.records */
+    float *exp_avg, *exp_avg_sq;        /* [n, n_props], in place */
+    const float *d_means;               /* [n, 3] */
+    const float *d_covariances;         /* [n, 3, 3] */
+    const float *d_harmonics;           /* [n, 3, sh_coeffs] */
+    const float *d_opacities;           /* [n] */
+    float *d_records;                   /* [n, n_props] or NULL */
+} ps_ply_refine_desc;
+
+PS_API int ps_ply_refine_step(const ps_ply_refine_desc *desc, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

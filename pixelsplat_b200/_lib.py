@@ -157,6 +157,17 @@ class PlyImportDesc(ctypes.Structure):
         [(n, ctypes.c_void_p) for n in ("records", "means", "covariances", "harmonics", "opacities")]
 
 
+PLY_REFINE_MAX_PROPERTIES = 256
+
+
+class PlyRefineDesc(ctypes.Structure):
+    _fields_ = [("unpack", PlyImportDesc), ("step", ctypes.c_int64)] + \
+        [(n, ctypes.c_double) for n in ("beta1", "beta2", "eps")] + \
+        [("lr", ctypes.c_double * PLY_REFINE_MAX_PROPERTIES)] + \
+        [(n, ctypes.c_void_p) for n in ("records_out", "exp_avg", "exp_avg_sq", "d_means", "d_covariances",
+                                        "d_harmonics", "d_opacities", "d_records")]
+
+
 class RasterCameraGrads(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in ("d_viewmatrix", "d_projmatrix", "d_campos", "d_tanfov", "workspace")] + \
         [("workspace_bytes", ctypes.c_size_t)]
@@ -180,7 +191,8 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_lpips_forward", "ps_lpips_backward", "ps_vit_attention_forward",
            "ps_vit_attention_backward_workspace_bytes", "ps_vit_attention_backward", "ps_image_resample",
            "ps_eval_images_workspace_bytes", "ps_eval_images", "ps_clip_adam_segment_chunks",
-           "ps_clip_adam_workspace_bytes", "ps_clip_adam_step", "ps_ply_pack", "ps_ply_unpack", "ps_view_overlap")
+           "ps_clip_adam_workspace_bytes", "ps_clip_adam_step", "ps_ply_pack", "ps_ply_unpack", "ps_view_overlap",
+           "ps_ply_refine_step")
 
 
 class NativeLibraryMissing(ImportError):
@@ -295,6 +307,8 @@ def _load() -> ctypes.CDLL:
     lib.ps_ply_pack.restype = ctypes.c_int
     lib.ps_ply_unpack.argtypes = [P(PlyImportDesc), ctypes.c_void_p]
     lib.ps_ply_unpack.restype = ctypes.c_int
+    lib.ps_ply_refine_step.argtypes = [P(PlyRefineDesc), ctypes.c_void_p]
+    lib.ps_ply_refine_step.restype = ctypes.c_int
     for f in ("ps_raster_sizes_query", "ps_raster_layout_query", "ps_raster_forward", "ps_raster_backward"):
         getattr(lib, f).restype = ctypes.c_int
     return lib

@@ -17,6 +17,7 @@
 //
 // Only the question "which CTA is last" goes through an atomic; every sum has a fixed order, so a step gives the same
 // bits on every run.  Nothing is read back by the host: the call can be captured in a CUDA graph.
+#include "adam.cuh"
 #include "ps_common.cuh"
 
 namespace ps {
@@ -152,17 +153,9 @@ k_clip_adam_norm(ps_clip_adam_desc d, const ps_clip_adam_segment *__restrict__ s
     }
 }
 
-struct AdamConsts {
-    float w1, b2, w2, eps;   // 1 - beta1, beta2, 1 - beta2, eps
-};
-
-// torch.optim.Adam's float32 update of one element: exp_avg.lerp_(g, 1 - beta1); exp_avg_sq.mul_(beta2).addcmul_(g,
-// g, 1 - beta2); p.addcdiv_(exp_avg, exp_avg_sq.sqrt() / sqrt(bc2) + eps, -step_size).
+// Adam (adam.cuh) on the clipped gradient coef * g, with the step's scalars.
 __device__ __forceinline__ void adam(float &p, float g, float &m, float &v, const AdamConsts &k, const OptHeader &h) {
-    g *= h.coef;
-    m = fmaf(k.w1, g - m, m);
-    v = fmaf(k.w2 * g, g, v * k.b2);
-    p -= h.step_size * (m / (sqrtf(v) / h.bc2_sqrt + k.eps));
+    adam(p, g * h.coef, m, v, k, h.step_size, h.bc2_sqrt);
 }
 
 __global__ void __launch_bounds__(kOptThreads)

@@ -33,6 +33,13 @@ views from <ply>/<scene>.ply, put back into the scene's world by <scene>.frame.j
 evaluator does (so compute-metrics can score them as a --method) with metrics.json.  Spin mode writes an orbit of
 one file about its +z axis as an mp4, colour beside turbo depth.
 
+    python -m pixelsplat_b200.evaluation refine-ply --ply outputs/ply/re10k --dataset-root datasets/re10k \
+        --index assets/evaluation_index_re10k.json --output outputs/ply_refined/re10k [--steps 100]
+
+refines each index scene's <ply>/<scene>.ply (pixelsplat_b200.ply_refine) in its world against the scene's context
+views only, and writes <output>/<scene>.ply, a copy of <scene>.frame.json and refine.json (each scene's context-view
+MSE before and after).  render-ply --ply <output> then scores the refined scenes on the held-out targets.
+
     python -m pixelsplat_b200.evaluation generate-index --dataset-root datasets/re10k \
         --output outputs/evaluation_index_re10k [--video]
 
@@ -373,6 +380,83 @@ def render_ply(argv: list[str]) -> dict:
     return out
 
 
+def _non_negative(kind):
+    def parse(text: str):
+        value = kind(text)
+        if not value >= 0:
+            raise argparse.ArgumentTypeError(f"{text} is negative")
+        return value
+    return parse
+
+
+def parse_refine_ply(argv: list[str]) -> argparse.Namespace:
+    from ..ply_refine import DEFAULT_LR, GROUPS
+    p = argparse.ArgumentParser(prog="python -m pixelsplat_b200.evaluation refine-ply",
+                                description="Refine exported 3D Gaussian splatting PLY files on each test scene's "
+                                            "context views.")
+    p.add_argument("--ply", type=Path, required=True, help="directory of <scene>.ply and <scene>.frame.json")
+    p.add_argument("--dataset-root", type=Path, required=True, help="dataset root holding test/index.json")
+    p.add_argument("--index", type=Path, required=True, help="evaluation index (scene -> context / target)")
+    p.add_argument("--output", type=Path, required=True,
+                   help="directory of the refined <scene>.ply, <scene>.frame.json and refine.json")
+    p.add_argument("--scene", action="append", default=None, metavar="NAME",
+                   help="refine only this scene (repeatable; default: every index scene)")
+    p.add_argument("--steps", type=_non_negative(int), default=100, help="Adam steps per scene (default: 100)")
+    p.add_argument("--num-workers", type=int, default=4, help="DataLoader workers (the reference's test loader: 4)")
+    for g in GROUPS:
+        p.add_argument(f"--lr-{g.replace('_', '-')}", dest=f"lr_{g}", type=_non_negative(float), default=DEFAULT_LR[g],
+                       help=f"learning rate of the {g} properties (default: 3DGS's {DEFAULT_LR[g]:g})")
+    args = p.parse_args(argv)
+    args.lr = {g: getattr(args, f"lr_{g}") for g in GROUPS}
+    return args
+
+
+def refine_ply(argv: list[str]) -> dict:
+    """Every index scene's <ply>/<scene>.ply refined in its world (<scene>.frame.json) on the scene's context views,
+    loaded as render-ply loads its targets; the targets stay held out."""
+    args = parse_refine_ply(argv)
+    import shutil
+    from ..data import device_shim
+    from ..ply_import import read_frame_json, read_ply_body
+    from ..ply_refine import refine_ply as refine, refine_records
+    from .presets import IMAGE_SHAPE
+    device = torch.device("cuda", torch.cuda.current_device())
+    cfg, loader = _loader(args)
+    background = torch.tensor(cfg.background_color, dtype=torch.float32, device=device)
+    wanted = None if args.scene is None else set(args.scene)
+    scenes = {}
+    for batch in loader:
+        (scene,) = batch["scene"]
+        if wanted is not None and scene not in wanted:
+            continue
+        frame = args.ply / f"{scene}.frame.json"
+        if not frame.exists():
+            raise SystemExit(f"evaluation refine-ply: {frame} is missing; export the scenes with "
+                             "`export-ply --write-frame` to refine them in their world")
+        ctx = device_shim(batch, IMAGE_SHAPE, device)["context"]
+        result = refine(args.ply / f"{scene}.ply", frame, extrinsics=ctx["extrinsics"][0],
+                        intrinsics=ctx["intrinsics"][0], near=ctx["near"][0], far=ctx["far"][0],
+                        images=ctx["image"][0], background_color=background, steps=args.steps,
+                        out_path=args.output / f"{scene}.ply", lr=args.lr, device=device)
+        shutil.copyfile(frame, args.output / f"{scene}.frame.json")
+        if result is None:   # --steps 0: the file is copied; its MSE is one render
+            layout, records = read_ply_body(args.ply / f"{scene}.ply", device)
+            result = refine_records(records, layout.properties, layout.sh_degree,
+                                    frame=read_frame_json(frame, device), extrinsics=ctx["extrinsics"][0],
+                                    intrinsics=ctx["intrinsics"][0], near=ctx["near"][0], far=ctx["far"][0],
+                                    images=ctx["image"][0], background_color=background, steps=0)
+        loss = result.loss.tolist()
+        scenes[scene] = {"mse_before": loss[0], "mse_after": loss[-1], "steps": args.steps}
+        print(f"{scene}: context MSE {loss[0]:.6f} -> {loss[-1]:.6f} in {args.steps} steps")
+    missing = sorted(wanted - set(scenes)) if wanted is not None else []
+    if missing:
+        raise SystemExit(f"evaluation refine-ply: no index scene named {', '.join(missing)}")
+    out = {"steps": args.steps, "lr": args.lr, "scenes": scenes}
+    args.output.mkdir(parents=True, exist_ok=True)
+    (args.output / "refine.json").write_text(json.dumps(out, indent=1) + "\n")
+    return out
+
+
 def parse_generate_index(argv: list[str]) -> argparse.Namespace:
     from .index_generator import EvaluationIndexGeneratorCfg
     d = EvaluationIndexGeneratorCfg()
@@ -427,6 +511,8 @@ def main(argv: list[str] | None = None) -> None:
         render_videos(argv[1:])
     elif argv and argv[0] == "render-ply":
         render_ply(argv[1:])
+    elif argv and argv[0] == "refine-ply":
+        refine_ply(argv[1:])
     else:
         evaluate(argv)
 

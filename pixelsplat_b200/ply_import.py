@@ -141,7 +141,6 @@ def unpack_records(records: Tensor, properties, sh_degree: int, *, frame: Option
     `Gaussians` of dense float32 tensors ([n, 3], [n, 3, 3], [n, 3, sh_coeffs], [n]), receives the result instead
     of new tensors."""
     from .decoder import Gaussians
-    from .rasterizer import get_sh_basis
     fn = "unpack_records"
     properties = list(properties)
     if not isinstance(records, Tensor) or not records.is_cuda or records.dtype != torch.float32 or \
@@ -162,8 +161,22 @@ def unpack_records(records: Tensor, properties, sh_degree: int, *, frame: Option
         if t.shape != shape or t.dtype != torch.float32 or t.device != dev or not t.is_contiguous():
             raise ValueError(f"{fn}: `out.{name}` must be a dense float32 {list(shape)} tensor on {dev}")
     records = records.contiguous()
+    desc = import_desc(properties, sh_degree, coeffs, n, frame)
+    desc.records = records.data_ptr()
+    for name in shapes:
+        setattr(desc, name, getattr(out, name).data_ptr())
+    _launch(desc, dev)
+    return out
+
+
+def import_desc(properties, sh_degree: int, sh_coeffs: int, n: int,
+                frame: Optional[ExportFrame] = None) -> _lib.PlyImportDesc:
+    """The descriptor of `ps_ply_unpack` for records with `properties`, without its pointers: columns, frame and
+    the import SH blocks of the rasterizer's basis."""
+    from .rasterizer import get_sh_basis
+    nc = (sh_degree + 1) ** 2
     col = {p: i for i, p in enumerate(properties)}
-    desc = _lib.PlyImportDesc(sh_degree=sh_degree, sh_coeffs=coeffs, n_props=len(properties), n_gaussians=n)
+    desc = _lib.PlyImportDesc(sh_degree=sh_degree, sh_coeffs=sh_coeffs, n_props=len(properties), n_gaussians=n)
     desc.col_xyz[:] = [col[k] for k in ("x", "y", "z")]
     desc.col_dc[:] = [col[f"f_dc_{c}"] for c in range(3)]
     for i in range(3 * (nc - 1)):
@@ -181,11 +194,7 @@ def unpack_records(records: Tensor, properties, sh_degree: int, *, frame: Option
     blocks = import_sh_blocks(None if frame is None else frame.rotation, sh_degree, get_sh_basis())
     for l, block in enumerate(blocks):
         desc.sh_transform[_BLOCK_OFFSETS[l]:_BLOCK_OFFSETS[l] + block.numel()] = [float(v) for v in block.reshape(-1)]
-    desc.records = records.data_ptr()
-    for name in shapes:
-        setattr(desc, name, getattr(out, name).data_ptr())
-    _launch(desc, dev)
-    return out
+    return desc
 
 
 def _launch(desc: _lib.PlyImportDesc, device) -> None:
