@@ -858,6 +858,54 @@ typedef struct {
 
 PS_API int ps_ply_refine_step(const ps_ply_refine_desc *desc, void *stream);
 
+/* ---- PLY densification: 3DGS's adaptive density control on a scene's vertex records (csrc/ply_densify.cu) --------
+ * Three entry points over the n = n_gaussians records [n, n_props] of a refinement (ps_ply_refine_step's layout):
+ *   ps_ply_densify_stats   per Gaussian i, in view order v = 0..n_views-1 where radii[v, i] > 0:
+ *                          accum[i] += |d_means2d[v, i, 0:2]| (the norm in float64, rounded once; the sum in float32)
+ *                          and count[i] += 1.  d_means2d [n_views, n, 3], radii [n_views, n] int32: the rasterizer's
+ *                          screen-space gradient and radii of one call over the views.  One writer per entry.
+ *   ps_ply_densify_count   per Gaussian: g = count > 0 ? accum / count : 0 (float32); big = max_k exp(l_k) >
+ *                          percent_dense extent (float64); clone = g >= grad_threshold && !big, split = g >=
+ *                          grad_threshold && big; prune(o, l) = sigmoid(o) < min_opacity || (prune_world && max_k
+ *                          exp(l_k) > 0.1 extent), both in float64.  keep = !split && !prune(o, l); a clone is kept
+ *                          when !prune(o, l); both copies of a split are kept when !prune(o, l') with l' the copies'
+ *                          float32 log-scales.  Writes the flags and per-CTA segment offsets to the workspace, and
+ *                          counts[0..3] = kept originals, kept clones, kept splits (each split gives two rows), n_new.
+ *   ps_ply_densify_apply   records_out, exp_avg_out, exp_avg_sq_out [n_new, n_props] from the flags and offsets in
+ *                          3DGS's order: kept originals (record and moments copied), clones (record copied, moments
+ *                          0), first copies of the splits, second copies (moments 0).  Every segment keeps input order.
+ *                          A split's copy k (0, 1) is the record with p' = p + R(q^) (exp(l) * eps[k, i, :]) and
+ *                          l' = l - log(1.6), in float64 rounded once (a zero quaternion is the identity); every other
+ *                          column is copied bit for bit.  eps [2, n, 3] float32: N(0, 1) draws.
+ * count and apply read the same workspace (ps_ply_densify_workspace_bytes(n)); count's counts must be in place when
+ * apply runs (stream order).  Nothing past n_new is written, there are no atomics (equal inputs give equal bits) and
+ * no host synchronisation.  Rejects a NULL or misaligned pointer (16 bytes for the record arrays, 8 for counts, 4 for
+ * the others), n < 1, n_views < 1, n_props outside [1, PS_PLY_REFINE_MAX_PROPERTIES], a column outside [0, n_props),
+ * a threshold that is negative or not finite, extent <= 0 and a workspace smaller than the query with
+ * PS_ERR_INVALID_ARGUMENT before anything is enqueued. */
+typedef struct {
+    int64_t n_gaussians;
+    int32_t n_props;                    /* floats per record */
+    int32_t prune_world;                /* 1: also prune max_k exp(l_k) > 0.1 extent */
+    int32_t col_xyz[3];                 /* column of each field in the record */
+    int32_t col_opacity;
+    int32_t col_scale[3];
+    int32_t col_rot[4];                 /* wxyz */
+    int32_t reserved;
+    double grad_threshold, percent_dense, min_opacity, extent;
+} ps_ply_densify_desc;
+
+PS_API int ps_ply_densify_workspace_bytes(int64_t n_gaussians, size_t *bytes);
+PS_API int ps_ply_densify_stats(int64_t n_gaussians, int32_t n_views, const float *d_means2d, const int32_t *radii,
+                                float *accum, int32_t *count, void *stream);
+PS_API int ps_ply_densify_count(const ps_ply_densify_desc *desc, const float *records, const float *accum,
+                                const int32_t *count, void *workspace, size_t workspace_bytes, int64_t *counts,
+                                void *stream);
+PS_API int ps_ply_densify_apply(const ps_ply_densify_desc *desc, const float *records, const float *exp_avg,
+                                const float *exp_avg_sq, const float *eps, const void *workspace,
+                                size_t workspace_bytes, const int64_t *counts, float *records_out,
+                                float *exp_avg_out, float *exp_avg_sq_out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -168,6 +168,13 @@ class PlyRefineDesc(ctypes.Structure):
                                         "d_harmonics", "d_opacities", "d_records")]
 
 
+class PlyDensifyDesc(ctypes.Structure):
+    _fields_ = [("n_gaussians", ctypes.c_int64), ("n_props", ctypes.c_int32), ("prune_world", ctypes.c_int32),
+                ("col_xyz", ctypes.c_int32 * 3), ("col_opacity", ctypes.c_int32), ("col_scale", ctypes.c_int32 * 3),
+                ("col_rot", ctypes.c_int32 * 4), ("reserved", ctypes.c_int32)] + \
+        [(n, ctypes.c_double) for n in ("grad_threshold", "percent_dense", "min_opacity", "extent")]
+
+
 class RasterCameraGrads(ctypes.Structure):
     _fields_ = [(n, ctypes.c_void_p) for n in ("d_viewmatrix", "d_projmatrix", "d_campos", "d_tanfov", "workspace")] + \
         [("workspace_bytes", ctypes.c_size_t)]
@@ -192,7 +199,8 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_vit_attention_backward_workspace_bytes", "ps_vit_attention_backward", "ps_image_resample",
            "ps_eval_images_workspace_bytes", "ps_eval_images", "ps_clip_adam_segment_chunks",
            "ps_clip_adam_workspace_bytes", "ps_clip_adam_step", "ps_ply_pack", "ps_ply_unpack", "ps_view_overlap",
-           "ps_ply_refine_step")
+           "ps_ply_refine_step", "ps_ply_densify_workspace_bytes", "ps_ply_densify_stats", "ps_ply_densify_count",
+           "ps_ply_densify_apply")
 
 
 class NativeLibraryMissing(ImportError):
@@ -309,6 +317,16 @@ def _load() -> ctypes.CDLL:
     lib.ps_ply_unpack.restype = ctypes.c_int
     lib.ps_ply_refine_step.argtypes = [P(PlyRefineDesc), ctypes.c_void_p]
     lib.ps_ply_refine_step.restype = ctypes.c_int
+    lib.ps_ply_densify_workspace_bytes.argtypes = [ctypes.c_int64, P(ctypes.c_size_t)]
+    lib.ps_ply_densify_workspace_bytes.restype = ctypes.c_int
+    lib.ps_ply_densify_stats.argtypes = [ctypes.c_int64, ctypes.c_int32] + [ctypes.c_void_p] * 5
+    lib.ps_ply_densify_stats.restype = ctypes.c_int
+    lib.ps_ply_densify_count.argtypes = [P(PlyDensifyDesc)] + [ctypes.c_void_p] * 4 + [ctypes.c_size_t] + \
+        [ctypes.c_void_p] * 2
+    lib.ps_ply_densify_count.restype = ctypes.c_int
+    lib.ps_ply_densify_apply.argtypes = [P(PlyDensifyDesc)] + [ctypes.c_void_p] * 5 + [ctypes.c_size_t] + \
+        [ctypes.c_void_p] * 5
+    lib.ps_ply_densify_apply.restype = ctypes.c_int
     for f in ("ps_raster_sizes_query", "ps_raster_layout_query", "ps_raster_forward", "ps_raster_backward"):
         getattr(lib, f).restype = ctypes.c_int
     return lib

@@ -12,41 +12,12 @@
 // of the unpack's outputs, forms each record's gradient (unpack_record_backward), updates the CTA's record entries
 // and moments in file order, and unpacks the updated records through the same unpack_record.
 #include "adam.cuh"
-#include "ps_common.cuh"
+#include "ply_stage.cuh"
 
 namespace ps {
 
-constexpr int kPlyImportThreads = 64;
-
-// Odd strides: a warp's threads read the same column of 32 staged rows (and write the same entry of 32 outputs), so
-// an even stride would put several of them in one shared-memory bank.
-__host__ __device__ constexpr int odd(int n) { return n | 1; }
-
 __host__ __device__ constexpr int ply_import_smem_floats(int n_props, int sh_coeffs) {
     return kPlyImportThreads * (odd(n_props) + 3 + 9 + 1 + odd(3 * sh_coeffs));
-}
-
-// `count` floats to global `dst` (16-byte aligned): element e is src[(e / width) stride + e % width] in shared memory
-__device__ __forceinline__ void store_range(float *__restrict__ dst, const float *__restrict__ src, int count,
-                                            int width, int stride) {
-    auto at = [&](int e) { const int row = e / width; return src[row * stride + e - row * width]; };
-    float4 *d4 = reinterpret_cast<float4 *>(dst);
-    for (int i = threadIdx.x; i < count / 4; i += kPlyImportThreads)
-        d4[i] = make_float4(at(4 * i), at(4 * i + 1), at(4 * i + 2), at(4 * i + 3));
-    for (int i = (count & ~3) + threadIdx.x; i < count; i += kPlyImportThreads) dst[i] = at(i);
-}
-
-// Staging: `total` floats of global `src` (16-byte aligned) into shared memory, element e to
-// dst[(e / width) stride + e % width].  store_range reversed.
-__device__ __forceinline__ void load_range(float *__restrict__ dst, const float *__restrict__ src, int count,
-                                           int width, int stride) {
-    auto put = [&](int e, float v) { const int row = e / width; dst[row * stride + e - row * width] = v; };
-    const float4 *s4 = reinterpret_cast<const float4 *>(src);
-    for (int i = threadIdx.x; i < count / 4; i += kPlyImportThreads) {
-        const float4 v = __ldg(s4 + i);
-        put(4 * i, v.x); put(4 * i + 1, v.y); put(4 * i + 2, v.z); put(4 * i + 3, v.w);
-    }
-    for (int i = (count & ~3) + threadIdx.x; i < count; i += kPlyImportThreads) put(i, __ldg(src + i));
 }
 
 // What the covariance of a record is made of: the normalised quaternion (identity for a zero one), R(q^), the
@@ -59,17 +30,9 @@ struct RecordShape {
 __device__ __forceinline__ void record_shape(const ps_ply_import_desc &d, const float *r, RecordShape &o) {
     const double s = d.scale;
     double qw = r[d.col_rot[0]], qx = r[d.col_rot[1]], qy = r[d.col_rot[2]], qz = r[d.col_rot[3]];
-    const double qn = qw * qw + qx * qx + qy * qy + qz * qz;
-    if (qn > 0.0) {
-        const double inv = 1.0 / sqrt(qn);
-        qw *= inv; qx *= inv; qy *= inv; qz *= inv;
-    } else {
-        qw = 1.0;   // a zero quaternion is the identity rotation
-    }
-    o.qw = qw; o.qx = qx; o.qy = qy; o.qz = qz; o.qn = qn;
-    const double rot[3][3] = {{1.0 - 2.0 * (qy * qy + qz * qz), 2.0 * (qx * qy - qw * qz), 2.0 * (qx * qz + qw * qy)},
-                              {2.0 * (qx * qy + qw * qz), 1.0 - 2.0 * (qx * qx + qz * qz), 2.0 * (qy * qz - qw * qx)},
-                              {2.0 * (qx * qz - qw * qy), 2.0 * (qy * qz + qw * qx), 1.0 - 2.0 * (qx * qx + qy * qy)}};
+    double rot[3][3];
+    o.qn = unit_rotation(qw, qx, qy, qz, rot);
+    o.qw = qw; o.qx = qx; o.qy = qy; o.qz = qz;
 #pragma unroll
     for (int i = 0; i < 3; ++i)
 #pragma unroll

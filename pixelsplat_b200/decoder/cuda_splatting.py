@@ -99,10 +99,11 @@ def _render(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor, i
             background_color: Tensor, gaussian_means: Tensor, gaussian_covariances: Tensor,
             gaussian_sh_coefficients: Tensor, gaussian_opacities: Tensor, scale_invariant: bool, use_sh: bool = True,
             state_out: Optional[list] = None, target: Optional[Tensor] = None,
-            mode: Optional[DepthRenderingMode] = None, want_color: bool = True):
+            mode: Optional[DepthRenderingMode] = None, want_color: bool = True, means2d: Optional[Tensor] = None):
     """One rasterizer call for [s, v] cameras over [s, g] Gaussians, with the loss epilogue when `target`
-    [s, v, 3, h, w] is given and the depth channel when `mode` is.  -> (color [s, v, 3, h, w] or None when
-    want_color=False, depth [s, v, h, w] | None, sse [s, v] | None, sse_clipped [s, v] | None)."""
+    [s, v, 3, h, w] is given, the depth channel when `mode` is, and the projected means' gradient into `means2d`
+    [s v, g, 3] when it is given.  -> (color [s, v, 3, h, w] or None when want_color=False, depth [s, v, h, w] | None,
+    sse [s, v] | None, sse_clipped [s, v] | None, radii [s v, g] int32)."""
     s, v = extrinsics.shape[:2]
     n = s * v
     h, w = image_shape
@@ -112,7 +113,7 @@ def _render(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor, i
         colors, layout = gaussian_sh_coefficients, _lib.PS_SH_3M
     else:
         colors, layout = gaussian_sh_coefficients[..., 0], _lib.PS_SH_M3
-    color, depth, _, sse, sse_clipped = _rasterize(
+    color, depth, radii, sse, sse_clipped = _rasterize(
         gaussian_means, gaussian_covariances, gaussian_opacities, colors,
         viewmatrix=cams["viewmatrix"], projmatrix=cams["projmatrix"], campos=cams["campos"],
         tanfov=cams["tanfov"], background=background_color.reshape(n, 3).to(torch.float32),
@@ -121,11 +122,11 @@ def _render(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor, i
         state_out=state_out, target=None if target is None else target.reshape(n, 3, h, w).to(torch.float32),
         depth_mode=mode,
         near_far=None if mode is None else torch.stack([near.reshape(n), far.reshape(n)], -1).to(torch.float32),
-        want_color=want_color)
+        want_color=want_color, means2d=means2d)
     return (color.reshape(s, v, 3, h, w) if want_color else None,
             None if depth is None else depth.reshape(s, v, h, w),
             None if sse is None else sse.reshape(s, v),
-            None if sse_clipped is None else sse_clipped.reshape(s, v))
+            None if sse_clipped is None else sse_clipped.reshape(s, v), radii)
 
 
 def render_views(
@@ -145,7 +146,7 @@ def render_views(
 ) -> Tensor:                       # [s, v, 3, h, w]
     """V cameras per scene share the scene's Gaussians (no `repeat`)."""
     assert use_sh or gaussian_sh_coefficients.shape[-1] == 1
-    color, _, _, _ = _render(extrinsics, intrinsics, near, far, image_shape, background_color, gaussian_means,
+    color, _, _, _, _ = _render(extrinsics, intrinsics, near, far, image_shape, background_color, gaussian_means,
                              gaussian_covariances, gaussian_sh_coefficients, gaussian_opacities, scale_invariant,
                              use_sh=use_sh, state_out=state_out)
     return color
@@ -159,10 +160,25 @@ def render_views_mse(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: 
     [s, v, 3, h, w] -> (sse [s, v] differentiable sum of squared errors, sse_clipped [s, v] the same on images
     clipped to [0, 1] (what compute_psnr needs), color [s, v, 3, h, w] detached or None).  See
     pixelsplat_b200/loss.py for the LossMse / PSNR built on top."""
-    color, _, sse, sse_clipped = _render(extrinsics, intrinsics, near, far, image_shape, background_color,
+    color, _, sse, sse_clipped, _ = _render(extrinsics, intrinsics, near, far, image_shape, background_color,
                                          gaussian_means, gaussian_covariances, gaussian_sh_coefficients,
                                          gaussian_opacities, scale_invariant, target=target, want_color=want_color)
     return sse, sse_clipped, color
+
+
+def render_views_mse_means2d(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor,
+                             image_shape: tuple[int, int], background_color: Tensor, gaussian_means: Tensor,
+                             gaussian_covariances: Tensor, gaussian_sh_coefficients: Tensor,
+                             gaussian_opacities: Tensor, target: Tensor, means2d: Tensor, scale_invariant: bool = True,
+                             want_color: bool = True):
+    """render_views_mse with upstream's screen-space gradient holder: `means2d` [s v, g, 3], a tensor that requires
+    grad, receives the gradient of the loss with respect to each view's projected means (3DGS's densification
+    statistic).  -> (sse [s, v], sse_clipped [s, v], color or None, radii [s v, g] int32)."""
+    color, _, sse, sse_clipped, radii = _render(extrinsics, intrinsics, near, far, image_shape, background_color,
+                                                gaussian_means, gaussian_covariances, gaussian_sh_coefficients,
+                                                gaussian_opacities, scale_invariant, target=target,
+                                                want_color=want_color, means2d=means2d)
+    return sse, sse_clipped, color, radii
 
 
 def _legacy_compositor() -> bool:
@@ -185,7 +201,7 @@ def render_views_with_depth(extrinsics: Tensor, intrinsics: Tensor, near: Tensor
                              state_out=state_out)
         return color, render_depth_views(extrinsics, intrinsics, near, far, image_shape, gaussian_means,
                                          gaussian_covariances, gaussian_opacities, scale_invariant, mode)
-    color, depth, _, _ = _render(extrinsics, intrinsics, near, far, image_shape, background_color, gaussian_means,
+    color, depth, _, _, _ = _render(extrinsics, intrinsics, near, far, image_shape, background_color, gaussian_means,
                                  gaussian_covariances, gaussian_sh_coefficients, gaussian_opacities, scale_invariant,
                                  state_out=state_out, mode=mode)
     return color, depth
@@ -198,7 +214,7 @@ def render_views_mse_with_depth(extrinsics: Tensor, intrinsics: Tensor, near: Te
                                 mode: DepthRenderingMode = "depth", want_color: bool = True):
     """render_views_mse with the depth channel of render_views_with_depth: -> (sse [s, v], sse_clipped [s, v],
     color [s, v, 3, h, w] detached or None, depth [s, v, h, w] differentiable)."""
-    color, depth, sse, sse_clipped = _render(extrinsics, intrinsics, near, far, image_shape, background_color,
+    color, depth, sse, sse_clipped, _ = _render(extrinsics, intrinsics, near, far, image_shape, background_color,
                                              gaussian_means, gaussian_covariances, gaussian_sh_coefficients,
                                              gaussian_opacities, scale_invariant, target=target, mode=mode,
                                              want_color=want_color)

@@ -38,7 +38,10 @@ one file about its +z axis as an mp4, colour beside turbo depth.
 
 refines each index scene's <ply>/<scene>.ply (pixelsplat_b200.ply_refine) in its world against the scene's context
 views only, and writes <output>/<scene>.ply, a copy of <scene>.frame.json and refine.json (each scene's context-view
-MSE before and after).  render-ply --ply <output> then scores the refined scenes on the held-out targets.
+MSE before and after).  --densify-until N adds 3DGS's densification, pruning and opacity reset before step N
+(--densify-from, --densify-every, --densify-grad, --min-opacity, --opacity-reset-every, --densify-seed; 3DGS's
+defaults), and refine.json's gaussians_before / gaussians_after.  render-ply --ply <output> then scores the refined
+scenes on the held-out targets.
 
     python -m pixelsplat_b200.evaluation generate-index --dataset-root datasets/re10k \
         --output outputs/evaluation_index_re10k [--video]
@@ -65,6 +68,7 @@ lpips package's lin weights from disk (--lpips-vgg / --lpips-lin, or where those
 from __future__ import annotations
 
 import argparse
+import dataclasses
 import json
 import sys
 from pathlib import Path
@@ -390,7 +394,7 @@ def _non_negative(kind):
 
 
 def parse_refine_ply(argv: list[str]) -> argparse.Namespace:
-    from ..ply_refine import DEFAULT_LR, GROUPS
+    from ..ply_refine import DEFAULT_LR, GROUPS, DensifyConfig
     p = argparse.ArgumentParser(prog="python -m pixelsplat_b200.evaluation refine-ply",
                                 description="Refine exported 3D Gaussian splatting PLY files on each test scene's "
                                             "context views.")
@@ -406,8 +410,34 @@ def parse_refine_ply(argv: list[str]) -> argparse.Namespace:
     for g in GROUPS:
         p.add_argument(f"--lr-{g.replace('_', '-')}", dest=f"lr_{g}", type=_non_negative(float), default=DEFAULT_LR[g],
                        help=f"learning rate of the {g} properties (default: 3DGS's {DEFAULT_LR[g]:g})")
+    d = DensifyConfig()
+    p.add_argument("--densify-until", type=_non_negative(int), default=0,
+                   help="densify, prune and reset opacities before this step, as 3DGS does (default: 0, off; "
+                        f"3DGS: {d.until_step})")
+    p.add_argument("--densify-from", type=_non_negative(int), default=d.from_step,
+                   help=f"densify after this step (default: 3DGS's {d.from_step})")
+    p.add_argument("--densify-every", type=int, default=d.every,
+                   help=f"steps between densifications (default: 3DGS's {d.every})")
+    p.add_argument("--densify-grad", type=_non_negative(float), default=d.grad_threshold,
+                   help=f"mean screen-space gradient norm that selects a Gaussian (default: 3DGS's "
+                        f"{d.grad_threshold:g}, calibrated for its loss, not this one)")
+    p.add_argument("--min-opacity", type=_non_negative(float), default=d.min_opacity,
+                   help=f"prune Gaussians below this opacity (default: 3DGS's {d.min_opacity:g})")
+    p.add_argument("--opacity-reset-every", type=_non_negative(int), default=d.opacity_reset_every,
+                   help=f"steps between opacity resets, 0 for none (default: 3DGS's {d.opacity_reset_every})")
+    p.add_argument("--densify-seed", type=_non_negative(int), default=d.seed,
+                   help=f"seed of the split copies' draws (default: {d.seed})")
     args = p.parse_args(argv)
     args.lr = {g: getattr(args, f"lr_{g}") for g in GROUPS}
+    args.densify = None
+    if args.densify_until > 0:
+        try:
+            args.densify = DensifyConfig(from_step=args.densify_from, until_step=args.densify_until,
+                                         every=args.densify_every, grad_threshold=args.densify_grad,
+                                         min_opacity=args.min_opacity, opacity_reset_every=args.opacity_reset_every,
+                                         seed=args.densify_seed)
+        except ValueError as e:
+            p.error(str(e))
     return args
 
 
@@ -437,7 +467,7 @@ def refine_ply(argv: list[str]) -> dict:
         result = refine(args.ply / f"{scene}.ply", frame, extrinsics=ctx["extrinsics"][0],
                         intrinsics=ctx["intrinsics"][0], near=ctx["near"][0], far=ctx["far"][0],
                         images=ctx["image"][0], background_color=background, steps=args.steps,
-                        out_path=args.output / f"{scene}.ply", lr=args.lr, device=device)
+                        out_path=args.output / f"{scene}.ply", lr=args.lr, device=device, densify=args.densify)
         shutil.copyfile(frame, args.output / f"{scene}.frame.json")
         if result is None:   # --steps 0: the file is copied; its MSE is one render
             layout, records = read_ply_body(args.ply / f"{scene}.ply", device)
@@ -447,11 +477,20 @@ def refine_ply(argv: list[str]) -> dict:
                                     images=ctx["image"][0], background_color=background, steps=0)
         loss = result.loss.tolist()
         scenes[scene] = {"mse_before": loss[0], "mse_after": loss[-1], "steps": args.steps}
-        print(f"{scene}: context MSE {loss[0]:.6f} -> {loss[-1]:.6f} in {args.steps} steps")
+        line = f"{scene}: context MSE {loss[0]:.6f} -> {loss[-1]:.6f} in {args.steps} steps"
+        if args.densify is not None:
+            before, after = (result.gaussians[0], result.gaussians[-1]) if result.gaussians else (None, None)
+            if before is None:   # --steps 0: the file is copied
+                before = after = result.records.shape[0]
+            scenes[scene].update(gaussians_before=before, gaussians_after=after)
+            line += f", {before} -> {after} Gaussians"
+        print(line)
     missing = sorted(wanted - set(scenes)) if wanted is not None else []
     if missing:
         raise SystemExit(f"evaluation refine-ply: no index scene named {', '.join(missing)}")
     out = {"steps": args.steps, "lr": args.lr, "scenes": scenes}
+    if args.densify is not None:
+        out["densify"] = dataclasses.asdict(args.densify)
     args.output.mkdir(parents=True, exist_ok=True)
     (args.output / "refine.json").write_text(json.dumps(out, indent=1) + "\n")
     return out

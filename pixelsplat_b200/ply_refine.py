@@ -4,11 +4,20 @@
 Each step renders the views with `render_views_mse` (the unpacked Gaussians are the autograd leaves), then one kernel
 (csrc/ply_import.cu, `ps_ply_refine_step`) differentiates the unpack, applies Adam with one learning rate per
 property group and unpacks the updated records into the Gaussians the next step renders.  Records stay in the file's
-layout throughout, so a refined file has the input's header and property order.
+layout throughout, so a refined file has the input's header and property order (with densification, a new vertex
+count).
 
 Learning rates are 3DGS's per-group rates.  The position rate is in the file's units: a viewer-format export
 normalises the scene so that the 0.95 quantile of its centred means is 1 (`ply_export.export_frame`), which plays the
-part of 3DGS's scene extent.  The position rate is constant; there is no densification, pruning or opacity reset.
+part of 3DGS's scene extent.  The position rate is constant.
+
+With a `DensifyConfig`, the loop also runs 3DGS's adaptive density control (csrc/ply_densify.cu): each step before
+`until_step` renders with a screen-space gradient holder and folds each view's projected-mean gradient norm into
+per-Gaussian statistics; every `every` steps after `from_step` the records are cloned, split and pruned in 3DGS's
+order, with the Adam moments carried along (zero for new rows); every `opacity_reset_every` steps the opacity logits
+are clamped to logit(0.01).  The scene extent is 1 in a viewer-format export's units.  The gradient threshold is
+3DGS's 2e-4, which was calibrated for its single-view L1 + D-SSIM loss, not for the fused MSE over all context
+views minimised here; it has not been tuned for this loss.
 """
 from __future__ import annotations
 
@@ -40,6 +49,48 @@ class RefineResult:
     loss: Tensor
     exp_avg: Optional[Tensor] = None
     exp_avg_sq: Optional[Tensor] = None
+    gaussians: Optional[list[int]] = None    # with densification: the record count at each entry of `loss`
+
+
+@dataclass
+class DensifyConfig:
+    """3DGS's adaptive density control during refinement; the defaults are 3DGS's.  At step t (1-based):
+    statistics are kept while t < until_step; clone / split / prune runs when from_step < t < until_step and
+    t % every == 0; the opacity reset runs when opacity_reset_every > 0, t % opacity_reset_every == 0 and
+    t < until_step; the world-size prune (max scale above 0.1 extent) is on once t > opacity_reset_every (with the
+    reset on).  `extent` is the scene extent in the records' units; `seed` seeds the split copies' draws."""
+    from_step: int = 500
+    until_step: int = 15000
+    every: int = 100
+    grad_threshold: float = 2e-4
+    percent_dense: float = 0.01
+    min_opacity: float = 0.005
+    opacity_reset_every: int = 3000
+    extent: float = 1.0
+    seed: int = 0
+
+    def __post_init__(self):
+        for k in ("from_step", "until_step", "every", "opacity_reset_every", "seed"):
+            v = getattr(self, k)
+            if isinstance(v, bool) or not isinstance(v, int) or v < (1 if k == "every" else 0):
+                raise ValueError(f"DensifyConfig.{k} must be an int >= {1 if k == 'every' else 0}, got {v!r}")
+        for k in ("grad_threshold", "percent_dense", "min_opacity", "extent"):
+            v = getattr(self, k)
+            if not (isinstance(v, (int, float)) and math.isfinite(v) and v >= 0) or (k == "extent" and v <= 0):
+                raise ValueError(f"DensifyConfig.{k} must be a finite number {'> 0' if k == 'extent' else '>= 0'}, "
+                                 f"got {v!r}")
+
+    def stats_at(self, t: int) -> bool:
+        return t < self.until_step
+
+    def densifies_at(self, t: int) -> bool:
+        return self.from_step < t < self.until_step and t % self.every == 0
+
+    def resets_at(self, t: int) -> bool:
+        return self.opacity_reset_every > 0 and t % self.opacity_reset_every == 0 and t < self.until_step
+
+    def prunes_world_at(self, t: int) -> bool:
+        return self.opacity_reset_every > 0 and t > self.opacity_reset_every
 
 
 def group_of(name: str, sh_degree: int) -> Optional[str]:
@@ -130,6 +181,106 @@ class RefineStep:
         _lib.check(rc, "ps_ply_refine_step")
 
 
+MAX_GAUSSIANS = 2 ** 31 - 1    # the rasterizer's int32 n_gaussians
+OPACITY_RESET_LOGIT = math.log(0.01 / 0.99)
+
+
+def _stream(dev) -> ctypes.c_void_p:
+    return ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def _dense(name: str, t: Tensor, shape, dtype, dev) -> None:
+    if not isinstance(t, Tensor) or tuple(t.shape) != tuple(shape) or t.dtype != dtype or t.device != dev \
+            or not t.is_contiguous():
+        raise ValueError(f"densify: `{name}` must be a dense {str(dtype)[6:]} {list(shape)} tensor on {dev}")
+
+
+def densify_stats(d_means2d: Tensor, radii: Tensor, accum: Tensor, count: Tensor) -> None:
+    """`ps_ply_densify_stats`: for each view v where radii[v, i] > 0, accum[i] += |d_means2d[v, i, :2]| and
+    count[i] += 1, in place.  d_means2d float32 [V, n, 3], radii int32 [V, n], accum float32 [n], count int32 [n]."""
+    v, n = radii.shape
+    dev = accum.device
+    _dense("d_means2d", d_means2d, (v, n, 3), torch.float32, dev)
+    _dense("radii", radii, (v, n), torch.int32, dev)
+    _dense("accum", accum, (n,), torch.float32, dev)
+    _dense("count", count, (n,), torch.int32, dev)
+    with torch.cuda.device(dev):
+        rc = _lib.lib.ps_ply_densify_stats(n, v, d_means2d.data_ptr(), radii.data_ptr(), accum.data_ptr(),
+                                           count.data_ptr(), _stream(dev))
+    _lib.check(rc, "ps_ply_densify_stats")
+
+
+def densify_desc(properties, n: int, cfg: DensifyConfig, prune_world: bool) -> _lib.PlyDensifyDesc:
+    col = {name: i for i, name in enumerate(properties)}
+    need = ["x", "y", "z", "opacity"] + [f"scale_{k}" for k in range(3)] + [f"rot_{k}" for k in range(4)]
+    missing = [k for k in need if k not in col]
+    if missing:
+        raise ValueError(f"densify: the records have no {', '.join(missing)} property")
+    return _lib.PlyDensifyDesc(
+        n_gaussians=n, n_props=len(properties), prune_world=int(prune_world),
+        col_xyz=(ctypes.c_int32 * 3)(*(col[k] for k in "xyz")), col_opacity=col["opacity"],
+        col_scale=(ctypes.c_int32 * 3)(*(col[f"scale_{k}"] for k in range(3))),
+        col_rot=(ctypes.c_int32 * 4)(*(col[f"rot_{k}"] for k in range(4))),
+        grad_threshold=cfg.grad_threshold, percent_dense=cfg.percent_dense, min_opacity=cfg.min_opacity,
+        extent=cfg.extent)
+
+
+def densify_workspace_bytes(n: int) -> int:
+    out = ctypes.c_size_t()
+    _lib.check(_lib.lib.ps_ply_densify_workspace_bytes(n, ctypes.byref(out)), "ps_ply_densify_workspace_bytes")
+    return out.value
+
+
+def densify_records(records: Tensor, exp_avg: Tensor, exp_avg_sq: Tensor, accum: Tensor, count: Tensor, properties,
+                    cfg: DensifyConfig, *, prune_world: bool, eps: Tensor, out=None):
+    """3DGS's clone / split / prune of `records` [n, P] with their Adam moments (`ps_ply_densify_count`, one read of
+    the new count, then `ps_ply_densify_apply`), from the statistics accum [n] / count [n] and the split draws `eps`
+    float32 [2, n, 3].  -> (records, exp_avg, exp_avg_sq) [n_new, P]: kept originals, clones, first and second split
+    copies.  `out`, when given, is three float32 [>= n_new, P] tensors to write instead of new ones.  Raises
+    ValueError, with nothing written, when n_new would be 0 or above the rasterizer's MAX_GAUSSIANS."""
+    n, p = records.shape
+    dev = records.device
+    if not records.is_cuda:
+        raise ValueError("densify: `records` must be a CUDA tensor (pixelsplat_b200 has no CPU path)")
+    for name, t in (("records", records), ("exp_avg", exp_avg), ("exp_avg_sq", exp_avg_sq)):
+        _dense(name, t, (n, p), torch.float32, dev)
+    _dense("accum", accum, (n,), torch.float32, dev)
+    _dense("count", count, (n,), torch.int32, dev)
+    _dense("eps", eps, (2, n, 3), torch.float32, dev)
+    desc = densify_desc(properties, n, cfg, prune_world)
+    ws = torch.empty(densify_workspace_bytes(n), dtype=torch.uint8, device=dev)
+    counts = torch.empty(4, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        rc = _lib.lib.ps_ply_densify_count(ctypes.byref(desc), records.data_ptr(), accum.data_ptr(), count.data_ptr(),
+                                           ws.data_ptr(), ws.numel(), counts.data_ptr(), _stream(dev))
+    _lib.check(rc, "ps_ply_densify_count")
+    n_new = int(counts[3].item())      # the one device-to-host synchronisation of a densification
+    if n_new == 0:
+        raise ValueError("densify: every Gaussian would be pruned; lower min_opacity or densify less often")
+    if n_new > MAX_GAUSSIANS:
+        raise ValueError(f"densify: {n_new} Gaussians are more than the rasterizer takes ({MAX_GAUSSIANS})")
+    if out is None:
+        out = [torch.empty((n_new, p), device=dev) for _ in range(3)]
+    for name, t in zip(("records_out", "exp_avg_out", "exp_avg_sq_out"), out):
+        if not isinstance(t, Tensor) or t.dim() != 2 or t.shape[0] < n_new or t.shape[1] != p \
+                or t.dtype != torch.float32 or t.device != dev or not t.is_contiguous():
+            raise ValueError(f"densify: `{name}` must be a dense float32 [>= {n_new}, {p}] tensor on {dev}")
+    with torch.cuda.device(dev):
+        rc = _lib.lib.ps_ply_densify_apply(ctypes.byref(desc), records.data_ptr(), exp_avg.data_ptr(),
+                                           exp_avg_sq.data_ptr(), eps.data_ptr(), ws.data_ptr(), ws.numel(),
+                                           counts.data_ptr(), *(t.data_ptr() for t in out), _stream(dev))
+    _lib.check(rc, "ps_ply_densify_apply")
+    return tuple(t[:n_new] for t in out)
+
+
+def reset_opacity(records: Tensor, exp_avg: Tensor, exp_avg_sq: Tensor, properties) -> None:
+    """3DGS's opacity reset, in place: o = min(o, logit(0.01)) and the opacity column's moments set to 0."""
+    c = list(properties).index("opacity")
+    records[:, c].clamp_(max=OPACITY_RESET_LOGIT)
+    exp_avg[:, c] = 0.0
+    exp_avg_sq[:, c] = 0.0
+
+
 def refine_step(records: Tensor, properties, sh_degree: int, exp_avg: Tensor, exp_avg_sq: Tensor, grads, out,
                 step: int, *, frame: Optional[ExportFrame] = None, lr: Optional[dict] = None,
                 records_out: Optional[Tensor] = None, d_records: Optional[Tensor] = None,
@@ -143,28 +294,36 @@ def refine_step(records: Tensor, properties, sh_degree: int, exp_avg: Tensor, ex
 
 def refine_records(records: Tensor, properties, sh_degree: int, *, frame: Optional[ExportFrame] = None,
                    extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor, images: Tensor,
-                   background_color: Tensor, steps: int, lr: Optional[dict] = None) -> RefineResult:
+                   background_color: Tensor, steps: int, lr: Optional[dict] = None,
+                   densify: Optional[DensifyConfig] = None) -> RefineResult:
     """`steps` Adam steps on `records` (float32 [n, P] on a CUDA device, from `ply_import.read_ply_body` or
     `ply_export.pack_viewer`, with `properties`) against the MSE of renders of the views (extrinsics [v, 4, 4],
     intrinsics [v, 3, 3], near / far [v], images [v, 3, h, w], background_color [3]) in the world of `frame`.
-    `lr` maps groups (GROUPS) to learning rates over DEFAULT_LR.  The input is not modified; with steps=0 it is
-    returned as it is."""
+    `lr` maps groups (GROUPS) to learning rates over DEFAULT_LR.  With `densify`, 3DGS's densification, pruning and
+    opacity reset run after each step's Adam update as the config schedules them, and the result's `gaussians` holds
+    the count at each loss entry.  The input is not modified; with steps=0 it is returned as it is."""
     from .decoder import Gaussians
-    from .decoder.cuda_splatting import render_views_mse
+    from .decoder.cuda_splatting import render_views_mse, render_views_mse_means2d
     from .ply_import import unpack_records
     properties = list(properties)
     if isinstance(steps, bool) or not isinstance(steps, int) or steps < 0:
         raise ValueError(f"refine_records: `steps` must be an int >= 0, got {steps!r}")
     column_lr(properties, sh_degree, lr)
+    if densify is not None and not isinstance(densify, DensifyConfig):
+        raise ValueError(f"refine_records: `densify` must be a DensifyConfig or None, got {densify!r}")
     dev = records.device
     v, _, h, w = images.shape
     views = [t.to(dev, torch.float32)[None] for t in (extrinsics, intrinsics, near, far)]
     target = images.to(dev, torch.float32)[None]
     background = background_color.to(dev, torch.float32).reshape(1, 1, 3).expand(1, v, 3)
     n, coeffs = records.shape[0], (sh_degree + 1) ** 2
-    leaves = [torch.empty((1, n, 3), device=dev), torch.empty((1, n, 3, 3), device=dev),
-              torch.empty((1, n, 3, coeffs), device=dev), torch.empty((1, n), device=dev)]
-    out = Gaussians(*(t[0] for t in leaves))
+
+    def gaussians_for(count: int):
+        leaves = [torch.empty((1, count, 3), device=dev), torch.empty((1, count, 3, 3), device=dev),
+                  torch.empty((1, count, 3, coeffs), device=dev), torch.empty((1, count), device=dev)]
+        return leaves, Gaussians(*(t[0] for t in leaves))
+
+    leaves, out = gaussians_for(n)
     work = records if steps == 0 else records.clone().contiguous()
     unpack_records(work, properties, sh_degree, frame=frame, out=out)
     loss = torch.empty(steps + 1, device=dev)
@@ -175,31 +334,71 @@ def refine_records(records: Tensor, properties, sh_degree: int, *, frame: Option
         return sse.sum() / denom
 
     m = v2 = None
+    counts = None if densify is None else [n]
     if steps:
         m, v2 = torch.zeros_like(work), torch.zeros_like(work)
         step_fn = RefineStep(properties, sh_degree, n, sh_coeffs=coeffs, frame=frame, lr=lr)
         for leaf in leaves:
             leaf.requires_grad_(True)
+        if densify is not None:
+            accum = torch.zeros(n, device=dev)
+            seen = torch.zeros(n, dtype=torch.int32, device=dev)
+            draws = torch.Generator(dev).manual_seed(densify.seed)
         for t in range(1, steps + 1):
-            value = mse()
-            value.backward()
+            if densify is not None and densify.stats_at(t):
+                means2d = torch.zeros((v, n, 3), device=dev, requires_grad=True)
+                sse, _, _, radii = render_views_mse_means2d(*views, (h, w), background, *leaves, target=target,
+                                                            means2d=means2d, want_color=False)
+                value = sse.sum() / denom
+                value.backward()
+                densify_stats(means2d.grad, radii, accum, seen)
+            else:
+                value = mse()
+                value.backward()
             loss[t - 1] = value.detach()
             grads = [leaf.grad[0].contiguous() for leaf in leaves]
             for leaf in leaves:
                 leaf.grad = None
             step_fn(work, m, v2, grads, out, t)
+            if densify is None:
+                continue
+            if densify.densifies_at(t):
+                eps = torch.randn((2, n, 3), device=dev, generator=draws)
+                work, m, v2 = densify_records(work, m, v2, accum, seen, properties, densify,
+                                              prune_world=densify.prunes_world_at(t), eps=eps)
+                n = work.shape[0]
+                accum, seen = torch.zeros(n, device=dev), torch.zeros(n, dtype=torch.int32, device=dev)
+                leaves, out = gaussians_for(n)
+                step_fn = RefineStep(properties, sh_degree, n, sh_coeffs=coeffs, frame=frame, lr=lr)
+            if densify.resets_at(t):
+                reset_opacity(work, m, v2, properties)
+            if densify.densifies_at(t) or densify.resets_at(t):
+                unpack_records(work, properties, sh_degree, frame=frame, out=out)
+                for leaf in leaves:
+                    leaf.requires_grad_(True)
+            counts.append(n)
     with torch.no_grad():
         loss[steps] = mse()
-    return RefineResult(work, loss, m, v2)
+    return RefineResult(work, loss, m, v2, counts)
+
+
+def rewrite_vertex_count(head: bytes, count: int) -> bytes:
+    """The header bytes `head` (up to and including end_header) with the `element vertex N` line's N set to `count`;
+    every other byte is kept."""
+    start = head.index(b"\nelement vertex ") + len(b"\nelement vertex ")
+    end = head.index(b"\n", start)
+    return head[:start] + str(count).encode() + head[end:]
 
 
 def refine_ply(path: Union[Path, str], frame: Union[ExportFrame, Path, str, None], *, extrinsics: Tensor,
                intrinsics: Tensor, near: Tensor, far: Tensor, images: Tensor, background_color: Tensor, steps: int,
-               out_path: Union[Path, str], lr: Optional[dict] = None, device=None) -> Optional[RefineResult]:
+               out_path: Union[Path, str], lr: Optional[dict] = None, device=None,
+               densify: Optional[DensifyConfig] = None) -> Optional[RefineResult]:
     """`refine_records` on the file at `path` (in the world of `frame`: an `ExportFrame`, a `<scene>.frame.json`
-    path, or None for the file's own frame), written to `out_path` as the input's header bytes, unchanged, followed
-    by the refined records: property order, extra properties and comments are kept.  With steps=0 the input's
-    bytes are written as they are, without any device work, and the result is None."""
+    path, or None for the file's own frame), written to `out_path` as the input's header bytes followed by the
+    refined records: property order, extra properties and comments are kept, and only the `element vertex` count
+    changes when densification changed it.  With steps=0 the input's bytes are written as they are, without any
+    device work, and the result is None."""
     path, out_path = Path(path), Path(out_path)
     with open(path, "rb") as f:
         head = f.read(_MAX_HEADER_BYTES)
@@ -214,7 +413,10 @@ def refine_ply(path: Union[Path, str], frame: Union[ExportFrame, Path, str, None
     _, records = read_ply_body(path, device)
     result = refine_records(records, layout.properties, layout.sh_degree, frame=frame, extrinsics=extrinsics,
                             intrinsics=intrinsics, near=near, far=far, images=images,
-                            background_color=background_color, steps=steps, lr=lr)
+                            background_color=background_color, steps=steps, lr=lr, densify=densify)
     body = result.records.cpu().numpy().astype("<f4", copy=False).tobytes()
-    out_path.write_bytes(head[:layout.body_offset] + body)
+    header = head[:layout.body_offset]
+    if result.records.shape[0] != layout.count:
+        header = rewrite_vertex_count(header, result.records.shape[0])
+    out_path.write_bytes(header + body)
     return result
