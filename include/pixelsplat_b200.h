@@ -532,6 +532,23 @@ PS_API int ps_ssim_backward(int32_t n_planes, int32_t H, int32_t W, const float 
                             const float *d_mean, float *d_x /* or NULL */, float *d_y, void *workspace,
                             size_t workspace_bytes, void *stream);
 
+/* ---- 3DGS's L1 + D-SSIM loss (csrc/l1_dssim.cu) ------------------------------------------------------------
+ * For prediction `pred` and ground truth `gt` [n, C, H, W], per image: loss = (1 - lambda) L1 + lambda (1 - SSIM),
+ * L1 = mean |pred - gt|, SSIM = 3DGS's training SSIM: the 11x11 Gaussian window of sigma 1.5 correlated "same"-size
+ * with zero padding, population (co)variances, C1 = 0.01^2, C2 = 0.03^2, the map averaged over every pixel and channel
+ * (no crop; not the evaluation's ps_ssim_*).  Any H, W >= 1.  One launch over (plane, 16 x 32 tile) writes per-tile
+ * partial sums and, when d_pred is not NULL, d_pred = d(sum_n loss_n)/d pred (fully written; L1 part
+ * (1 - lambda) sign(pred - gt) / (C H W), sign(0) = 0); a second one adds the partials in a fixed order, so the
+ * results are the same bits every run and do not depend on whether d_pred is asked for.  No call synchronises the
+ * host.  Every entry point rejects a non-positive extent, a grid that does not fit one launch, lambda outside [0, 1]
+ * or NaN, NULL required pointers and a short workspace with PS_ERR_INVALID_ARGUMENT before anything is enqueued. */
+PS_API int ps_l1_dssim_workspace_bytes(int32_t n, int32_t C, int32_t H, int32_t W, size_t *out);
+
+/* out_loss [n]; out_l1 [n] and out_ssim [n] (the two terms) when not NULL. */
+PS_API int ps_l1_dssim(int32_t n, int32_t C, int32_t H, int32_t W, const float *pred, const float *gt, float lambda,
+                       float *out_loss, float *out_l1 /* or NULL */, float *out_ssim /* or NULL */,
+                       float *d_pred /* or NULL */, void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- ViT self-attention, flash-style (csrc/vit_attention.cu; wgmma, TF32 operands, FP32 accumulate) --------
  * The attention of DINO's ViT blocks, softmax(q k^T * scale) v, without any L x L tensor:
  *   qkv  [n_images, tokens, 3 * heads * 64]   "(qkv h d)": DINO's qkv(x).reshape(B, N, 3, H, C // H)

@@ -200,7 +200,7 @@ EXPORTS = ("ps_version", "ps_last_error", "ps_raster_sizes_query", "ps_raster_la
            "ps_eval_images_workspace_bytes", "ps_eval_images", "ps_clip_adam_segment_chunks",
            "ps_clip_adam_workspace_bytes", "ps_clip_adam_step", "ps_ply_pack", "ps_ply_unpack", "ps_view_overlap",
            "ps_ply_refine_step", "ps_ply_densify_workspace_bytes", "ps_ply_densify_stats", "ps_ply_densify_count",
-           "ps_ply_densify_apply")
+           "ps_ply_densify_apply", "ps_l1_dssim_workspace_bytes", "ps_l1_dssim")
 
 
 class NativeLibraryMissing(ImportError):
@@ -284,6 +284,11 @@ def _load() -> ctypes.CDLL:
     lib.ps_ssim_forward.restype = ctypes.c_int
     lib.ps_ssim_backward.argtypes = [ctypes.c_int32] * 3 + [ctypes.c_void_p] * 6 + [ctypes.c_size_t, ctypes.c_void_p]
     lib.ps_ssim_backward.restype = ctypes.c_int
+    lib.ps_l1_dssim_workspace_bytes.argtypes = [ctypes.c_int32] * 4 + [P(ctypes.c_size_t)]
+    lib.ps_l1_dssim_workspace_bytes.restype = ctypes.c_int
+    lib.ps_l1_dssim.argtypes = [ctypes.c_int32] * 4 + [ctypes.c_void_p] * 2 + [ctypes.c_float] + \
+        [ctypes.c_void_p] * 5 + [ctypes.c_size_t, ctypes.c_void_p]
+    lib.ps_l1_dssim.restype = ctypes.c_int
     lib.ps_lpips_workspace_bytes.argtypes = [P(LpipsDesc), P(ctypes.c_size_t)]
     lib.ps_lpips_workspace_bytes.restype = ctypes.c_int
     lib.ps_lpips_forward.argtypes = [P(LpipsDesc), ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]

@@ -181,6 +181,18 @@ def render_views_mse_means2d(extrinsics: Tensor, intrinsics: Tensor, near: Tenso
     return sse, sse_clipped, color, radii
 
 
+def render_views_means2d(extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor,
+                         image_shape: tuple[int, int], background_color: Tensor, gaussian_means: Tensor,
+                         gaussian_covariances: Tensor, gaussian_sh_coefficients: Tensor, gaussian_opacities: Tensor,
+                         means2d: Tensor, scale_invariant: bool = True):
+    """render_views with the screen-space gradient holder of render_views_mse_means2d, for a loss computed on the
+    colour render.  -> (color [s, v, 3, h, w] differentiable, radii [s v, g] int32)."""
+    color, _, _, _, radii = _render(extrinsics, intrinsics, near, far, image_shape, background_color, gaussian_means,
+                                    gaussian_covariances, gaussian_sh_coefficients, gaussian_opacities,
+                                    scale_invariant, means2d=means2d)
+    return color, radii
+
+
 def _legacy_compositor() -> bool:
     """The legacy CTA-per-tile compositor (composite_impl = 1) has no depth channel."""
     return _lib.get_option("composite_impl") == 1

@@ -40,8 +40,11 @@ refines each index scene's <ply>/<scene>.ply (pixelsplat_b200.ply_refine) in its
 views only, and writes <output>/<scene>.ply, a copy of <scene>.frame.json and refine.json (each scene's context-view
 MSE before and after).  --densify-until N adds 3DGS's densification, pruning and opacity reset before step N
 (--densify-from, --densify-every, --densify-grad, --min-opacity, --opacity-reset-every, --densify-seed; 3DGS's
-defaults), and refine.json's gaussians_before / gaussians_after.  render-ply --ply <output> then scores the refined
-scenes on the held-out targets.
+defaults), and refine.json's gaussians_before / gaussians_after.  --loss l1-dssim minimises 3DGS's
+(1 - lambda) L1 + lambda D-SSIM summed over the context views instead of their MSE (--lambda-dssim, 3DGS's 0.2;
+refine.json adds each scene's loss_before / loss_after), and --lr-xyz-final decays the position rate exponentially to
+that value over --lr-xyz-steps steps (default: --steps), as 3DGS's schedule does.  render-ply --ply <output> then
+scores the refined scenes on the held-out targets.
 
     python -m pixelsplat_b200.evaluation generate-index --dataset-root datasets/re10k \
         --output outputs/evaluation_index_re10k [--video]
@@ -393,6 +396,22 @@ def _non_negative(kind):
     return parse
 
 
+def _positive(kind):
+    def parse(text: str):
+        value = kind(text)
+        if not value > 0:
+            raise argparse.ArgumentTypeError(f"{text} is not positive")
+        return value
+    return parse
+
+
+def _unit_interval(text: str) -> float:
+    value = float(text)
+    if not 0 <= value <= 1:
+        raise argparse.ArgumentTypeError(f"{text} is not in [0, 1]")
+    return value
+
+
 def parse_refine_ply(argv: list[str]) -> argparse.Namespace:
     from ..ply_refine import DEFAULT_LR, GROUPS, DensifyConfig
     p = argparse.ArgumentParser(prog="python -m pixelsplat_b200.evaluation refine-ply",
@@ -420,14 +439,30 @@ def parse_refine_ply(argv: list[str]) -> argparse.Namespace:
                    help=f"steps between densifications (default: 3DGS's {d.every})")
     p.add_argument("--densify-grad", type=_non_negative(float), default=d.grad_threshold,
                    help=f"mean screen-space gradient norm that selects a Gaussian (default: 3DGS's "
-                        f"{d.grad_threshold:g}, calibrated for its loss, not this one)")
+                        f"{d.grad_threshold:g}, calibrated for its L1 + D-SSIM loss; with --loss mse the gradients "
+                        "are smaller and it has not been tuned)")
     p.add_argument("--min-opacity", type=_non_negative(float), default=d.min_opacity,
                    help=f"prune Gaussians below this opacity (default: 3DGS's {d.min_opacity:g})")
     p.add_argument("--opacity-reset-every", type=_non_negative(int), default=d.opacity_reset_every,
                    help=f"steps between opacity resets, 0 for none (default: 3DGS's {d.opacity_reset_every})")
     p.add_argument("--densify-seed", type=_non_negative(int), default=d.seed,
                    help=f"seed of the split copies' draws (default: {d.seed})")
+    p.add_argument("--loss", choices=("mse", "l1-dssim"), default="mse",
+                   help="mse: the MSE over the context views (default); l1-dssim: 3DGS's (1 - lambda) L1 + lambda "
+                        "D-SSIM, summed over the context views")
+    p.add_argument("--lambda-dssim", type=_unit_interval, default=0.2,
+                   help="D-SSIM weight of --loss l1-dssim (default: 3DGS's 0.2)")
+    p.add_argument("--lr-xyz-final", type=_positive(float), default=None,
+                   help="decay the position rate exponentially from --lr-xyz to this rate (default: off, a constant "
+                        "rate; 3DGS: 1.6e-6)")
+    p.add_argument("--lr-xyz-steps", type=_positive(int), default=None,
+                   help="steps of the position rate's decay (default: --steps; 3DGS: 30000)")
     args = p.parse_args(argv)
+    args.loss = args.loss.replace("-", "_")
+    if args.lr_xyz_steps is not None and args.lr_xyz_final is None:
+        p.error("--lr-xyz-steps needs --lr-xyz-final")
+    if args.lr_xyz_final is not None and not args.lr_xyz > 0:
+        p.error("--lr-xyz-final needs --lr-xyz > 0")
     args.lr = {g: getattr(args, f"lr_{g}") for g in GROUPS}
     args.densify = None
     if args.densify_until > 0:
@@ -439,6 +474,36 @@ def parse_refine_ply(argv: list[str]) -> argparse.Namespace:
         except ValueError as e:
             p.error(str(e))
     return args
+
+
+def _refine_options(args) -> dict:
+    """The refinement's loss and schedule arguments of `ply_refine.refine_records`."""
+    return dict(loss=args.loss, lambda_dssim=args.lambda_dssim, lr_xyz_final=args.lr_xyz_final,
+                lr_xyz_steps=args.lr_xyz_steps)
+
+
+def _refine_scene_report(args, result) -> dict:
+    """One scene's entry of refine.json: the context MSE before and after (with L1 + D-SSIM from the result's `mse`,
+    beside the mean per-view loss before and after)."""
+    loss = result.loss.tolist()
+    if args.loss == "mse":
+        return {"mse_before": loss[0], "mse_after": loss[-1], "steps": args.steps}
+    mse = result.mse.tolist()
+    return {"mse_before": mse[0], "mse_after": mse[-1], "steps": args.steps, "loss_before": loss[0],
+            "loss_after": loss[-1]}
+
+
+def _refine_report(args, scenes: dict) -> dict:
+    """refine.json: the settings and each scene's entry; the loss and the decay are recorded only when not off."""
+    out = {"steps": args.steps, "lr": args.lr, "scenes": scenes}
+    if args.densify is not None:
+        out["densify"] = dataclasses.asdict(args.densify)
+    if args.loss != "mse":
+        out.update(loss=args.loss, lambda_dssim=args.lambda_dssim)
+    if args.lr_xyz_final is not None:
+        out.update(lr_xyz_final=args.lr_xyz_final,
+                   lr_xyz_steps=args.steps if args.lr_xyz_steps is None else args.lr_xyz_steps)
+    return out
 
 
 def refine_ply(argv: list[str]) -> dict:
@@ -467,17 +532,21 @@ def refine_ply(argv: list[str]) -> dict:
         result = refine(args.ply / f"{scene}.ply", frame, extrinsics=ctx["extrinsics"][0],
                         intrinsics=ctx["intrinsics"][0], near=ctx["near"][0], far=ctx["far"][0],
                         images=ctx["image"][0], background_color=background, steps=args.steps,
-                        out_path=args.output / f"{scene}.ply", lr=args.lr, device=device, densify=args.densify)
+                        out_path=args.output / f"{scene}.ply", lr=args.lr, device=device, densify=args.densify,
+                        **_refine_options(args))
         shutil.copyfile(frame, args.output / f"{scene}.frame.json")
         if result is None:   # --steps 0: the file is copied; its MSE is one render
             layout, records = read_ply_body(args.ply / f"{scene}.ply", device)
             result = refine_records(records, layout.properties, layout.sh_degree,
                                     frame=read_frame_json(frame, device), extrinsics=ctx["extrinsics"][0],
                                     intrinsics=ctx["intrinsics"][0], near=ctx["near"][0], far=ctx["far"][0],
-                                    images=ctx["image"][0], background_color=background, steps=0)
-        loss = result.loss.tolist()
-        scenes[scene] = {"mse_before": loss[0], "mse_after": loss[-1], "steps": args.steps}
-        line = f"{scene}: context MSE {loss[0]:.6f} -> {loss[-1]:.6f} in {args.steps} steps"
+                                    images=ctx["image"][0], background_color=background, steps=0,
+                                    **_refine_options(args))
+        scenes[scene] = _refine_scene_report(args, result)
+        r = scenes[scene]
+        line = f"{scene}: context MSE {r['mse_before']:.6f} -> {r['mse_after']:.6f} in {args.steps} steps"
+        if args.loss != "mse":
+            line += f", L1 + D-SSIM {r['loss_before']:.6f} -> {r['loss_after']:.6f}"
         if args.densify is not None:
             before, after = (result.gaussians[0], result.gaussians[-1]) if result.gaussians else (None, None)
             if before is None:   # --steps 0: the file is copied
@@ -488,9 +557,7 @@ def refine_ply(argv: list[str]) -> dict:
     missing = sorted(wanted - set(scenes)) if wanted is not None else []
     if missing:
         raise SystemExit(f"evaluation refine-ply: no index scene named {', '.join(missing)}")
-    out = {"steps": args.steps, "lr": args.lr, "scenes": scenes}
-    if args.densify is not None:
-        out["densify"] = dataclasses.asdict(args.densify)
+    out = _refine_report(args, scenes)
     args.output.mkdir(parents=True, exist_ok=True)
     (args.output / "refine.json").write_text(json.dumps(out, indent=1) + "\n")
     return out

@@ -16,6 +16,10 @@ sm_90a kernels of csrc/ssim.cu (`ps_ssim_forward` / `ps_ssim_backward`) instead 
 loop over images.  `ssim` is differentiable in both images (1 - ssim is the usual partner of the photometric loss);
 `compute_ssim` is the no-grad metric.
 
+`l1_dssim` is 3DGS's photometric loss, (1 - lambda) L1 + lambda (1 - SSIM) per image with 3DGS's training SSIM
+(zero-padded window, population covariance, no crop: not the evaluation's `ssim`), as one sm_90a pass that writes
+the loss and its gradient (csrc/l1_dssim.cu, `ps_l1_dssim`).
+
 `LossLpips` / `LossLpipsCfg` / `LossLpipsCfgWrapper` and `compute_lpips` are the drop-ins for
 /root/reference/src/loss/loss_lpips.py and evaluation/metrics.py:22-33, on `pixelsplat_b200.lpips.Lpips` (VGG16 trunk
 in torch, the distance head fused in csrc/lpips.cu).
@@ -150,6 +154,57 @@ def ssim(ground_truth: Tensor, predicted: Tensor) -> Tensor:
 def compute_ssim(ground_truth: Tensor, predicted: Tensor) -> Tensor:
     """[batch, c, h, w] x 2 -> [batch] (metrics.py:36-52), on the prediction's device, without a host copy."""
     return ssim(ground_truth, predicted).to(predicted.dtype)
+
+
+class _L1Dssim(torch.autograd.Function):
+    """[n, c, h, w] x 2 -> [n]; the forward's one launch writes the gradient of the sum of the losses when the
+    prediction requires grad, and the backward scales each image's by its upstream gradient."""
+
+    @staticmethod
+    def forward(ctx, predicted: Tensor, ground_truth: Tensor, lambda_dssim: float) -> Tensor:
+        from . import _lib
+        n, c, h, w = predicted.shape
+        size = ctypes.c_size_t()
+        _lib.check(_lib.lib.ps_l1_dssim_workspace_bytes(n, c, h, w, ctypes.byref(size)), "ps_l1_dssim_workspace_bytes")
+        ws = torch.empty(size.value, dtype=torch.uint8, device=predicted.device)
+        out = torch.empty(n, dtype=torch.float32, device=predicted.device)
+        d_pred = torch.empty_like(predicted) if ctx.needs_input_grad[0] else None
+        stream = torch.cuda.current_stream(predicted.device).cuda_stream
+        rc = _lib.on_device(predicted.device, _lib.lib.ps_l1_dssim, n, c, h, w, predicted.data_ptr(),
+                            ground_truth.data_ptr(), lambda_dssim, out.data_ptr(), None, None,
+                            None if d_pred is None else d_pred.data_ptr(), ws.data_ptr(), ws.numel(), stream)
+        _lib.check(rc, "ps_l1_dssim")
+        if d_pred is not None:
+            ctx.save_for_backward(d_pred)
+        return out
+
+    @staticmethod
+    def backward(ctx, d_out: Tensor):
+        (d_pred,) = ctx.saved_tensors
+        return d_pred * d_out.to(d_pred.dtype).view(-1, 1, 1, 1), None, None
+
+
+def l1_dssim(predicted: Tensor, ground_truth: Tensor, lambda_dssim: float = 0.2) -> Tensor:
+    """3DGS's loss of each image, [n, c, h, w] x 2 float32 CUDA -> [n]: (1 - lambda_dssim) mean |predicted -
+    ground_truth| + lambda_dssim (1 - SSIM), with 3DGS's SSIM (11 x 11 Gaussian window of sigma 1.5 correlated with
+    zero padding, population (co)variances, C1 = 0.01^2, C2 = 0.03^2, mean over every pixel and channel).  Any
+    h, w >= 1.  Differentiable in `predicted` only: a ground truth that requires grad is refused.  Inputs are not
+    clipped."""
+    if predicted.dim() != 4 or ground_truth.shape != predicted.shape:
+        raise ValueError(f"l1_dssim: expected two [batch, channel, height, width] tensors of one shape, got "
+                         f"{tuple(predicted.shape)} and {tuple(ground_truth.shape)}")
+    if ground_truth.dtype != torch.float32 or predicted.dtype != torch.float32:
+        raise ValueError(f"l1_dssim: expected float32 images, got {predicted.dtype} and {ground_truth.dtype}")
+    if predicted.numel() == 0:
+        raise ValueError(f"l1_dssim: empty images {tuple(predicted.shape)}")
+    if isinstance(lambda_dssim, bool) or not isinstance(lambda_dssim, (int, float)) or not 0 <= lambda_dssim <= 1:
+        raise ValueError(f"l1_dssim: lambda_dssim must be a number in [0, 1], got {lambda_dssim!r}")
+    if not (ground_truth.is_cuda and predicted.is_cuda) or ground_truth.device != predicted.device:
+        raise ValueError(f"l1_dssim: expected CUDA tensors on one device, got {predicted.device} and "
+                         f"{ground_truth.device}; there is no CPU path")
+    if ground_truth.requires_grad:
+        raise ValueError("l1_dssim: the ground truth is not differentiated; detach it")
+    return _L1Dssim.apply(predicted.contiguous(), ground_truth.contiguous(), float(lambda_dssim))
 
 
 @dataclass

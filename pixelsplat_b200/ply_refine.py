@@ -1,7 +1,10 @@
 """Test-time refinement of a 3D Gaussian splatting scene: Adam on the vertex records of a PLY file (or of
-`ply_export.pack_viewer`), against the fused-MSE loss of renders of the scene's own views, as 3DGS optimises a scene.
+`ply_export.pack_viewer`), against a loss of renders of the scene's own views, as 3DGS optimises a scene.
 
-Each step renders the views with `render_views_mse` (the unpacked Gaussians are the autograd leaves), then one kernel
+The loss is the fused MSE over all views (`loss="mse"`, the default) or 3DGS's (1 - lambda) L1 + lambda D-SSIM
+(`loss="l1_dssim"`, `loss.l1_dssim`, csrc/l1_dssim.cu), summed over the views: each view's gradient is then the one
+3DGS's single-view step would give at that view.  Each step renders the views (with `render_views_mse`, or in colour
+with `render_views` for L1 + D-SSIM; the unpacked Gaussians are the autograd leaves), then one kernel
 (csrc/ply_import.cu, `ps_ply_refine_step`) differentiates the unpack, applies Adam with one learning rate per
 property group and unpacks the updated records into the Gaussians the next step renders.  Records stay in the file's
 layout throughout, so a refined file has the input's header and property order (with densification, a new vertex
@@ -9,15 +12,18 @@ count).
 
 Learning rates are 3DGS's per-group rates.  The position rate is in the file's units: a viewer-format export
 normalises the scene so that the 0.95 quantile of its centred means is 1 (`ply_export.export_frame`), which plays the
-part of 3DGS's scene extent.  The position rate is constant.
+part of 3DGS's scene extent.  The position rate is constant unless `lr_xyz_final` is given; then it decays
+exponentially from the xyz rate to `lr_xyz_final` over `lr_xyz_steps` steps, as 3DGS's schedule does (3DGS: 1.6e-6
+over 30 000 steps).
 
 With a `DensifyConfig`, the loop also runs 3DGS's adaptive density control (csrc/ply_densify.cu): each step before
 `until_step` renders with a screen-space gradient holder and folds each view's projected-mean gradient norm into
 per-Gaussian statistics; every `every` steps after `from_step` the records are cloned, split and pruned in 3DGS's
 order, with the Adam moments carried along (zero for new rows); every `opacity_reset_every` steps the opacity logits
 are clamped to logit(0.01).  The scene extent is 1 in a viewer-format export's units.  The gradient threshold is
-3DGS's 2e-4, which was calibrated for its single-view L1 + D-SSIM loss, not for the fused MSE over all context
-views minimised here; it has not been tuned for this loss.
+3DGS's 2e-4, which was calibrated for its L1 + D-SSIM loss: with `loss="l1_dssim"` each view's statistic is the
+quantity it was calibrated on; with the fused MSE over all context views the gradients are smaller, and the threshold
+has not been tuned for that loss.
 """
 from __future__ import annotations
 
@@ -38,18 +44,21 @@ GROUPS = ("xyz", "f_dc", "f_rest", "opacity", "scale", "rot")
 DEFAULT_LR = {"xyz": 0.00016, "f_dc": 0.0025, "f_rest": 0.0025 / 20, "opacity": 0.05, "scale": 0.005, "rot": 0.001}
 BETAS = (0.9, 0.999)
 EPS = 1e-15          # 3DGS's Adam eps
+LOSSES = ("mse", "l1_dssim")
 
 
 @dataclass
 class RefineResult:
     """`records` float32 [n, P] on the device, in the input's layout; `loss` float32 [steps + 1] on the device: the
-    context-view MSE before each step, and last the MSE of the refined records; `exp_avg` and `exp_avg_sq` the
-    Adam moments in the records' layout (None after no step)."""
+    loss before each step, and last the loss of the refined records (the context-view MSE, or with L1 + D-SSIM the
+    mean per-view loss, the objective over the number of views); `exp_avg` and `exp_avg_sq` the Adam moments in the
+    records' layout (None after no step)."""
     records: Tensor
     loss: Tensor
     exp_avg: Optional[Tensor] = None
     exp_avg_sq: Optional[Tensor] = None
     gaussians: Optional[list[int]] = None    # with densification: the record count at each entry of `loss`
+    mse: Optional[Tensor] = None             # with L1 + D-SSIM: float32 [2], the context-view MSE before and after
 
 
 @dataclass
@@ -127,7 +136,8 @@ class RefineStep:
     """`ps_ply_refine_step` for the records of one scene: n records with `properties`, SH degree `sh_degree`,
     Gaussians of `sh_coeffs` coefficients per channel, `frame`, learning rates `lr` (groups over DEFAULT_LR).  The
     descriptor (columns, frame, SH blocks, per-column rates) is built once, here; each call only sets the step
-    number and the pointers and enqueues the kernel, with nothing read back from the device."""
+    number, the pointers and, when given, the rate of the position columns, and enqueues the kernel, with nothing
+    read back from the device."""
 
     def __init__(self, properties, sh_degree: int, n: int, *, sh_coeffs: Optional[int] = None,
                  frame: Optional[ExportFrame] = None, lr: Optional[dict] = None,
@@ -141,14 +151,16 @@ class RefineStep:
         self.desc = _lib.PlyRefineDesc(unpack=import_desc(properties, sh_degree, self.coeffs, n, frame),
                                        beta1=betas[0], beta2=betas[1], eps=eps)
         self.desc.lr[:p] = column_lr(properties, sh_degree, lr)
+        self.xyz_columns = [i for i, name in enumerate(properties) if group_of(name, sh_degree) == "xyz"]
 
     def __call__(self, records: Tensor, exp_avg: Tensor, exp_avg_sq: Tensor, grads, out, step: int, *,
-                 records_out: Optional[Tensor] = None, d_records: Optional[Tensor] = None) -> None:
+                 records_out: Optional[Tensor] = None, d_records: Optional[Tensor] = None,
+                 lr_xyz: Optional[float] = None) -> None:
         """Adam step number `step` (>= 1): `grads` (d_means [n, 3], d_covariances [n, 3, 3], d_harmonics
         [n, 3, C], d_opacities [n]) are the loss's gradients for `out` (a `Gaussians` of the same shapes, the unpack
         of `records`); `records_out` (default: `records`, in place) and the moments are updated, `out` receives the
-        unpack of the updated records and `d_records`, when given, the records' gradient.  Every tensor is dense
-        float32 on the records' device."""
+        unpack of the updated records and `d_records`, when given, the records' gradient.  `lr_xyz`, when given,
+        is the position columns' rate from this call on.  Every tensor is dense float32 on the records' device."""
         n, p, c, dev = self.n, self.p, self.coeffs, records.device
         if not isinstance(records, Tensor) or not records.is_cuda:
             raise ValueError("refine_step: `records` must be a CUDA tensor (pixelsplat_b200 has no CPU path)")
@@ -168,6 +180,9 @@ class RefineStep:
                 raise ValueError(f"refine_step: `{name}` must be a dense float32 {list(shape)} tensor on {dev}")
         d = self.desc
         d.step = step
+        if lr_xyz is not None:
+            for c in self.xyz_columns:
+                d.lr[c] = lr_xyz
         d.unpack.records = records.data_ptr()
         for name in ("means", "covariances", "harmonics", "opacities"):
             setattr(d.unpack, name, getattr(out, name).data_ptr())
@@ -292,18 +307,45 @@ def refine_step(records: Tensor, properties, sh_degree: int, exp_avg: Tensor, ex
     step_fn(records, exp_avg, exp_avg_sq, grads, out, step, records_out=records_out, d_records=d_records)
 
 
+def xyz_lr_at(step: int, lr_xyz: float, lr_xyz_final: float, lr_xyz_steps: int) -> float:
+    """The position rate at `step` (1-based) of 3DGS's exponential decay (get_expon_lr_func with no delay), in
+    float64: exp((1 - u) ln lr_xyz + u ln lr_xyz_final), u = clip(step / lr_xyz_steps, 0, 1)."""
+    u = min(max(step / lr_xyz_steps, 0.0), 1.0)
+    return math.exp((1.0 - u) * math.log(lr_xyz) + u * math.log(lr_xyz_final))
+
+
+def _check_schedule(lr: Optional[dict], lr_xyz_final, lr_xyz_steps) -> None:
+    if lr_xyz_final is None:
+        if lr_xyz_steps is not None:
+            raise ValueError("refine_records: `lr_xyz_steps` needs `lr_xyz_final`")
+        return
+    if isinstance(lr_xyz_final, bool) or not isinstance(lr_xyz_final, (int, float)) \
+            or not (math.isfinite(lr_xyz_final) and lr_xyz_final > 0):
+        raise ValueError(f"refine_records: `lr_xyz_final` must be a finite number > 0, got {lr_xyz_final!r}")
+    if not dict(DEFAULT_LR, **(lr or {}))["xyz"] > 0:
+        raise ValueError("refine_records: the position rate decays only from an xyz rate > 0")
+    if lr_xyz_steps is not None and (isinstance(lr_xyz_steps, bool) or not isinstance(lr_xyz_steps, int)
+                                     or lr_xyz_steps < 1):
+        raise ValueError(f"refine_records: `lr_xyz_steps` must be an int >= 1, got {lr_xyz_steps!r}")
+
+
 def refine_records(records: Tensor, properties, sh_degree: int, *, frame: Optional[ExportFrame] = None,
                    extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor, images: Tensor,
                    background_color: Tensor, steps: int, lr: Optional[dict] = None,
-                   densify: Optional[DensifyConfig] = None) -> RefineResult:
+                   densify: Optional[DensifyConfig] = None, loss: str = "mse", lambda_dssim: float = 0.2,
+                   lr_xyz_final: Optional[float] = None, lr_xyz_steps: Optional[int] = None) -> RefineResult:
     """`steps` Adam steps on `records` (float32 [n, P] on a CUDA device, from `ply_import.read_ply_body` or
-    `ply_export.pack_viewer`, with `properties`) against the MSE of renders of the views (extrinsics [v, 4, 4],
+    `ply_export.pack_viewer`, with `properties`) against a loss of renders of the views (extrinsics [v, 4, 4],
     intrinsics [v, 3, 3], near / far [v], images [v, 3, h, w], background_color [3]) in the world of `frame`.
-    `lr` maps groups (GROUPS) to learning rates over DEFAULT_LR.  With `densify`, 3DGS's densification, pruning and
-    opacity reset run after each step's Adam update as the config schedules them, and the result's `gaussians` holds
-    the count at each loss entry.  The input is not modified; with steps=0 it is returned as it is."""
+    `loss` is "mse" (the fused MSE over the views) or "l1_dssim" (the sum over the views of 3DGS's
+    (1 - lambda_dssim) L1 + lambda_dssim D-SSIM; the result's `mse` then holds the context MSE before and after).
+    `lr` maps groups (GROUPS) to learning rates over DEFAULT_LR.  With `lr_xyz_final`, the position rate at step t is
+    `xyz_lr_at(t, lr["xyz"], lr_xyz_final, lr_xyz_steps or steps)`.  With `densify`, 3DGS's densification, pruning
+    and opacity reset run after each step's Adam update as the config schedules them, and the result's `gaussians`
+    holds the count at each loss entry.  The input is not modified; with steps=0 it is returned as it is."""
     from .decoder import Gaussians
-    from .decoder.cuda_splatting import render_views_mse, render_views_mse_means2d
+    from .decoder.cuda_splatting import render_views, render_views_means2d, render_views_mse, render_views_mse_means2d
+    from .loss import l1_dssim
     from .ply_import import unpack_records
     properties = list(properties)
     if isinstance(steps, bool) or not isinstance(steps, int) or steps < 0:
@@ -311,6 +353,13 @@ def refine_records(records: Tensor, properties, sh_degree: int, *, frame: Option
     column_lr(properties, sh_degree, lr)
     if densify is not None and not isinstance(densify, DensifyConfig):
         raise ValueError(f"refine_records: `densify` must be a DensifyConfig or None, got {densify!r}")
+    if loss not in LOSSES:
+        raise ValueError(f"refine_records: `loss` must be one of {', '.join(LOSSES)}, got {loss!r}")
+    if isinstance(lambda_dssim, bool) or not isinstance(lambda_dssim, (int, float)) or not 0 <= lambda_dssim <= 1:
+        raise ValueError(f"refine_records: `lambda_dssim` must be a number in [0, 1], got {lambda_dssim!r}")
+    _check_schedule(lr, lr_xyz_final, lr_xyz_steps)
+    lr_xyz = dict(DEFAULT_LR, **(lr or {}))["xyz"]
+    decay_steps = steps if lr_xyz_steps is None else lr_xyz_steps
     dev = records.device
     v, _, h, w = images.shape
     views = [t.to(dev, torch.float32)[None] for t in (extrinsics, intrinsics, near, far)]
@@ -326,13 +375,26 @@ def refine_records(records: Tensor, properties, sh_degree: int, *, frame: Option
     leaves, out = gaussians_for(n)
     work = records if steps == 0 else records.clone().contiguous()
     unpack_records(work, properties, sh_degree, frame=frame, out=out)
-    loss = torch.empty(steps + 1, device=dev)
+    losses = torch.empty(steps + 1, device=dev)
     denom = float(v * 3 * h * w)
 
     def mse() -> Tensor:
         sse, _, _ = render_views_mse(*views, (h, w), background, *leaves, target=target, want_color=False)
         return sse.sum() / denom
 
+    def photometric(means2d: Optional[Tensor] = None):
+        """The L1 + D-SSIM objective (the sum over the views) and, with the holder `means2d`, the radii."""
+        if means2d is None:
+            color, radii = render_views(*views, (h, w), background, *leaves), None
+        else:
+            color, radii = render_views_means2d(*views, (h, w), background, *leaves, means2d=means2d)
+        return l1_dssim(color[0], target[0], lambda_dssim).sum(), radii
+
+    dssim = loss == "l1_dssim"
+    mse_before = None
+    if dssim:
+        with torch.no_grad():
+            mse_before = mse()
     m = v2 = None
     counts = None if densify is None else [n]
     if steps:
@@ -347,19 +409,23 @@ def refine_records(records: Tensor, properties, sh_degree: int, *, frame: Option
         for t in range(1, steps + 1):
             if densify is not None and densify.stats_at(t):
                 means2d = torch.zeros((v, n, 3), device=dev, requires_grad=True)
-                sse, _, _, radii = render_views_mse_means2d(*views, (h, w), background, *leaves, target=target,
-                                                            means2d=means2d, want_color=False)
-                value = sse.sum() / denom
+                if dssim:
+                    value, radii = photometric(means2d)
+                else:
+                    sse, _, _, radii = render_views_mse_means2d(*views, (h, w), background, *leaves, target=target,
+                                                                means2d=means2d, want_color=False)
+                    value = sse.sum() / denom
                 value.backward()
                 densify_stats(means2d.grad, radii, accum, seen)
             else:
-                value = mse()
+                value = photometric()[0] if dssim else mse()
                 value.backward()
-            loss[t - 1] = value.detach()
+            losses[t - 1] = value.detach() / v if dssim else value.detach()
             grads = [leaf.grad[0].contiguous() for leaf in leaves]
             for leaf in leaves:
                 leaf.grad = None
-            step_fn(work, m, v2, grads, out, t)
+            step_fn(work, m, v2, grads, out, t,
+                    lr_xyz=None if lr_xyz_final is None else xyz_lr_at(t, lr_xyz, lr_xyz_final, decay_steps))
             if densify is None:
                 continue
             if densify.densifies_at(t):
@@ -378,8 +444,12 @@ def refine_records(records: Tensor, properties, sh_degree: int, *, frame: Option
                     leaf.requires_grad_(True)
             counts.append(n)
     with torch.no_grad():
-        loss[steps] = mse()
-    return RefineResult(work, loss, m, v2, counts)
+        if dssim:
+            losses[steps] = photometric()[0] / v
+            mse_after = mse_before if steps == 0 else mse()
+            return RefineResult(work, losses, m, v2, counts, torch.stack([mse_before, mse_after]))
+        losses[steps] = mse()
+    return RefineResult(work, losses, m, v2, counts)
 
 
 def rewrite_vertex_count(head: bytes, count: int) -> bytes:
@@ -393,7 +463,8 @@ def rewrite_vertex_count(head: bytes, count: int) -> bytes:
 def refine_ply(path: Union[Path, str], frame: Union[ExportFrame, Path, str, None], *, extrinsics: Tensor,
                intrinsics: Tensor, near: Tensor, far: Tensor, images: Tensor, background_color: Tensor, steps: int,
                out_path: Union[Path, str], lr: Optional[dict] = None, device=None,
-               densify: Optional[DensifyConfig] = None) -> Optional[RefineResult]:
+               densify: Optional[DensifyConfig] = None, loss: str = "mse", lambda_dssim: float = 0.2,
+               lr_xyz_final: Optional[float] = None, lr_xyz_steps: Optional[int] = None) -> Optional[RefineResult]:
     """`refine_records` on the file at `path` (in the world of `frame`: an `ExportFrame`, a `<scene>.frame.json`
     path, or None for the file's own frame), written to `out_path` as the input's header bytes followed by the
     refined records: property order, extra properties and comments are kept, and only the `element vertex` count
@@ -413,7 +484,8 @@ def refine_ply(path: Union[Path, str], frame: Union[ExportFrame, Path, str, None
     _, records = read_ply_body(path, device)
     result = refine_records(records, layout.properties, layout.sh_degree, frame=frame, extrinsics=extrinsics,
                             intrinsics=intrinsics, near=near, far=far, images=images,
-                            background_color=background_color, steps=steps, lr=lr, densify=densify)
+                            background_color=background_color, steps=steps, lr=lr, densify=densify, loss=loss,
+                            lambda_dssim=lambda_dssim, lr_xyz_final=lr_xyz_final, lr_xyz_steps=lr_xyz_steps)
     body = result.records.cpu().numpy().astype("<f4", copy=False).tobytes()
     header = head[:layout.body_offset]
     if result.records.shape[0] != layout.count:
