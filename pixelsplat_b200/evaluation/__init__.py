@@ -7,6 +7,8 @@ no float image goes to the host.
 
 - `Evaluator(encoder, decoder, output_path).run(loader)`: ModelWrapper.test_step over a split, with PSNR / SSIM /
   LPIPS per scene and their mean over scenes; `load_checkpoint` reads a pixelSplat `.ckpt` into the encoder.
+  `Evaluator(..., refine={"steps": N, ...})` refines each scene's Gaussians on its context views in memory
+  (`ply_refine.refine_gaussians`) before scoring the targets, and writes refine.json.
 - `compute_metrics(methods, loader)`: MetricComputer over saved frame directories.
 - `frame_metrics`, `frame_pass` and the image_io drop-ins `prep_image`, `save_image`, `load_image`.
 - `generate_index(scenes, h, w, EvaluationIndexGeneratorCfg())`: the reference's evaluation-index generator, with the

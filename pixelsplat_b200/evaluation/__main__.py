@@ -7,6 +7,13 @@ runs the reference's test step over the test split: it prints the PSNR / SSIM / 
 (the paper's numbers) and, with --output, writes the frames (unless --no-frames), benchmark.json,
 peak_memory.json and metrics.json (the mean and each scene's metrics).
 
+With --refine-steps N (N >= 0), each scene's Gaussians are refined in memory on its context views before the targets
+are rendered: the route export-ply --write-frame -> refine-ply --steps N -> render-ply takes through two PLY files
+per scene, with the same frames, metrics and refine.json (written beside metrics.json).  --refine-steps 0 scores the
+export round trip unrefined, the baseline a refined score is compared with.  refine-ply's options (--lr-*,
+--densify-*, --min-opacity, --opacity-reset-every, --loss, --lambda-dssim, --lr-xyz-final, --lr-xyz-steps) apply, and
+only with --refine-steps.  With --preset re10k_3_view the refinement uses all three context views.
+
     python -m pixelsplat_b200.evaluation compute-metrics --dataset-root datasets/re10k \\
         --index assets/evaluation_index_re10k.json --method pixelSplat:ours:outputs/test/re10k \\
         --output-metrics outputs/metrics.json
@@ -71,7 +78,6 @@ lpips package's lin weights from disk (--lpips-vgg / --lpips-lin, or where those
 from __future__ import annotations
 
 import argparse
-import dataclasses
 import json
 import sys
 from pathlib import Path
@@ -129,7 +135,29 @@ def parse_evaluate(argv: list[str]) -> argparse.Namespace:
     p.add_argument("--no-frames", action="store_true", help="write no PNG (metrics and JSON files only)")
     p.add_argument("--global-step", type=int, default=0,
                    help="step given to the encoder (the presets' opacity mapping does not depend on it)")
-    return p.parse_args(argv)
+    p.add_argument("--refine-steps", type=_non_negative(int), default=None,
+                   help="refine each scene's Gaussians on its context views with this many Adam steps before the "
+                        "targets are rendered, in memory, as export-ply --write-frame, refine-ply and render-ply do "
+                        "with files; 0 scores the export round trip unrefined, the baseline (default: off)")
+    options = _add_refine_arguments(p, "--refine-steps")
+    args = p.parse_args(argv)
+    names = ["refine_steps"] + [a.dest for a in options]
+    if args.refine_steps is None:
+        # argparse's own matching (abbreviations, --opt=value) tells which refinement options were given
+        for a in options:
+            a.default = argparse.SUPPRESS
+        given = vars(p.parse_known_args(argv)[0])
+        stray = [a.option_strings[0] for a in options if a.dest in given]
+        if stray:
+            p.error(f"{', '.join(stray)} without --refine-steps: refinement is off unless --refine-steps is given")
+        args.refine = None
+    else:
+        _refine_settings(p, args)
+        args.refine = dict(steps=args.refine_steps, lr=args.lr, densify=args.densify, **_refine_options(args))
+        names += ["lr", "densify"]
+    for name in names:
+        delattr(args, name)
+    return args
 
 
 def evaluate(argv: list[str]) -> dict:
@@ -143,8 +171,11 @@ def evaluate(argv: list[str]) -> dict:
     print(f"Loaded {args.checkpoint} (trained for {step} steps).")
     evaluator = Evaluator(encoder.to(device).eval(), decoder.to(device), args.output, _lpips(args, device),
                           deterministic=args.deterministic, global_step=args.global_step,
-                          write_frames=not args.no_frames)
+                          write_frames=not args.no_frames, refine=args.refine)
     result = evaluator.run(loader, seed=SEED if args.seed is None else args.seed, device=device)
+    if args.refine is not None:
+        for s in result.scenes:
+            print(_refine_line(s.scene, s.refine))
     print(f"{len(result.scenes)} scenes: " + ", ".join(f"{k} {v:.4f}" for k, v in result.mean.items()))
     out = {"mean": result.mean, "scenes": {s.scene: s.metrics for s in result.scenes}}
     if args.output is not None:
@@ -412,52 +443,51 @@ def _unit_interval(text: str) -> float:
     return value
 
 
-def parse_refine_ply(argv: list[str]) -> argparse.Namespace:
+def _add_refine_arguments(p: argparse.ArgumentParser, steps_flag: str) -> list[argparse.Action]:
+    """The refinement options refine-ply and evaluate share: learning rates, densification, loss and the position
+    rate's decay (`steps_flag` is the command's flag for the number of steps).  Returns their actions."""
     from ..ply_refine import DEFAULT_LR, GROUPS, DensifyConfig
-    p = argparse.ArgumentParser(prog="python -m pixelsplat_b200.evaluation refine-ply",
-                                description="Refine exported 3D Gaussian splatting PLY files on each test scene's "
-                                            "context views.")
-    p.add_argument("--ply", type=Path, required=True, help="directory of <scene>.ply and <scene>.frame.json")
-    p.add_argument("--dataset-root", type=Path, required=True, help="dataset root holding test/index.json")
-    p.add_argument("--index", type=Path, required=True, help="evaluation index (scene -> context / target)")
-    p.add_argument("--output", type=Path, required=True,
-                   help="directory of the refined <scene>.ply, <scene>.frame.json and refine.json")
-    p.add_argument("--scene", action="append", default=None, metavar="NAME",
-                   help="refine only this scene (repeatable; default: every index scene)")
-    p.add_argument("--steps", type=_non_negative(int), default=100, help="Adam steps per scene (default: 100)")
-    p.add_argument("--num-workers", type=int, default=4, help="DataLoader workers (the reference's test loader: 4)")
+    actions = []
     for g in GROUPS:
-        p.add_argument(f"--lr-{g.replace('_', '-')}", dest=f"lr_{g}", type=_non_negative(float), default=DEFAULT_LR[g],
-                       help=f"learning rate of the {g} properties (default: 3DGS's {DEFAULT_LR[g]:g})")
+        actions.append(p.add_argument(f"--lr-{g.replace('_', '-')}", dest=f"lr_{g}", type=_non_negative(float),
+                                      default=DEFAULT_LR[g],
+                                      help=f"learning rate of the {g} properties (default: 3DGS's {DEFAULT_LR[g]:g})"))
     d = DensifyConfig()
-    p.add_argument("--densify-until", type=_non_negative(int), default=0,
-                   help="densify, prune and reset opacities before this step, as 3DGS does (default: 0, off; "
-                        f"3DGS: {d.until_step})")
-    p.add_argument("--densify-from", type=_non_negative(int), default=d.from_step,
-                   help=f"densify after this step (default: 3DGS's {d.from_step})")
-    p.add_argument("--densify-every", type=int, default=d.every,
-                   help=f"steps between densifications (default: 3DGS's {d.every})")
-    p.add_argument("--densify-grad", type=_non_negative(float), default=d.grad_threshold,
-                   help=f"mean screen-space gradient norm that selects a Gaussian (default: 3DGS's "
-                        f"{d.grad_threshold:g}, calibrated for its L1 + D-SSIM loss; with --loss mse the gradients "
-                        "are smaller and it has not been tuned)")
-    p.add_argument("--min-opacity", type=_non_negative(float), default=d.min_opacity,
-                   help=f"prune Gaussians below this opacity (default: 3DGS's {d.min_opacity:g})")
-    p.add_argument("--opacity-reset-every", type=_non_negative(int), default=d.opacity_reset_every,
-                   help=f"steps between opacity resets, 0 for none (default: 3DGS's {d.opacity_reset_every})")
-    p.add_argument("--densify-seed", type=_non_negative(int), default=d.seed,
-                   help=f"seed of the split copies' draws (default: {d.seed})")
-    p.add_argument("--loss", choices=("mse", "l1-dssim"), default="mse",
-                   help="mse: the MSE over the context views (default); l1-dssim: 3DGS's (1 - lambda) L1 + lambda "
-                        "D-SSIM, summed over the context views")
-    p.add_argument("--lambda-dssim", type=_unit_interval, default=0.2,
-                   help="D-SSIM weight of --loss l1-dssim (default: 3DGS's 0.2)")
-    p.add_argument("--lr-xyz-final", type=_positive(float), default=None,
-                   help="decay the position rate exponentially from --lr-xyz to this rate (default: off, a constant "
-                        "rate; 3DGS: 1.6e-6)")
-    p.add_argument("--lr-xyz-steps", type=_positive(int), default=None,
-                   help="steps of the position rate's decay (default: --steps; 3DGS: 30000)")
-    args = p.parse_args(argv)
+    actions += [
+        p.add_argument("--densify-until", type=_non_negative(int), default=0,
+                       help="densify, prune and reset opacities before this step, as 3DGS does (default: 0, off; "
+                            f"3DGS: {d.until_step})"),
+        p.add_argument("--densify-from", type=_non_negative(int), default=d.from_step,
+                       help=f"densify after this step (default: 3DGS's {d.from_step})"),
+        p.add_argument("--densify-every", type=int, default=d.every,
+                       help=f"steps between densifications (default: 3DGS's {d.every})"),
+        p.add_argument("--densify-grad", type=_non_negative(float), default=d.grad_threshold,
+                       help=f"mean screen-space gradient norm that selects a Gaussian (default: 3DGS's "
+                            f"{d.grad_threshold:g}, calibrated for its L1 + D-SSIM loss; with --loss mse the "
+                            "gradients are smaller and it has not been tuned)"),
+        p.add_argument("--min-opacity", type=_non_negative(float), default=d.min_opacity,
+                       help=f"prune Gaussians below this opacity (default: 3DGS's {d.min_opacity:g})"),
+        p.add_argument("--opacity-reset-every", type=_non_negative(int), default=d.opacity_reset_every,
+                       help=f"steps between opacity resets, 0 for none (default: 3DGS's {d.opacity_reset_every})"),
+        p.add_argument("--densify-seed", type=_non_negative(int), default=d.seed,
+                       help=f"seed of the split copies' draws (default: {d.seed})"),
+        p.add_argument("--loss", choices=("mse", "l1-dssim"), default="mse",
+                       help="mse: the MSE over the context views (default); l1-dssim: 3DGS's (1 - lambda) L1 + "
+                            "lambda D-SSIM, summed over the context views"),
+        p.add_argument("--lambda-dssim", type=_unit_interval, default=0.2,
+                       help="D-SSIM weight of --loss l1-dssim (default: 3DGS's 0.2)"),
+        p.add_argument("--lr-xyz-final", type=_positive(float), default=None,
+                       help="decay the position rate exponentially from --lr-xyz to this rate (default: off, a "
+                            "constant rate; 3DGS: 1.6e-6)"),
+        p.add_argument("--lr-xyz-steps", type=_positive(int), default=None,
+                       help=f"steps of the position rate's decay (default: {steps_flag}; 3DGS: 30000)")]
+    return actions
+
+
+def _refine_settings(p: argparse.ArgumentParser, args: argparse.Namespace) -> None:
+    """The checks and derived values of `_add_refine_arguments`' options, in place: `loss` as refine_records names
+    it, `lr` (every group's rate) and `densify` (a DensifyConfig, or None with --densify-until 0)."""
+    from ..ply_refine import GROUPS, DensifyConfig
     args.loss = args.loss.replace("-", "_")
     if args.lr_xyz_steps is not None and args.lr_xyz_final is None:
         p.error("--lr-xyz-steps needs --lr-xyz-final")
@@ -473,6 +503,24 @@ def parse_refine_ply(argv: list[str]) -> argparse.Namespace:
                                          seed=args.densify_seed)
         except ValueError as e:
             p.error(str(e))
+
+
+def parse_refine_ply(argv: list[str]) -> argparse.Namespace:
+    p = argparse.ArgumentParser(prog="python -m pixelsplat_b200.evaluation refine-ply",
+                                description="Refine exported 3D Gaussian splatting PLY files on each test scene's "
+                                            "context views.")
+    p.add_argument("--ply", type=Path, required=True, help="directory of <scene>.ply and <scene>.frame.json")
+    p.add_argument("--dataset-root", type=Path, required=True, help="dataset root holding test/index.json")
+    p.add_argument("--index", type=Path, required=True, help="evaluation index (scene -> context / target)")
+    p.add_argument("--output", type=Path, required=True,
+                   help="directory of the refined <scene>.ply, <scene>.frame.json and refine.json")
+    p.add_argument("--scene", action="append", default=None, metavar="NAME",
+                   help="refine only this scene (repeatable; default: every index scene)")
+    p.add_argument("--steps", type=_non_negative(int), default=100, help="Adam steps per scene (default: 100)")
+    p.add_argument("--num-workers", type=int, default=4, help="DataLoader workers (the reference's test loader: 4)")
+    _add_refine_arguments(p, "--steps")
+    args = p.parse_args(argv)
+    _refine_settings(p, args)
     return args
 
 
@@ -483,27 +531,25 @@ def _refine_options(args) -> dict:
 
 
 def _refine_scene_report(args, result) -> dict:
-    """One scene's entry of refine.json: the context MSE before and after (with L1 + D-SSIM from the result's `mse`,
-    beside the mean per-view loss before and after)."""
-    loss = result.loss.tolist()
-    if args.loss == "mse":
-        return {"mse_before": loss[0], "mse_after": loss[-1], "steps": args.steps}
-    mse = result.mse.tolist()
-    return {"mse_before": mse[0], "mse_after": mse[-1], "steps": args.steps, "loss_before": loss[0],
-            "loss_after": loss[-1]}
+    """One scene's entry of refine.json (`ply_refine.scene_report`) for the parsed refinement options."""
+    from ..ply_refine import scene_report
+    return scene_report(result, args.steps, args.loss, args.densify)
 
 
 def _refine_report(args, scenes: dict) -> dict:
-    """refine.json: the settings and each scene's entry; the loss and the decay are recorded only when not off."""
-    out = {"steps": args.steps, "lr": args.lr, "scenes": scenes}
-    if args.densify is not None:
-        out["densify"] = dataclasses.asdict(args.densify)
-    if args.loss != "mse":
-        out.update(loss=args.loss, lambda_dssim=args.lambda_dssim)
-    if args.lr_xyz_final is not None:
-        out.update(lr_xyz_final=args.lr_xyz_final,
-                   lr_xyz_steps=args.steps if args.lr_xyz_steps is None else args.lr_xyz_steps)
-    return out
+    """refine.json (`ply_refine.refine_report`) for the parsed refinement options."""
+    from ..ply_refine import refine_report
+    return refine_report(scenes, args.steps, args.lr, args.densify, **_refine_options(args))
+
+
+def _refine_line(scene: str, r: dict) -> str:
+    """A scene's refine.json entry as one line of output."""
+    line = f"{scene}: context MSE {r['mse_before']:.6f} -> {r['mse_after']:.6f} in {r['steps']} steps"
+    if "loss_before" in r:
+        line += f", L1 + D-SSIM {r['loss_before']:.6f} -> {r['loss_after']:.6f}"
+    if "gaussians_before" in r:
+        line += f", {r['gaussians_before']} -> {r['gaussians_after']} Gaussians"
+    return line
 
 
 def refine_ply(argv: list[str]) -> dict:
@@ -543,17 +589,7 @@ def refine_ply(argv: list[str]) -> dict:
                                     images=ctx["image"][0], background_color=background, steps=0,
                                     **_refine_options(args))
         scenes[scene] = _refine_scene_report(args, result)
-        r = scenes[scene]
-        line = f"{scene}: context MSE {r['mse_before']:.6f} -> {r['mse_after']:.6f} in {args.steps} steps"
-        if args.loss != "mse":
-            line += f", L1 + D-SSIM {r['loss_before']:.6f} -> {r['loss_after']:.6f}"
-        if args.densify is not None:
-            before, after = (result.gaussians[0], result.gaussians[-1]) if result.gaussians else (None, None)
-            if before is None:   # --steps 0: the file is copied
-                before = after = result.records.shape[0]
-            scenes[scene].update(gaussians_before=before, gaussians_after=after)
-            line += f", {before} -> {after} Gaussians"
-        print(line)
+        print(_refine_line(scene, scenes[scene]))
     missing = sorted(wanted - set(scenes)) if wanted is not None else []
     if missing:
         raise SystemExit(f"evaluation refine-ply: no index scene named {', '.join(missing)}")

@@ -75,6 +75,7 @@ class SceneResult:
     metrics: dict[str, float]            # the scene's mean of each metric over its targets
     per_view: dict[str, Tensor]          # float32 [v] per metric
     frames: Optional[Tensor] = None      # uint8 [v, h, w, 3] on the device, the bytes written as PNGs
+    refine: Optional[dict] = None        # the scene's refine.json entry (ply_refine.scene_report), or None
 
 
 @dataclass
@@ -93,11 +94,18 @@ def mean_over_scenes(per_scene: Iterable[dict[str, float]]) -> dict[str, float]:
 
 class Evaluator:
     """Runs `encoder` (an EncoderEpipolar with its weights loaded) and `decoder` (DecoderSplattingCUDA) over a test
-    split.  `lpips` is an `Lpips` module (default: `Lpips.from_files()`); `output_path` None writes no file."""
+    split.  `lpips` is an `Lpips` module (default: `Lpips.from_files()`); `output_path` None writes no file.
+
+    `refine`, when given, is {"steps": N} with any of `ply_refine.refine_records`' options (ply_refine.OPTIONS): each
+    scene's Gaussians are then refined on its context views (`ply_refine.refine_gaussians`) before its targets are
+    rendered, as export-ply --write-frame, refine-ply and render-ply do through files, and `run` writes refine.json.
+    Refinement and target renders take the device shim's views, as those commands do; only the encoder sees the
+    data shim's (whose bounds shim replaces near / far)."""
 
     def __init__(self, encoder: nn.Module, decoder: nn.Module, output_path: Path | str | None = None,
                  lpips: nn.Module | None = None, deterministic: bool = False, global_step: int = 0,
-                 write_frames: bool = True) -> None:
+                 write_frames: bool = True, refine: Optional[dict] = None) -> None:
+        from ..ply_refine import OPTIONS, check_refine_options
         self.encoder = encoder
         self.decoder = decoder
         self.output_path = None if output_path is None else Path(output_path)
@@ -105,13 +113,21 @@ class Evaluator:
         self.deterministic = deterministic
         self.global_step = global_step
         self.write_frames = write_frames
+        if refine is not None:
+            if "steps" not in refine:
+                raise ValueError(f"Evaluator: `refine` must hold 'steps' and any of {', '.join(OPTIONS)}; got "
+                                 f"{sorted(refine)}")
+            check_refine_options(**refine)
+        self.refine = None if refine is None else dict(refine)
         self.data_shim = encoder.get_data_shim()
         self.benchmarker = Benchmarker()
 
     @torch.no_grad()
     def test_step(self, batch: dict) -> SceneResult:
         """One scene of a device-resident test batch (what `device_shim` returns): render, quantise, score and
-        optionally write its frames."""
+        optionally write its frames.  With refinement, the encoder's Gaussians are refined on the context views and
+        the targets rendered from them, both with the device shim's views and cameras."""
+        views = batch
         shape_in = tuple(batch["target"]["image"].shape)
         batch = self.data_shim(batch)
         b, v, _, h, w = batch["target"]["image"].shape
@@ -124,6 +140,10 @@ class Evaluator:
         tgt = batch["target"]
         with self.benchmarker.time("encoder"):
             gaussians = self.encoder(batch["context"], self.global_step, deterministic=self.deterministic)
+        refined = None
+        if self.refine is not None:
+            gaussians, refined = self._refine(gaussians, views["context"])
+            tgt = views["target"]
         with self.benchmarker.time("decoder", num_calls=v):
             color = torch.cat([self.decoder.forward(gaussians, tgt["extrinsics"][:1, i:i + CHUNK],
                                                     tgt["intrinsics"][:1, i:i + CHUNK], tgt["near"][:1, i:i + CHUNK],
@@ -133,7 +153,7 @@ class Evaluator:
         frames = per_view.pop("frames")
         (scene,) = batch["scene"]
         result = SceneResult(scene, [int(i) for i in batch["context"]["index"][0]], [int(i) for i in tgt["index"][0]],
-                             {k: float(per_view[k].mean()) for k in METRICS}, per_view, frames)
+                             {k: float(per_view[k].mean()) for k in METRICS}, per_view, frames, refined)
         if self.output_path is not None and self.write_frames:
             root = self.output_path / scene
             for index, frame in zip(result.target_index, frames.cpu().numpy()):
@@ -142,6 +162,19 @@ class Evaluator:
                 save_frame(frame, root / "context" / f"{index:0>6}.png")
         self.benchmarker.collect()
         return result
+
+    def _refine(self, gaussians, context: dict):
+        """`ply_refine.refine_gaussians` on the scene's context views, timed as "refine" (pack, refine and unpack)
+        -> (the refined Gaussians, the scene's refine.json entry)."""
+        from ..ply_refine import refine_gaussians, scene_report
+        options = {k: v for k, v in self.refine.items() if k != "steps"}
+        steps = self.refine["steps"]
+        with self.benchmarker.time("refine"):
+            gaussians, result = refine_gaussians(
+                gaussians, context["extrinsics"][0, 0], context_extrinsics=context["extrinsics"][0],
+                intrinsics=context["intrinsics"][0], near=context["near"][0], far=context["far"][0],
+                images=context["image"][0], background_color=self.decoder.background_color, steps=steps, **options)
+        return gaussians, scene_report(result, steps, options.get("loss", "mse"), options.get("densify"))
 
     def run(self, loader: Iterable[dict], image_shape: tuple[int, int] = (256, 256), seed: int = 111123,
             device: torch.device | str | None = None, keep_frames: bool = False, log=print) -> EvaluationResult:
@@ -163,4 +196,8 @@ class Evaluator:
         if self.output_path is not None:
             self.benchmarker.dump(self.output_path / "benchmark.json")
             self.benchmarker.dump_memory(self.output_path / "peak_memory.json", device)
+            if self.refine is not None:
+                from ..ply_refine import refine_report
+                report = refine_report({s.scene: s.refine for s in scenes}, **self.refine)
+                (self.output_path / "refine.json").write_text(json.dumps(report, indent=1) + "\n")
         return result

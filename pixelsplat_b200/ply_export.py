@@ -78,8 +78,10 @@ def sh_transform(frame: Tensor, degree: int, basis) -> Tensor:
 
 
 def normalisation(means: Tensor) -> tuple[Tensor, Tensor]:
-    """(median of the means [3], s [1]) on the means' device, as the reference computes them."""
-    center = means.median(dim=0).values
+    """(median of the means [3], s [1]) on the means' device, as the reference computes them.  The median is the
+    lower-interpolated 0.5 quantile: the element torch.median(dim=0) returns, NaN propagation included, without
+    its indices, which CUDA cannot compute under torch.use_deterministic_algorithms."""
+    center = means.quantile(0.5, dim=0, interpolation="lower")
     scale = (means - center).abs().quantile(0.95, dim=0).max().reshape(1)
     return center.contiguous(), scale
 

@@ -24,12 +24,16 @@ are clamped to logit(0.01).  The scene extent is 1 in a viewer-format export's u
 3DGS's 2e-4, which was calibrated for its L1 + D-SSIM loss: with `loss="l1_dssim"` each view's statistic is the
 quantity it was calibrated on; with the fused MSE over all context views the gradients are smaller, and the threshold
 has not been tuned for that loss.
+
+`refine_gaussians` refines one scene's encoder Gaussians in memory: the export, the refinement and the import that
+`export-ply --write-frame`, `refine-ply` and `render-ply` chain through files, with the same bits.  `scene_report` and
+`refine_report` build refine.json for both routes.
 """
 from __future__ import annotations
 
 import ctypes
 import math
-from dataclasses import dataclass
+from dataclasses import asdict, dataclass
 from pathlib import Path
 from typing import Optional, Union
 
@@ -329,6 +333,20 @@ def _check_schedule(lr: Optional[dict], lr_xyz_final, lr_xyz_steps) -> None:
         raise ValueError(f"refine_records: `lr_xyz_steps` must be an int >= 1, got {lr_xyz_steps!r}")
 
 
+def _check_options(steps, lr: Optional[dict], densify, loss, lambda_dssim, lr_xyz_final, lr_xyz_steps) -> None:
+    """What `refine_records` refuses in its arguments, checked on the host before any launch."""
+    if isinstance(steps, bool) or not isinstance(steps, int) or steps < 0:
+        raise ValueError(f"refine_records: `steps` must be an int >= 0, got {steps!r}")
+    column_lr((), 0, lr)
+    if densify is not None and not isinstance(densify, DensifyConfig):
+        raise ValueError(f"refine_records: `densify` must be a DensifyConfig or None, got {densify!r}")
+    if loss not in LOSSES:
+        raise ValueError(f"refine_records: `loss` must be one of {', '.join(LOSSES)}, got {loss!r}")
+    if isinstance(lambda_dssim, bool) or not isinstance(lambda_dssim, (int, float)) or not 0 <= lambda_dssim <= 1:
+        raise ValueError(f"refine_records: `lambda_dssim` must be a number in [0, 1], got {lambda_dssim!r}")
+    _check_schedule(lr, lr_xyz_final, lr_xyz_steps)
+
+
 def refine_records(records: Tensor, properties, sh_degree: int, *, frame: Optional[ExportFrame] = None,
                    extrinsics: Tensor, intrinsics: Tensor, near: Tensor, far: Tensor, images: Tensor,
                    background_color: Tensor, steps: int, lr: Optional[dict] = None,
@@ -348,16 +366,7 @@ def refine_records(records: Tensor, properties, sh_degree: int, *, frame: Option
     from .loss import l1_dssim
     from .ply_import import unpack_records
     properties = list(properties)
-    if isinstance(steps, bool) or not isinstance(steps, int) or steps < 0:
-        raise ValueError(f"refine_records: `steps` must be an int >= 0, got {steps!r}")
-    column_lr(properties, sh_degree, lr)
-    if densify is not None and not isinstance(densify, DensifyConfig):
-        raise ValueError(f"refine_records: `densify` must be a DensifyConfig or None, got {densify!r}")
-    if loss not in LOSSES:
-        raise ValueError(f"refine_records: `loss` must be one of {', '.join(LOSSES)}, got {loss!r}")
-    if isinstance(lambda_dssim, bool) or not isinstance(lambda_dssim, (int, float)) or not 0 <= lambda_dssim <= 1:
-        raise ValueError(f"refine_records: `lambda_dssim` must be a number in [0, 1], got {lambda_dssim!r}")
-    _check_schedule(lr, lr_xyz_final, lr_xyz_steps)
+    _check_options(steps, lr, densify, loss, lambda_dssim, lr_xyz_final, lr_xyz_steps)
     lr_xyz = dict(DEFAULT_LR, **(lr or {}))["xyz"]
     decay_steps = steps if lr_xyz_steps is None else lr_xyz_steps
     dev = records.device
@@ -450,6 +459,83 @@ def refine_records(records: Tensor, properties, sh_degree: int, *, frame: Option
             return RefineResult(work, losses, m, v2, counts, torch.stack([mse_before, mse_after]))
         losses[steps] = mse()
     return RefineResult(work, losses, m, v2, counts)
+
+
+OPTIONS = ("lr", "densify", "loss", "lambda_dssim", "lr_xyz_final", "lr_xyz_steps")   # refine_records' options
+
+
+def check_refine_options(steps, **options) -> None:
+    """Refuses, on the host, what `refine_records` would refuse in `steps` and its `options` (OPTIONS), and any
+    other option."""
+    unknown = sorted(set(options) - set(OPTIONS))
+    if unknown:
+        raise ValueError(f"refine: unknown option {', '.join(unknown)}; the options are {', '.join(OPTIONS)}")
+    _check_options(steps, options.get("lr"), options.get("densify"), options.get("loss", "mse"),
+                   options.get("lambda_dssim", 0.2), options.get("lr_xyz_final"), options.get("lr_xyz_steps"))
+
+
+def refine_gaussians(gaussians, extrinsics: Tensor, *, context_extrinsics: Tensor, intrinsics: Tensor, near: Tensor,
+                     far: Tensor, images: Tensor, background_color: Tensor, steps: int, **options):
+    """One scene's Gaussians as the encoder returns them (batch 1), refined in memory as `export-ply --write-frame`,
+    `refine-ply` and `render-ply` refine and load them from files: `ply_export.pack_viewer` at its default degree
+    with context view 0's pose `extrinsics` [4, 4], `refine_records` in the world of
+    `ply_export.export_frame(means, extrinsics)` against the context views (context_extrinsics [v, 4, 4],
+    intrinsics [v, 3, 3], near / far [v], images [v, 3, h, w]), and `ply_import.unpack_records` with the file's
+    (d + 1)^2 coefficients.  `options` are refine_records' (OPTIONS).  -> (batch-1 `Gaussians` for the decoder,
+    the `RefineResult`); with steps=0, the export round trip alone and the context loss once.  Runs with autograd
+    on whatever the caller's grad mode; refuses bad arguments before any launch."""
+    from .decoder import Gaussians
+    from .ply_export import export_frame, pack_viewer
+    from .ply_import import unpack_records
+    check_refine_options(steps, **options)
+    means = getattr(gaussians, "means", None)
+    if not isinstance(means, Tensor) or means.dim() != 3 or means.shape[0] != 1:
+        shape = list(means.shape) if isinstance(means, Tensor) else None
+        raise ValueError(f"refine_gaussians: `gaussians` must hold one scene with a batch dimension of 1 (means "
+                         f"[1, n, 3]), got means of shape {shape}")
+    records, properties = pack_viewer(gaussians, extrinsics)
+    frame = export_frame(means[0], extrinsics)
+    sh_degree = math.isqrt(sum(p.startswith("f_rest_") for p in properties) // 3 + 1) - 1
+    with torch.enable_grad():
+        result = refine_records(records, properties, sh_degree, frame=frame, extrinsics=context_extrinsics,
+                                intrinsics=intrinsics, near=near, far=far, images=images,
+                                background_color=background_color, steps=steps, **options)
+    g = unpack_records(result.records, properties, sh_degree, frame=frame)
+    return Gaussians(*(t[None] for t in (g.means, g.covariances, g.harmonics, g.opacities))), result
+
+
+def scene_report(result: RefineResult, steps: int, loss: str = "mse",
+                 densify: Optional[DensifyConfig] = None) -> dict:
+    """One scene's entry of refine.json: the context MSE before and after and the steps; with L1 + D-SSIM also the
+    mean per-view loss before and after (the MSE then comes from the result's `mse`); with densification the
+    Gaussian count before and after (the records' count when the result kept no counts)."""
+    history = result.loss.tolist()
+    if loss == "mse":
+        out = {"mse_before": history[0], "mse_after": history[-1], "steps": steps}
+    else:
+        mse = result.mse.tolist()
+        out = {"mse_before": mse[0], "mse_after": mse[-1], "steps": steps, "loss_before": history[0],
+               "loss_after": history[-1]}
+    if densify is not None:
+        before, after = (result.gaussians[0], result.gaussians[-1]) if result.gaussians else \
+            (result.records.shape[0],) * 2
+        out.update(gaussians_before=before, gaussians_after=after)
+    return out
+
+
+def refine_report(scenes: dict, steps: int, lr: Optional[dict] = None, densify: Optional[DensifyConfig] = None,
+                  loss: str = "mse", lambda_dssim: float = 0.2, lr_xyz_final: Optional[float] = None,
+                  lr_xyz_steps: Optional[int] = None) -> dict:
+    """refine.json: the settings (every group's rate) and each scene's entry (`scene_report`); the densification,
+    the loss and the decay are recorded only when not off."""
+    out = {"steps": steps, "lr": dict(DEFAULT_LR, **(lr or {})), "scenes": scenes}
+    if densify is not None:
+        out["densify"] = asdict(densify)
+    if loss != "mse":
+        out.update(loss=loss, lambda_dssim=lambda_dssim)
+    if lr_xyz_final is not None:
+        out.update(lr_xyz_final=lr_xyz_final, lr_xyz_steps=steps if lr_xyz_steps is None else lr_xyz_steps)
+    return out
 
 
 def rewrite_vertex_count(head: bytes, count: int) -> bytes:
