@@ -154,6 +154,10 @@ typedef struct ps_raster_layout {
     size_t run_hits;      /* binning: u32 [S*V*tiles*8*4] their lengths                                        */
     size_t run_state;     /* image: f32x4 [S*V*3*H*W] (T, Cr, Cg, Cb) in front of list runs 1..3 when the
                              compositor cuts a tile's list into runs (small batches)            */
+    size_t sh_jacobian;   /* geom: f32x4 [S*V*P][3] per on-screen (view, Gaussian) pair, row c = the gradient of
+                             colour channel c before the clamp with respect to the normalised view direction
+                             (x, y, z, unused); written by the forward, read by the backward.  0 and not
+                             allocated when sh_coeffs == 0.  (The depth fields stay last.)                     */
     /* appended with depth_mode (both 0 and not allocated when depth_mode == 0) */
     size_t depth_image;   /* image: f32 [S*V*H*W] the composited depth channel                                  */
     size_t run_depth;     /* image: f32 [S*V*3*H*W] depth in front of list runs 1..3 (next to run_state)        */
@@ -172,8 +176,8 @@ typedef struct ps_raster_layout {
  * `workspace` (16-byte aligned, no initialisation) has ps_raster_camera_workspace_bytes: the preprocess backward
  * stores one partial sum per (warp of 32 Gaussians, view) there and a finish kernel adds them in a fixed order.
  * Camera-only backward: with `camera` set, d_means, d_cov, d_opacities, d_sh and d_means2d may ALL be NULL.  The call
- * then writes the camera gradients and nothing else (no Gaussian gradient is formed; the SH rows are read only for
- * the campos term of on-screen Gaussians).  Its camera gradients are the full backward's (the same per-Gaussian terms
+ * then writes the camera gradients and nothing else (no Gaussian gradient is formed; for the campos term the forward's
+ * colour-direction Jacobian, ps_raster_layout.sh_jacobian, is read instead of the SH rows).  Its camera gradients are the full backward's (the same per-Gaussian terms
  * summed in the same order; the compiler may round the campos term differently), and it takes the same scratch and
  * workspace sizes and the same number of launches.  Some but not all of the four required Gaussian pointers NULL, or all five
  * NULL without `camera`, is PS_ERR_INVALID_ARGUMENT before anything is enqueued. */

@@ -57,7 +57,8 @@ class RasterLayout(ctypes.Structure):
     _fields_ = [(n, ctypes.c_size_t) for n in (
         "depth", "radii", "xy", "conic_opacity", "rgb", "rect", "clamped", "tile_count",
         "tile_start", "tile_cursor", "n_instances", "vis_pairs", "vis_any", "keys", "keys_alt", "final_T",
-        "n_contrib", "cull", "color", "block_hits", "run_hits", "run_state", "depth_image", "run_depth")]
+        "n_contrib", "cull", "color", "block_hits", "run_hits", "run_state", "sh_jacobian",
+        "depth_image", "run_depth")]
 
 
 class EpipolarDesc(ctypes.Structure):

@@ -25,6 +25,7 @@ struct Geom {
     long long *n_instances;   // [0] instances, [1] longest segment, [2] #vis_pairs, [3] unused (0)
     uint32_t *vis_pairs;      // compact list of (view, Gaussian) flat indices that are on screen
     float4 *cull;             // xy + half-extents of the alpha >= 1/255 box (compositor's cull record)
+    float4 *sh_jac;           // [S*V*P][3] (M > 0, else null): d(colour channel before the clamp) / d(direction)
 };
 
 // Per-view image-space state kept from forward to backward.

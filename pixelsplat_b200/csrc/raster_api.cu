@@ -164,6 +164,7 @@ static Layout make_layout(const ps_raster_desc *d) {
     L.off.vis_pairs = take(vp * 4);
     L.off.vis_any = take((size_t)m.S * m.P * 4);   // unused; kept so that the ABI layout does not change
     L.off.cull = take(vp * 16);
+    L.off.sh_jacobian = m.M > 0 ? take(vp * 48) : 0;
     L.sizes.geom_bytes = o;
     o = 0;
     L.off.keys = take((size_t)m.capacity * 8);
@@ -221,6 +222,7 @@ static Geom make_geom(const Layout &L, void *geom) {
     g.n_instances = reinterpret_cast<long long *>(b + L.off.n_instances);
     g.vis_pairs = reinterpret_cast<uint32_t *>(b + L.off.vis_pairs);
     g.cull = reinterpret_cast<float4 *>(b + L.off.cull);
+    g.sh_jac = L.off.sh_jacobian ? reinterpret_cast<float4 *>(b + L.off.sh_jacobian) : nullptr;
     return g;
 }
 

@@ -189,17 +189,11 @@ __device__ __forceinline__ void gather_rows_wait() {
     __syncwarp();
 }
 
-// The inverse for consecutive rows: the warp's first `rows` staged rows go to dst[0 .. rows * sh_n) as one
-// contiguous, coalesced block (element e of it is column e % sh_n of staged row e / sh_n).
-__device__ __forceinline__ void store_rows(float *__restrict__ dst, int rows, int sh_n, const float *wrows,
-                                           int row_stride, int lane) {
-    const int dr = 32 / sh_n, dc = 32 - dr * sh_n;
-    int r = lane / sh_n, c = lane - r * sh_n;
-    for (int e = lane; e < rows * sh_n; e += 32) {
-        dst[e] = wrows[r * row_stride + c];
-        r += dr; c += dc;
-        if (c >= sh_n) { c -= sh_n; ++r; }
-    }
+// Zeros dst[0 .. n) with the warp: 16-byte stores where dst is 16-byte aligned.
+__device__ __forceinline__ void zero_fill_warp(float *__restrict__ dst, int n, int lane) {
+    const int nvec = (reinterpret_cast<uintptr_t>(dst) & 15) == 0 ? n >> 2 : 0;
+    for (int i = lane; i < nvec; i += 32) reinterpret_cast<float4 *>(dst)[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    for (int e = 4 * nvec + lane; e < n; e += 32) dst[e] = 0.0f;
 }
 
 __device__ __forceinline__ int sh_index(int layout, int M, int k, int ch) {

@@ -149,7 +149,9 @@ k_preprocess(Dims d, Inputs in, Geom geo, int use_smem_hist) {
 
 // SH -> RGB for the on-screen (view, Gaussian) pairs only, one thread per pair (dense warps).
 // The warp first copies its 32 (scattered) 3M-float rows into shared memory with coalesced
-// row-wise loads, then every lane evaluates its own row.
+// row-wise loads, then every lane evaluates its own row.  Beside the colour it stores the pair's
+// colour-direction Jacobian (geo.sh_jac, three float4 rows): the only use the backward has for
+// the coefficients, so k_preprocess_bwd and k_camera_bwd never read an SH row.
 constexpr int kShThreads = 128;
 
 __global__ void __launch_bounds__(kShThreads)
@@ -180,17 +182,34 @@ k_sh_color(Dims d, Inputs in, Geom geo, int row_stride) {
     if (!live) return;
     const float *row = wrows + lane * row_stride;
     float acc[3] = {0.0f, 0.0f, 0.0f};
+    // d acc[ch] / d(sh_arg's a, b, c), the sign of odd-k terms on the coefficient.  Explicit FMAs: this file is
+    // built without contraction for the colour's sake, and the Jacobian need not match any other rounding (both
+    // backward kernels read this one record).  Term 0 is a constant and has no derivative.
+    float jac[3][3] = {{0.0f, 0.0f, 0.0f}, {0.0f, 0.0f, 0.0f}, {0.0f, 0.0f, 0.0f}};
     const int M = d.M, layout = d.sh_layout;
     const float3 sa = sh_arg(d.sh_basis, x, y, z);
     const uint32_t flip = sh_flip_mask(d.sh_basis);
-    sh_for_each(d.deg, sa.x, sa.y, sa.z, [&](int k, float Yk, float, float, float) {
+    sh_for_each(d.deg, sa.x, sa.y, sa.z, [&](int k, float Yk, float Ya, float Yb, float Yc) {
         const float Y = sh_sign(flip, k, Yk);
 #pragma unroll
         for (int ch = 0; ch < 3; ++ch) {
             const float c = row[sh_index(layout, M, k, ch)];
             acc[ch] = k == 0 ? Y * c : acc[ch] + Y * c;
+            if (k != 0) {
+                const float cs = sh_sign(flip, k, c);
+                jac[ch][0] = __fmaf_rn(Ya, cs, jac[ch][0]);
+                jac[ch][1] = __fmaf_rn(Yb, cs, jac[ch][1]);
+                jac[ch][2] = __fmaf_rn(Yc, cs, jac[ch][2]);
+            }
         }
     });
+    // the backward's dL/d(direction) is sum_ch dL/dcolour[ch] jac[ch], in the direction's own (x, y, z) order
+    float4 *jrec = geo.sh_jac + 3 * (size_t)vg;
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) {
+        const float3 j = sh_grad_unpermute(d.sh_basis, jac[ch][0], jac[ch][1], jac[ch][2]);
+        jrec[ch] = make_float4(j.x, j.y, j.z, 0.0f);
+    }
     float rgb[3];
     uint8_t clamp_bits = 0;
 #pragma unroll

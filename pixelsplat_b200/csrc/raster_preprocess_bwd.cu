@@ -59,9 +59,17 @@ __device__ __forceinline__ void store_cam_partials(const float (&cam)[kCamEntrie
 // The gradient math of one on-screen (view, Gaussian) pair, shared by k_preprocess_bwd and k_camera_bwd so that the
 // camera gradients of both come out of the same expressions.  The statement order is the one the kernels were tuned
 // with (the dcov sums inside the denom2inv branch, then dM, dJ, dL/dt, g, then the perspective terms): computing all
-// of dM, dJ and dL/dt before the dcov sums makes k_preprocess_bwd<false, false> spill.  The SH walk that forms
-// dL/d(direction) for the campos entries stays written out in each kernel: moved into a shared function or visitor,
-// it changed the register allocation and instruction count of every k_preprocess_bwd instantiation.
+// of dM, dJ and dL/dt before the dcov sums makes k_preprocess_bwd<false, false> spill.
+
+// dL/d(normalised view direction) of a pair: its colour-direction Jacobian (k_sh_color's geo.sh_jac record, one
+// float4 row per channel) contracted with dL/dcolour, `dl` already masked by the clamp bits.  Explicit roundings, so
+// that k_preprocess_bwd and k_camera_bwd form the same bits whatever the compiler contracts around them.
+__device__ __forceinline__ float3 sh_direction_grad(const float4 *__restrict__ jrec, const float (&dl)[3]) {
+    const float4 j0 = jrec[0], j1 = jrec[1], j2 = jrec[2];
+    return make_float3(__fmaf_rn(dl[2], j2.x, __fmaf_rn(dl[1], j1.x, __fmul_rn(dl[0], j0.x))),
+                       __fmaf_rn(dl[2], j2.y, __fmaf_rn(dl[1], j1.y, __fmul_rn(dl[0], j0.y))),
+                       __fmaf_rn(dl[2], j2.z, __fmaf_rn(dl[1], j1.z, __fmul_rn(dl[0], j0.z))));
+}
 
 // What the projection backward of a pair leaves for its callers: dL/dM (rows of M = J W), dL/dJ, the view-space
 // gradient dL/dt, the perspective-divide terms, and the pair's gradient (gx, gy, gz) with respect to the scaled mean.
@@ -163,7 +171,7 @@ __device__ __forceinline__ void camera_geometry_grads(const PairGrad &q, const C
 }
 
 // campos entries [24..26]: minus the gradient of the view direction p - campos (dd = p - campos, len2 = |dd|^2,
-// inv3 = 1 / |dd|^3, dLd = dL/d(normalised direction) from the SH walk).  Rounded intrinsics: plain products shared
+// inv3 = 1 / |dd|^3, dLd = dL/d(normalised direction) from sh_direction_grad).  Rounded intrinsics: plain products shared
 // with the Gaussian's own direction chain in k_preprocess_bwd would change how that is contracted, and the Gaussian
 // gradients must keep their bits.
 __device__ __forceinline__ void camera_campos_grads(float ddx, float ddy, float ddz, float len2, float inv3,
@@ -187,19 +195,21 @@ __device__ __forceinline__ void camera_depth_grads(float dz, float mx0, float my
 // output gradient, which the caller may hand over uninitialised: a Gaussian that is on screen in no view gets zeros,
 // and so does every Gaussian when the binning overflowed its capacity (the composite backward then did not run).  A
 // warp none of whose Gaussians is on screen only stores zeros.  On screen in view v means radii > 0, the rows
-// k_clear_pair_grads cleared and the composite backward accumulated into.  SH rows are staged per warp in shared
-// memory: the coefficients of the on-screen lanes come in with cp.async, dL/dSH of all 32 rows goes out as one
-// contiguous block.
-// DEPTH: the depth value's chain to the means is added (a depth gradient was given); built for 4 resident CTAs so
-// that it does not spill.
+// k_clear_pair_grads cleared and the composite backward accumulated into.  dL/dSH rows are staged per warp in shared
+// memory and go out as one contiguous block of all 32 rows.  No SH coefficient is read: dL/dSH needs only the basis,
+// and the direction's gradient comes from the Jacobian k_sh_color stored for the pair.
+// DEPTH: the depth value's chain to the means is added (a depth gradient was given).
 // CAM: camera gradients are requested.  Each lane also forms its Gaussian's contribution to the kCamEntries camera
 // entries of every view it is on screen in; the warp sums them per (scene, view) in a fixed shuffle order and
 // stores one partial row per (warp, view) into `cam_ws` (layout: cam_row), zeros included, which k_camera_finish
-// sums.  Built for 2 resident CTAs: the 29 partial sums are live beside the colour chain.
+// sums.
+// Residency: 38.4 KB of gradient rows per CTA at M = 25 allow 5 CTAs per SM, for any V; 5 is also the register bound
+// without CAM.  CAM is built for 3: the 29 partial sums are live beside the colour chain, and at 4 (128 registers)
+// it spills.  No instantiation spills (DESIGN.md section 5).
 template <bool DEPTH, bool CAM>
-__global__ void __launch_bounds__(kPreBwdThreads, CAM ? 2 : (DEPTH ? 4 : 5))
+__global__ void __launch_bounds__(kPreBwdThreads, CAM ? 3 : 5)
 k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int row_stride, float *cam_ws) {
-    extern __shared__ float s_dsh[];   // [warps][32][row_stride] coefficients (V == 1: reused for the gradient)
+    extern __shared__ float s_dsh[];   // [warps][32][row_stride] dL/dSH rows
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const long long sp = (long long)d.S * d.P;
     const long long sg0 = ((long long)blockIdx.x * kPreBwdThreads) + warp * 32;
@@ -218,10 +228,10 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int
         for (int v = 0; v < d.V; ++v) any |= geo.radii[(size_t)((int)scene * d.V + v) * d.P + g] > 0;
     const unsigned vis_lanes = __ballot_sync(0xffffffffu, any);
     if (vis_lanes == 0u) {
-        for (int e = lane; e < rows * 3; e += 32) out.d_means[3 * sg0 + e] = 0.0f;
-        for (int e = lane; e < rows * cov_n; e += 32) out.d_cov[cov_n * sg0 + e] = 0.0f;
+        zero_fill_warp(out.d_means + 3 * sg0, rows * 3, lane);
+        zero_fill_warp(out.d_cov + cov_n * sg0, rows * cov_n, lane);
         if (lane < rows) out.d_opacities[sg0 + lane] = 0.0f;
-        for (int e = lane; e < rows * sh_n; e += 32) out.d_sh[sh_n * sg0 + e] = 0.0f;
+        zero_fill_warp(out.d_sh + sh_n * sg0, rows * sh_n, lane);
         if (out.d_means2d && live)
             for (int v = 0; v < d.V; ++v) {
                 float *m2 = out.d_means2d + 3 * ((size_t)((int)scene * d.V + v) * d.P + g);
@@ -236,12 +246,7 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int
     }
 
     float *wrows = s_dsh + (size_t)warp * 32 * row_stride;
-    float *row = wrows + lane * row_stride;
-    const bool in_place = M > 0 && d.V == 1;     // read each coefficient, then overwrite its slot with the gradient
-    float *grow = in_place ? row : row + (size_t)kPreBwdThreads * row_stride;   // separate gradient rows when V > 1
-
-    // the SH rows stream into shared memory while the geometry part below runs; waited for at first use
-    if (M > 0) gather_rows_async(in.sh, (unsigned long long)sg, vis_lanes, sh_n, wrows, row_stride, lane);
+    float *grow = wrows + lane * row_stride;
 
     float mx0 = 0.0f, my0 = 0.0f, mz0 = 0.0f;
     if (any) { mx0 = in.means[3 * sg + 0]; my0 = in.means[3 * sg + 1]; mz0 = in.means[3 * sg + 2]; }
@@ -250,7 +255,7 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int
     float dmx = 0.0f, dmy = 0.0f, dmz = 0.0f, dop = 0.0f;
     float dcov[6] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
     float dcol[3] = {0.0f, 0.0f, 0.0f};
-    bool sh_written = false, sh_ready = false;
+    bool sh_written = false;
 
     for (int v = 0; v < d.V; ++v) {
         const int vid = (int)scene * d.V + v;
@@ -262,7 +267,7 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int
             m2[0] = t.x; m2[1] = t.y; m2[2] = 0.0f;
         }
         // (no `continue` for the views this Gaussian is not on screen in: the warp must stay convergent for the
-        //  shared-memory hand-over of the SH rows below)
+        //  camera partial sums' shuffles below)
         float gx = 0.0f, gy = 0.0f, gz = 0.0f;
         float4 gcol = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
         float cam[CAM ? kCamEntries : 1];   // this Gaussian's share of the view's camera gradient (cam_row order)
@@ -292,10 +297,6 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int
         if constexpr (CAM) camera_geometry_grads(q, cv, px, py, pz, g2, focal_x, focal_y, tanfovx, tanfovy, cam);
         }   // vis (geometry part)
 
-        if (M > 0 && !sh_ready) {          // warp-uniform; the rows have had the geometry math to arrive
-            gather_rows_wait();
-            sh_ready = true;
-        }
         if (M > 0 && vis) {
             const float cx = in.campos[3 * vid], cy = in.campos[3 * vid + 1], cz = in.campos[3 * vid + 2];
             const float ddx = px - cx, ddy = py - cy, ddz = pz - cz;
@@ -304,23 +305,18 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int
             const float x = ddx / len, y = ddy / len, z = ddz / len;
             const uint8_t cl = geo.clamped[vg];
             const float dl[3] = {(cl & 1) ? 0.0f : gcol.x, (cl & 2) ? 0.0f : gcol.y, (cl & 4) ? 0.0f : gcol.z};
-            float dLda = 0.0f, dLdb = 0.0f, dLdc = 0.0f;
             const bool first = !sh_written;
             const float3 sa = sh_arg(d.sh_basis, x, y, z);
             const uint32_t flip = sh_flip_mask(d.sh_basis);
-            sh_for_each(d.deg, sa.x, sa.y, sa.z, [&](int k, float Y, float Ya, float Yb, float Yc) {
+            sh_for_each(d.deg, sa.x, sa.y, sa.z, [&](int k, float Y, float, float, float) {
 #pragma unroll
                 for (int ch = 0; ch < 3; ++ch) {
                     const int idx = sh_index(layout, M, k, ch);
-                    const float coef = row[idx];
-                    const float sdl = sh_sign(flip, k, dl[ch]);      // the term's sign rides on dL/dcolour
-                    const float val = Y * sdl;
+                    const float val = Y * sh_sign(flip, k, dl[ch]);  // the term's sign rides on dL/dcolour
                     grow[idx] = first ? val : grow[idx] + val;
-                    const float cd = coef * sdl;
-                    dLda += Ya * cd; dLdb += Yb * cd; dLdc += Yc * cd;
                 }
             });
-            const float3 dLd = sh_grad_unpermute(d.sh_basis, dLda, dLdb, dLdc);
+            const float3 dLd = sh_direction_grad(geo.sh_jac + 3 * vg, dl);
             const float dLdx = dLd.x, dLdy = dLd.y, dLdz = dLd.z;
             if (first) {
                 const int nb = (d.deg + 1) * (d.deg + 1);
@@ -366,11 +362,10 @@ k_preprocess_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, GaussGrads out, int
         }
     }
     if (M > 0) {
-        if (!sh_written)                   // on screen in no view: the row was neither fetched nor written
+        if (!sh_written)                   // on screen in no view: the row was not written
             for (int c = 0; c < sh_n; ++c) grow[c] = 0.0f;
         __syncwarp();
-        const float *gsrc = in_place ? wrows : wrows + (size_t)kPreBwdThreads * row_stride;
-        store_rows(out.d_sh + (size_t)sg0 * sh_n, rows, sh_n, gsrc, row_stride, lane);
+        unstage_sh_rows(wrows, out.d_sh + (size_t)sg0 * sh_n, rows, sh_n, row_stride, lane);
     }
 }
 
@@ -400,17 +395,16 @@ int launch_clear_pair_grads(const Dims &d, const Geom &g, const ViewGrads &vg, c
 // Camera-only backward (ps_raster_grads with every Gaussian gradient NULL): the 29 camera entries of k_preprocess_bwd's
 // CAM path, formed by the same functions, and nothing else.  One thread per (view, Gaussian) pair; a CTA covers kCamBwdThreads consecutive (scene,
 // Gaussian) indices of S*P for ONE view v (blockIdx.x = chunk * V + v: the V CTAs of a chunk run side by side and share
-// its SH rows in L2), so each warp stores exactly the partial rows k_preprocess_bwd<·, true> stores for (its 32
-// indices, v), summed in the same order, and the same k_camera_finish adds them.  It reads the scratch of the on-screen
-// pairs and the means, covariances and (for campos) SH rows of the on-screen lanes only; no Gaussian gradient is formed
-// or stored.  Walking the Gaussians, not the compact list of on-screen pairs (whose order changes from run to run),
+// its means and covariances in L2), so each warp stores exactly the partial rows k_preprocess_bwd<·, true> stores for
+// (its 32 indices, v), summed in the same order, and the same k_camera_finish adds them.  It reads the scratch, the
+// means, covariances and (for campos) the stored colour-direction Jacobian of the on-screen pairs only; no Gaussian
+// gradient is formed or stored.  Walking the Gaussians, not the compact list of on-screen pairs (whose order changes from run to run),
 // keeps every float sum in a fixed order.
 constexpr int kCamBwdThreads = 128;
 
 template <bool DEPTH>
 __global__ void __launch_bounds__(kCamBwdThreads, 4)
-k_camera_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, int row_stride, float *cam_ws) {
-    extern __shared__ float s_sh[];    // [warps][32][row_stride] SH coefficients of the on-screen lanes
+k_camera_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, float *cam_ws) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int v = (int)(blockIdx.x % (unsigned)d.V);
     const long long sp = (long long)d.S * d.P;
@@ -423,7 +417,6 @@ k_camera_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, int row_stride, float *
     const size_t sg = sgi;
     const int vid = (int)scene * d.V + v;
     const size_t vg = (size_t)vid * d.P + g;
-    const int M = d.M, sh_n = 3 * M;
 
     const bool vis = live && *geo.n_instances <= d.capacity && geo.radii[vg] > 0;
     const unsigned vis_lanes = __ballot_sync(0xffffffffu, vis);
@@ -434,10 +427,6 @@ k_camera_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, int row_stride, float *
         store_cam_partials(cam, cam_ws, d, v, sg0, rows, scene, lane);
         return;
     }
-    float *wrows = s_sh + (size_t)warp * 32 * row_stride;
-    const float *row = wrows + lane * row_stride;
-    if (M > 0) gather_rows_async(in.sh, (unsigned long long)sg, vis_lanes, sh_n, wrows, row_stride, lane);
-
     float mx0 = 0.0f, my0 = 0.0f, mz0 = 0.0f;
     const float sc = in.scale ? in.scale[vid] : 1.0f;
     if (vis) {
@@ -456,8 +445,7 @@ k_camera_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, int row_stride, float *
         const PairGrad q = projection_bwd<false>(cv, s6, sc, vm, pm, focal_x, focal_y, px, py, pz, gc, g2, nullptr);
         camera_geometry_grads(q, cv, px, py, pz, g2, focal_x, focal_y, tanfovx, tanfovy, cam);
     }
-    if (M > 0) gather_rows_wait();         // warp-uniform
-    if (M > 0 && vis) {
+    if (d.M > 0 && vis) {
         // campos: minus the gradient of the view direction p - campos through the SH evaluation
         const float px = mx0 * sc, py = my0 * sc, pz = mz0 * sc;
         const float4 gcol = vgr.d_color[vg];
@@ -465,21 +453,9 @@ k_camera_bwd(Dims d, Inputs in, Geom geo, ViewGrads vgr, int row_stride, float *
         const float ddx = px - cx, ddy = py - cy, ddz = pz - cz;
         const float len2 = ddx * ddx + ddy * ddy + ddz * ddz;
         const float len = sqrtf(len2);
-        const float x = ddx / len, y = ddy / len, z = ddz / len;
         const uint8_t cl = geo.clamped[vg];
         const float dl[3] = {(cl & 1) ? 0.0f : gcol.x, (cl & 2) ? 0.0f : gcol.y, (cl & 4) ? 0.0f : gcol.z};
-        float dLda = 0.0f, dLdb = 0.0f, dLdc = 0.0f;
-        const float3 sa = sh_arg(d.sh_basis, x, y, z);
-        const uint32_t flip = sh_flip_mask(d.sh_basis);
-        const int layout = d.sh_layout;
-        sh_for_each(d.deg, sa.x, sa.y, sa.z, [&](int k, float Y, float Ya, float Yb, float Yc) {
-#pragma unroll
-            for (int ch = 0; ch < 3; ++ch) {
-                const float cd = row[sh_index(layout, M, k, ch)] * sh_sign(flip, k, dl[ch]);
-                dLda += Ya * cd; dLdb += Yb * cd; dLdc += Yc * cd;
-            }
-        });
-        const float3 dLd = sh_grad_unpermute(d.sh_basis, dLda, dLdb, dLdc);
+        const float3 dLd = sh_direction_grad(geo.sh_jac + 3 * vg, dl);
         const float inv3 = 1.0f / (len2 * len);
         camera_campos_grads(ddx, ddy, ddz, len2, inv3, dLd, cam);
     }
@@ -543,44 +519,30 @@ __global__ void __launch_bounds__(kCamFinishThreads) k_camera_finish(Dims d, flo
     if (t < 2 && cg.d_tanfov) cg.d_tanfov[2 * vid + t] = part[0][27 + t];
 }
 
-template <bool DEPTH, bool CAM>
-static int launch_preprocess_bwd_kernel(unsigned blocks, size_t smem, const Dims &d, const Inputs &in, const Geom &g,
-                                        const ViewGrads &vg, const GaussGrads &out, int row_stride, float *cam_ws,
-                                        cudaStream_t st) {
-    static unsigned long long attr_devices = 0;
-    if (first_use_on_device(attr_devices))
-        PS_CUDA_CHECK(cudaFuncSetAttribute(k_preprocess_bwd<DEPTH, CAM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           96 * 1024));
-    k_preprocess_bwd<DEPTH, CAM><<<blocks, kPreBwdThreads, smem, st>>>(d, in, g, vg, out, row_stride, cam_ws);
-    PS_LAUNCH_CHECK("k_preprocess_bwd");
-    return PS_OK;
-}
-
 int launch_preprocess_backward(const Dims &d, const Inputs &in, const Geom &g, const ViewGrads &vg,
                                const ps_raster_grads &grads, cudaStream_t st) {
     const int row_stride = d.M > 0 ? ((3 * d.M) | 1) : 1;   // odd word count: conflict-free per-lane rows
-    const size_t smem = d.M > 0 ? sizeof(float) * kPreBwdThreads * row_stride * (d.V == 1 ? 1 : 2) : 0;
+    // at most 38.4 KB (M <= 25): within the default dynamic shared memory limit
+    const size_t smem = d.M > 0 ? sizeof(float) * kPreBwdThreads * row_stride : 0;
     const long long sp = (long long)d.S * d.P;
     const unsigned blocks = (unsigned)((sp + kPreBwdThreads - 1) / kPreBwdThreads);
     const GaussGrads out{grads.d_means, grads.d_cov, grads.d_opacities, grads.d_sh, grads.d_means2d};
     const ps_raster_camera_grads *cg = grads.camera;
     float *ws = cg ? static_cast<float *>(cg->workspace) : nullptr;
-    int rc = PS_OK;
     if (!grads.d_means) {               // camera-only backward (the caller checked that cg is set)
         const unsigned cam_blocks = (unsigned)((sp + kCamBwdThreads - 1) / kCamBwdThreads) * (unsigned)d.V;
-        const size_t cam_smem = d.M > 0 ? sizeof(float) * kCamBwdThreads * row_stride : 0;
         if (d.depth_mode)
-            k_camera_bwd<true><<<cam_blocks, kCamBwdThreads, cam_smem, st>>>(d, in, g, vg, row_stride, ws);
+            k_camera_bwd<true><<<cam_blocks, kCamBwdThreads, 0, st>>>(d, in, g, vg, ws);
         else
-            k_camera_bwd<false><<<cam_blocks, kCamBwdThreads, cam_smem, st>>>(d, in, g, vg, row_stride, ws);
+            k_camera_bwd<false><<<cam_blocks, kCamBwdThreads, 0, st>>>(d, in, g, vg, ws);
         PS_LAUNCH_CHECK("k_camera_bwd");
-    } else if (d.depth_mode)
-        rc = cg ? launch_preprocess_bwd_kernel<true, true>(blocks, smem, d, in, g, vg, out, row_stride, ws, st)
-                : launch_preprocess_bwd_kernel<true, false>(blocks, smem, d, in, g, vg, out, row_stride, ws, st);
-    else
-        rc = cg ? launch_preprocess_bwd_kernel<false, true>(blocks, smem, d, in, g, vg, out, row_stride, ws, st)
-                : launch_preprocess_bwd_kernel<false, false>(blocks, smem, d, in, g, vg, out, row_stride, ws, st);
-    if (rc || !cg) return rc;
+    } else {
+        const auto kern = d.depth_mode ? (cg ? k_preprocess_bwd<true, true> : k_preprocess_bwd<true, false>)
+                                       : (cg ? k_preprocess_bwd<false, true> : k_preprocess_bwd<false, false>);
+        kern<<<blocks, kPreBwdThreads, smem, st>>>(d, in, g, vg, out, row_stride, ws);
+        PS_LAUNCH_CHECK("k_preprocess_bwd");
+    }
+    if (!cg) return PS_OK;
     const dim3 finish_grid((unsigned)((cam_rows_per_view(d.P) + kCamFinishRows - 1) / kCamFinishRows),
                            (unsigned)(d.S * d.V));
     k_camera_finish<<<finish_grid, kCamFinishThreads, 0, st>>>(d, ws, *cg);

@@ -189,6 +189,10 @@ class RasterOutputState:
             if d.depth_mode else None,
             run_depth=view(self.image, lay.run_depth, torch.float32, vt * 3 * hw, (vt, 3, d.height, d.width))
             if d.depth_mode else None,
+            # per on-screen pair: d(colour channel before the clamp) / d(normalised view direction), rows (x, y, z)
+            # (None with precomputed colours)
+            sh_jacobian=view(self.geom, lay.sh_jacobian, torch.float32, vp * 12, (vt, P, 3, 4))[..., :3]
+            if d.sh_coeffs else None,
             num_instances=n,
         )
 
